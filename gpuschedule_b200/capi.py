@@ -67,6 +67,17 @@ class GsResultLayout(C.Structure):
                 ("cap_ev", C.c_int64), ("cap_q", C.c_int64), ("cap_nodeev", C.c_int64), ("cap_spans", C.c_int64), ("n", C.c_int64), ("span_bytes", C.c_int64)]
 
 
+# gs_summary (include/gsched.h): one replica's run reduced to what the notebooks compute from cluster.csv / job.csv
+SUMMARY_DTYPE = np.dtype([("n", "<i8"), ("rows", "<i8"), ("done", "<i4"), ("status", "<i4"), ("makespan", "<i8"),
+                          ("busy_gpus_sum", "<i8"), ("running_sum", "<i8"), ("queued_sum", "<i8"),
+                          ("busy_gpus_max", "<i4"), ("running_max", "<i4"), ("queued_max", "<i4"), ("pend_max_max", "<i4"),
+                          ("pend_sum_lo", "<u8"), ("pend_sum_hi", "<u8"), ("mem_busy_lo", "<u8"), ("mem_busy_hi", "<u8"),
+                          ("pending_rows", "<i8"), ("avg_pending_sum", "<f8"), ("util_sum", "<f8"), ("finished", "<i8"),
+                          ("wait_sum", "<i8"), ("turnaround_sum", "<i8"), ("jct_sum", "<i8"), ("preempt_sum", "<i8"),
+                          ("gpu_ticks_sum", "<i8"), ("wait_q", "<i4", (5,)), ("turnaround_q", "<i4", (5,)), ("jct_q", "<i4", (5,)),
+                          ("reserved", "<i4", (5,))])
+assert SUMMARY_DTYPE.itemsize == 256
+
 JOBIN_DTYPE = np.dtype([("arrive_tick", "<i4"), ("gpus", "<i4"), ("gpu_per_task", "<i4"), ("ps_count", "<i4"),
                         ("mem_bytes", "<i8"), ("duration", "<f8")])
 NODE_DTYPE = np.dtype([("busy_mask", "<u8"), ("cpu_used", "<i4"), ("mem_used", "<i4")])
@@ -165,7 +176,8 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_last_error.argtypes = [C.c_void_p]
     lib.gs_horus_last_error.restype = C.c_char_p
     lib.gs_horus_build_tag.restype = C.c_char_p
-    for name in ("gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
+    lib.gs_horus_summarize.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, f64p]
+    for name in ("gs_horus_summarize", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
                  "gs_horus_run", "gs_horus_stats", "gs_horus_fetch"):
         getattr(lib, name).restype = C.c_int
     return lib
@@ -222,7 +234,8 @@ def load_library():
     lib.gs_load_traces_packed.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, i64p]
     lib.gs_result_layout.argtypes = [C.c_void_p, C.c_int, C.POINTER(GsResultLayout)]
     lib.gs_fetch_results.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
-    for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results"):
+    lib.gs_summarize.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, f64p]
+    for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize"):
         getattr(lib, name).restype = C.c_int
     lib.gs_switch_yarn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, f64p, C.c_int64,
                                    C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_int64]
@@ -434,6 +447,16 @@ class HorusEngine:
                                             _ptr(order, C.c_int32), C.byref(nr), C.byref(nf)), "gs_horus_fetch")
         return rows[:nr.value], util[:nr.value], flags[:nr.value], recs[:n], order[:nf.value]
 
+    def summarize(self, first=0, count=None, with_time=False):
+        """SUMMARY_DTYPE records of replicas [first, first+count) over every row they hold (include/gsched_horus.h);
+        with_time: (records, kernel milliseconds)"""
+        count = self.nsims - first if count is None else int(count)
+        out = np.zeros(max(count, 1), dtype=SUMMARY_DTYPE)
+        ms = C.c_double(0.0)
+        self._check(self.lib.gs_horus_summarize(self.h, int(first), count, out.ctypes.data_as(C.c_void_p), C.byref(ms)),
+                    "gs_horus_summarize")
+        return (out[:count], ms.value) if with_time else out[:count]
+
 
 class Engine:
     """One handle == `nsims` independent replicas on one CUDA device."""
@@ -453,7 +476,7 @@ class Engine:
     def _check(self, rc, what):
         if rc != 0:
             msg = self.lib.gs_last_error(self.h)
-            raise GsError(f"{what} failed ({rc}): {msg.decode() if msg else ''}")
+            raise GsError(f"{what} failed ({rc}): {msg.decode() if msg else ''}", rc)
 
     def close(self):
         if getattr(self, "h", None) and self.h.value:
@@ -678,6 +701,25 @@ class Engine:
         if not collect_rows:
             return None
         return [np.concatenate(p) if p else np.empty(0, dtype=ROW_DTYPE) for p in parts]
+
+    def summarize(self, first=0, count=None, with_time=False):
+        """SUMMARY_DTYPE records of replicas [first, first+count): folds the rows of the last window not folded yet,
+        recomputes the job part (include/gsched.h: gs_summarize).  Call it after every run() of a multi-window run.
+        with_time: (records, kernel milliseconds)"""
+        count = self.nsims - first if count is None else int(count)
+        out = np.zeros(max(count, 1), dtype=SUMMARY_DTYPE)
+        ms = C.c_double(0.0)
+        self._check(self.lib.gs_summarize(self.h, int(first), count, out.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_summarize")
+        return (out[:count], ms.value) if with_time else out[:count]
+
+    def run_summarized(self, rows_cap=0):
+        """Run every replica to its exit condition, summarising after every launch and fetching no rows; returns
+        the final SUMMARY_DTYPE records of all replicas."""
+        while True:
+            self.run(0, rows_cap)
+            out = self.summarize()
+            if out["done"].all():
+                return out
 
     def stats(self, sim=0) -> GsRunStats:
         st = GsRunStats()

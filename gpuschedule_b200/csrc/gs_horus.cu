@@ -9,6 +9,7 @@
 #define GS_HD __host__ __device__ __forceinline__
 #include "gs_horus_core.cuh"
 #include "gs_horus_host.h"
+#include "gs_summary.cuh"
 
 #ifdef __CUDACC__
 // lanes = simulations per warp: 32 (every lane drives one) or 1 (lane 0 only: no divergence inside the warp,
@@ -47,6 +48,33 @@ __global__ void __launch_bounds__(32) gs_horus_coop_kernel(HSim *sims, int nsims
   if (lane == 0) { h_write_records(s); sims[b] = s; }
 }
 
+// gs_horus_summarize: every row the replica holds, [0, ticks), one block per replica (gs_summary.cuh).
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_hsum_rows_kernel(const HSim *sims, int first, gs_summary *acc) {
+  const int r = first + blockIdx.x;
+  const HSim &S = sims[r];
+  GsSumPart p;
+  gs_sum_zero(p);
+  for (long long i = threadIdx.x; i < S.ticks; i += blockDim.x) gs_sum_row(p, S.rows[i], S.util[i]);
+  gs_sum_block_reduce(p);
+  if (threadIdx.x == 0) {
+    gs_summary &A = acc[r];
+    A.n = S.n; A.done = S.done; A.status = S.status;
+    gs_sum_add_rows(A, p);
+    if (S.ticks > 0) A.makespan = S.rows[S.ticks - 1].now;
+  }
+}
+
+struct GsSumHorusJobs {
+  const HSim *sims;
+  __device__ long long finished(int r) const { return sims[r].nfin; }
+  __device__ GsSumJob job(int r, long long i) const {
+    const HSim &S = sims[r];
+    const int j = S.fin[i];
+    const gs_horus_job_rec rec = S.recs[j];
+    return gs_sum_job(S.jobs[j].arrive, rec.start, rec.end, rec.jct, rec.preempt, S.jobs[j].gpus);
+  }
+};
+
 #endif  // __CUDACC__
 
 namespace {
@@ -80,6 +108,8 @@ struct gs_horus_handle_s {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   float last_ms = 0.f;
   long long launches = 0;
+  gs_summary *d_sum = nullptr;      // gs_horus_summarize: one record per replica
+  int *d_sum_scratch = nullptr; size_t sum_scratch_bytes = 0;
   std::string err;
   std::vector<double> shared;       // one stream consumed by every replica that did not get its own
   double *d_shared = nullptr; size_t shared_cap = 0; bool shared_dirty = false;
@@ -126,6 +156,8 @@ extern "C" int gs_horus_destroy(gs_horus_handle h) {
   if (h->d_shared) cudaFree(h->d_shared);
   if (h->shared_ws.dev) cudaFree(h->shared_ws.dev);
   if (h->d_sims) cudaFree(h->d_sims);
+  if (h->d_sum) cudaFree(h->d_sum);
+  if (h->d_sum_scratch) cudaFree(h->d_sum_scratch);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -402,5 +434,68 @@ extern "C" int gs_horus_fetch(gs_horus_handle h, int32_t sim, gs_tick_row *rows,
   HCU(cudaStreamSynchronize(h->stream));
   if (n_rows) *n_rows = D.ticks;
   if (n_finished) *n_finished = D.nfin;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t count, gs_summary *out, double *kernel_ms) {
+  if (!h) return GS_ERR_ARG;
+  const int nsims = (int)h->sims.size();
+  if (first < 0 || count < 0 || first > nsims - count || (count > 0 && !out)) return hfail(h, GS_ERR_ARG, "gs_horus_summarize: bad arguments");
+  if (kernel_ms) *kernel_ms = 0.0;
+  if (count == 0) return GS_OK;
+  long long kmax = 1;
+  for (int i = first; i < first + count; ++i) {
+    if (!h->sims[(size_t)i].prepared) return hfail(h, GS_ERR_STATE, "gs_horus_summarize: a replica has not run yet");
+    kmax = std::max(kmax, (long long)h->sims[(size_t)i].dev.nfin);
+  }
+  HCU(cudaSetDevice(h->device));
+  if (!h->d_sum) HCU(cudaMalloc(&h->d_sum, sizeof(gs_summary) * (size_t)nsims));
+  HCU(cudaMemsetAsync(h->d_sum + first, 0, sizeof(gs_summary) * (size_t)count, h->stream));
+#ifdef __CUDACC__
+  int per_sm = 1, sms = 132;
+  HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_sum_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+  const int grid = std::min(count, std::max(1, per_sm) * sms);
+  const size_t pitch = (size_t)(kmax + 63) / 64 * 64, need = 3 * sizeof(int) * pitch * (size_t)grid;
+  if (h->sum_scratch_bytes < need) {
+    if (h->d_sum_scratch) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_sum_scratch); }
+    h->d_sum_scratch = nullptr; h->sum_scratch_bytes = 0;
+    HCU(cudaMalloc(&h->d_sum_scratch, need));
+    h->sum_scratch_bytes = need;
+  }
+  HCU(cudaEventRecord(h->ev0, h->stream));
+  gs_hsum_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->d_sum);
+  HCU(cudaGetLastError());
+  gs_sum_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->d_sum,
+                                                                                      h->d_sum_scratch, (long long)pitch);
+  HCU(cudaGetLastError());
+  h->launches += 2;
+  HCU(cudaEventRecord(h->ev1, h->stream));
+#else   // host build for tests/emu: the same folds, one replica after the other
+  for (int r = first; r < first + count; ++r) {
+    const HSim &S = h->d_sims[r];
+    gs_summary &A = h->d_sum[r];
+    GsSumPart p;
+    gs_sum_zero(p);
+    for (long long i = 0; i < S.ticks; ++i) gs_sum_row(p, S.rows[i], S.util[i]);
+    A.n = S.n; A.done = S.done; A.status = S.status;
+    gs_sum_add_rows(A, p);
+    if (S.ticks > 0) A.makespan = S.rows[S.ticks - 1].now;
+    std::vector<GsSumJob> jobs((size_t)S.nfin);
+    for (int i = 0; i < S.nfin; ++i) {
+      const int j = S.fin[i];
+      jobs[(size_t)i] = gs_sum_job(S.jobs[j].arrive, S.recs[j].start, S.recs[j].end, S.recs[j].jct, S.recs[j].preempt, S.jobs[j].gpus);
+    }
+    gs_sum_jobs_serial(jobs.data(), S.nfin, A);
+  }
+  (void)kmax;
+#endif
+  HCU(cudaMemcpyAsync(out, h->d_sum + first, sizeof(gs_summary) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
+#ifdef __CUDACC__
+  float ms = 0.f;
+  HCU(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+  if (kernel_ms) *kernel_ms = ms;
+#endif
   return GS_OK;
 }

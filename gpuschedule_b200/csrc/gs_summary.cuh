@@ -1,0 +1,391 @@
+// gs_summary.cuh -- on-device run summaries (gs_summary, include/gsched.h), included by gsched.cu and gs_horus.cu.
+//
+// A replica's run is reduced to the few numbers the reference's notebooks compute from its cluster.csv / job.csv.
+// Two parts:
+//   * rows: one block per replica folds gs_tick_rows (event-driven policies, horus) or, for fifo, the compact
+//     records directly -- record k stands for the rows now_k .. now_(k+1) - 1, on which only `delta` and the pending
+//     terms move, linearly (gs_expand_rows_kernel), so each record is folded in closed form and no row is rebuilt;
+//   * jobs: the three per-job values (wait, turnaround, jct) of every finished job are written once to scratch, and
+//     a block-wide radix select over 9-bit digits finds the 15 order statistics (3 values x 5 ranks) in the same
+//     passes: ceil(bits / 9) passes, where bits is the width of the largest value range (about 18 on the BASELINE
+//     trace: two passes).
+// The per-row arithmetic, the record fold and the rank / digit arithmetic are __host__ __device__ functions: the
+// host-emulation build of gs_horus.cu (tests/emu) runs them on the CPU, and so can a CPU test.
+#pragma once
+
+#include <math.h>
+#include <stdint.h>
+
+#include "gsched.h"
+
+#ifndef __CUDACC__
+#ifndef __host__
+#define __host__
+#endif
+#ifndef __device__
+#define __device__
+#endif
+#endif
+
+#define GS_SUM_HD static __host__ __device__ inline
+#define GS_SUM_THREADS 256
+#define GS_SUM_BINS 512            // 9-bit digits
+#define GS_SUM_TARGETS 15          // {wait, turnaround, jct} x {50, 90, 95, 99, 100 %}
+
+static_assert(sizeof(gs_summary) == 256, "gs_summary is 256 bytes");
+
+typedef __int128 gs_i128;
+typedef unsigned __int128 gs_u128;
+
+// Partial fold of some rows (one thread's share, then block-reduced).
+struct GsSumPart {
+  long long rows, busy, running, queued, pending_rows;
+  int busy_max, running_max, queued_max, pend_max;
+  gs_i128 pend, mem;
+  double avg, util;
+};
+
+GS_SUM_HD void gs_sum_zero(GsSumPart &p) {
+  p.rows = p.busy = p.running = p.queued = p.pending_rows = 0;
+  p.busy_max = p.running_max = p.queued_max = p.pend_max = 0;
+  p.pend = 0; p.mem = 0; p.avg = 0.0; p.util = 0.0;
+}
+
+GS_SUM_HD int gs_sum_imax(int a, int b) { return a > b ? a : b; }
+
+GS_SUM_HD double gs_sum_i128_to_double(gs_i128 x) {
+  const long long lo = (long long)x;
+  if ((gs_i128)lo == x) return (double)lo;
+  return (double)(long long)(x >> 64) * 18446744073709551616.0 + (double)(unsigned long long)x;
+}
+
+// One cluster.csv row.  `util`: the sampled avg_gpu_utilization value (horus), NaN counted as 0; 0 when there is none.
+GS_SUM_HD void gs_sum_row(GsSumPart &p, const gs_tick_row &r, double util) {
+  p.rows += 1;
+  p.busy += r.busy_gpus; p.running += r.running; p.queued += r.queued;
+  p.busy_max = gs_sum_imax(p.busy_max, r.busy_gpus); p.running_max = gs_sum_imax(p.running_max, r.running);
+  p.queued_max = gs_sum_imax(p.queued_max, r.queued); p.pend_max = gs_sum_imax(p.pend_max, r.pend_max);
+  p.pend += (gs_i128)r.pend_sum; p.mem += (gs_i128)r.mem_busy_bytes;
+  if (r.queued > 0 && r.pend_sum != 0) {      // avg_pending_time != 0 (log_manager.pending_columns)
+    p.pending_rows += 1;
+    p.avg += (double)r.pend_sum / ((double)r.queued + 1e-9);
+  }
+  if (util == util) p.util += util;
+}
+
+// The rows v_lo .. v_hi (values of `delta`) of one fifo record: every counter is constant there, and the pending sum of
+// row v is queued * v - arrive_sum (q = the same-tick gs_qrow; arrive_sum / oldest are unused when queued == 0).
+// avg_pending_sum: the denominator queued + 1e-9 is constant within the record, so the record adds
+// (sum of its nonzero pending sums) / (queued + 1e-9).
+GS_SUM_HD void gs_sum_record(GsSumPart &p, const gs_evrow &e, long long arrive_sum, int oldest, long long v_lo, long long v_hi) {
+  const long long L = v_hi - v_lo + 1;
+  if (L <= 0) return;
+  p.rows += L;
+  p.busy += (long long)e.busy_gpus * L; p.running += (long long)e.running * L; p.queued += (long long)e.queued * L;
+  p.busy_max = gs_sum_imax(p.busy_max, e.busy_gpus); p.running_max = gs_sum_imax(p.running_max, e.running);
+  p.queued_max = gs_sum_imax(p.queued_max, e.queued);
+  p.mem += (gs_i128)e.mem_busy_bytes * L;
+  if (e.queued > 0) {
+    const long long q = e.queued;
+    const long long sv = (v_lo + v_hi) * L / 2;                     // sum of v over the record (exact: (v_lo + v_hi) * L is even)
+    const gs_i128 x = (gs_i128)q * sv - (gs_i128)L * arrive_sum;
+    p.pend += x;
+    p.pend_max = gs_sum_imax(p.pend_max, (int)(v_hi - oldest));
+    // q * v - arrive_sum grows with v: it is zero on at most one row, v = arrive_sum / q
+    const bool zero = arrive_sum % q == 0 && arrive_sum / q >= v_lo && arrive_sum / q <= v_hi;
+    const long long nz = L - (zero ? 1 : 0);
+    p.pending_rows += nz;
+    if (nz > 0) p.avg += gs_sum_i128_to_double(x) / ((double)q + 1e-9);
+  }
+}
+
+GS_SUM_HD void gs_sum_merge(GsSumPart &a, const GsSumPart &b) {
+  a.rows += b.rows; a.busy += b.busy; a.running += b.running; a.queued += b.queued; a.pending_rows += b.pending_rows;
+  a.busy_max = gs_sum_imax(a.busy_max, b.busy_max); a.running_max = gs_sum_imax(a.running_max, b.running_max);
+  a.queued_max = gs_sum_imax(a.queued_max, b.queued_max); a.pend_max = gs_sum_imax(a.pend_max, b.pend_max);
+  a.pend += b.pend; a.mem += b.mem; a.avg += b.avg; a.util += b.util;
+}
+
+GS_SUM_HD void gs_sum_add128(uint64_t &lo, uint64_t &hi, gs_i128 v) {
+  const gs_u128 s = (((gs_u128)hi << 64) | (gs_u128)lo) + (gs_u128)v;
+  lo = (uint64_t)s; hi = (uint64_t)(s >> 64);
+}
+
+// Add a fold to a summary's row part (rows, sums, maxima; makespan is set by the caller).
+GS_SUM_HD void gs_sum_add_rows(gs_summary &s, const GsSumPart &p) {
+  s.rows += p.rows;
+  s.busy_gpus_sum += p.busy; s.running_sum += p.running; s.queued_sum += p.queued;
+  s.busy_gpus_max = gs_sum_imax(s.busy_gpus_max, p.busy_max); s.running_max = gs_sum_imax(s.running_max, p.running_max);
+  s.queued_max = gs_sum_imax(s.queued_max, p.queued_max); s.pend_max_max = gs_sum_imax(s.pend_max_max, p.pend_max);
+  gs_sum_add128(s.pend_sum_lo, s.pend_sum_hi, p.pend);
+  gs_sum_add128(s.mem_busy_lo, s.mem_busy_hi, p.mem);
+  s.pending_rows += p.pending_rows; s.avg_pending_sum += p.avg; s.util_sum += p.util;
+}
+
+// ---- jobs
+struct GsSumJob { int wait, turn, jct, preempt, gpus; };
+
+GS_SUM_HD GsSumJob gs_sum_job(int arrive, int start, int end, int jct, int preempt, int gpus) {
+  GsSumJob v; v.wait = start - arrive; v.turn = end - arrive; v.jct = jct; v.preempt = preempt; v.gpus = gpus;
+  return v;
+}
+
+// fifo's run length, max(1, ceil(duration)) ticks (quirk Q11; need_of in gs_tick2.cuh)
+GS_SUM_HD int gs_sum_run_length(double dur) {
+  const double c = ceil(dur);
+  return c < 1.0 ? 1 : (c > 1.0e9 ? 0x7fffffff : (int)c);
+}
+
+GS_SUM_HD int gs_sum_permille(int t) { return t == 0 ? 500 : t == 1 ? 900 : t == 2 ? 950 : t == 3 ? 990 : 1000; }
+
+// Nearest rank: of k > 0 values sorted ascending, rank q per mille is element ceil(q * k / 1000) - 1.
+GS_SUM_HD long long gs_sum_rank(int permille, long long k) { return (permille * k + 999) / 1000 - 1; }
+
+// Radix passes over 9-bit digits needed for values whose range (max - min) is `span`.
+GS_SUM_HD int gs_sum_passes(unsigned long long span) {
+  int bits = 1;
+  while (bits < 64 && (span >> bits) != 0) ++bits;
+  return (bits + 8) / 9;
+}
+
+// One radix step: the digit whose bin holds element `rank` of the group the histogram counts; rank becomes the
+// element's rank inside that bin.
+GS_SUM_HD unsigned gs_sum_pick(const unsigned *hist, long long &rank) {
+  long long below = 0;
+  unsigned d = 0;
+  for (; d + 1 < GS_SUM_BINS; ++d) {
+    if (below + (long long)hist[d] > rank) break;
+    below += hist[d];
+  }
+  rank -= below;
+  return d;
+}
+
+#ifndef __CUDACC__
+// Host forms of the job part (the host-emulation build of gs_horus.cu, CPU tests): the same sums, and the same radix
+// select run serially, one target at a time.
+static inline void gs_sum_select_serial(const int *v, long long k, int out[5]) {
+  if (k == 0) { for (int t = 0; t < 5; ++t) out[t] = 0; return; }
+  int mn = v[0], mx = v[0];
+  for (long long i = 1; i < k; ++i) { mn = v[i] < mn ? v[i] : mn; mx = v[i] > mx ? v[i] : mx; }
+  const int passes = gs_sum_passes((unsigned long long)((long long)mx - mn));
+  unsigned hist[GS_SUM_BINS];
+  for (int t = 0; t < 5; ++t) {
+    long long rank = gs_sum_rank(gs_sum_permille(t), k);
+    unsigned long long prefix = 0;
+    for (int p = 0; p < passes; ++p) {
+      const int shift = (passes - 1 - p) * 9;
+      for (int b = 0; b < GS_SUM_BINS; ++b) hist[b] = 0;
+      for (long long i = 0; i < k; ++i) {
+        const unsigned long long u = (unsigned long long)((long long)v[i] - mn);
+        if ((u >> (shift + 9)) == prefix) hist[(u >> shift) & (GS_SUM_BINS - 1)] += 1;
+      }
+      prefix = (prefix << 9) | gs_sum_pick(hist, rank);
+    }
+    out[t] = (int)((long long)mn + (long long)prefix);
+  }
+}
+
+static inline void gs_sum_jobs_serial(const GsSumJob *jobs, long long k, gs_summary &s) {
+  s.finished = k;
+  s.wait_sum = s.turnaround_sum = s.jct_sum = s.preempt_sum = s.gpu_ticks_sum = 0;
+  int *vals = new int[(size_t)(3 * (k > 0 ? k : 1))];
+  for (long long i = 0; i < k; ++i) {
+    const GsSumJob &v = jobs[i];
+    s.wait_sum += v.wait; s.turnaround_sum += v.turn; s.jct_sum += v.jct; s.preempt_sum += v.preempt;
+    s.gpu_ticks_sum += (long long)v.gpus * v.jct;
+    vals[i] = v.wait; vals[k + i] = v.turn; vals[2 * k + i] = v.jct;
+  }
+  gs_sum_select_serial(vals, k, s.wait_q);
+  gs_sum_select_serial(vals + k, k, s.turnaround_q);
+  gs_sum_select_serial(vals + 2 * k, k, s.jct_q);
+  delete[] vals;
+}
+#endif
+
+#ifdef __CUDACC__
+namespace {
+
+__device__ __forceinline__ GsSumPart gs_sum_shfl_down(const GsSumPart &p, int o) {
+  GsSumPart q;
+  q.rows = __shfl_down_sync(0xffffffffu, p.rows, o); q.busy = __shfl_down_sync(0xffffffffu, p.busy, o);
+  q.running = __shfl_down_sync(0xffffffffu, p.running, o); q.queued = __shfl_down_sync(0xffffffffu, p.queued, o);
+  q.pending_rows = __shfl_down_sync(0xffffffffu, p.pending_rows, o);
+  q.busy_max = __shfl_down_sync(0xffffffffu, p.busy_max, o); q.running_max = __shfl_down_sync(0xffffffffu, p.running_max, o);
+  q.queued_max = __shfl_down_sync(0xffffffffu, p.queued_max, o); q.pend_max = __shfl_down_sync(0xffffffffu, p.pend_max, o);
+  const unsigned long long plo = __shfl_down_sync(0xffffffffu, (unsigned long long)p.pend, o);
+  const unsigned long long phi = __shfl_down_sync(0xffffffffu, (unsigned long long)((gs_u128)p.pend >> 64), o);
+  const unsigned long long mlo = __shfl_down_sync(0xffffffffu, (unsigned long long)p.mem, o);
+  const unsigned long long mhi = __shfl_down_sync(0xffffffffu, (unsigned long long)((gs_u128)p.mem >> 64), o);
+  q.pend = (gs_i128)(((gs_u128)phi << 64) | plo); q.mem = (gs_i128)(((gs_u128)mhi << 64) | mlo);
+  q.avg = __shfl_down_sync(0xffffffffu, p.avg, o); q.util = __shfl_down_sync(0xffffffffu, p.util, o);
+  return q;
+}
+
+// Block sum of the threads' folds: thread 0 returns with the total (warps merged in a fixed order: deterministic).
+__device__ void gs_sum_block_reduce(GsSumPart &p) {
+  __shared__ GsSumPart warp_part[GS_SUM_THREADS / 32];
+  for (int o = 16; o > 0; o >>= 1) { const GsSumPart q = gs_sum_shfl_down(p, o); gs_sum_merge(p, q); }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncthreads();                                          // warp_part may still be read by an earlier reduction
+  if (lane == 0) warp_part[warp] = p;
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) gs_sum_merge(p, warp_part[w]);
+}
+
+// fifo: fold the window's records (block-cooperative: every thread calls it).  Rows already folded (`delta` <= wm) are
+// skipped.  The gs_qrow of a record with a queue is found by counting such records (one gs_qrow each, in order);
+// a binary search by `now` checks and, should the streams not line up, finds it.
+__device__ void gs_sum_fold_records(GsSumPart &p, const gs_evrow *ev, int nev, const gs_qrow *qr, int nq, long long ticks,
+                                    long long wm) {
+  __shared__ int warp_cnt[GS_SUM_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  int qbase = 0;
+  for (int t0 = 0; t0 < nev; t0 += blockDim.x) {
+    const int k = t0 + threadIdx.x;
+    const bool in = k < nev;
+    gs_evrow e;
+    if (in) e = ev[k];
+    const bool hasq = in && e.queued > 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, hasq);
+    if (lane == 0) warp_cnt[warp] = __popc(bal);
+    __syncthreads();
+    int off = __popc(bal & ((1u << lane) - 1u)), total = 0;
+    for (int w = 0; w < nwarps; ++w) { const int c = warp_cnt[w]; off += w < warp ? c : 0; total += c; }
+    __syncthreads();
+    if (in) {
+      const long long t_first = e.now;
+      const long long t_last = k + 1 < nev ? (long long)ev[k + 1].now - 1 : ticks;
+      const long long v_lo = t_first > wm + 1 ? t_first : wm + 1;
+      if (t_last >= v_lo) {
+        long long arrive_sum = 0; int oldest = 0;
+        if (hasq) {
+          int qi = qbase + off;
+          if (qi >= nq || qr[qi].now != e.now) {
+            int lo = 0, hi = nq - 1;
+            while (lo < hi) { const int mid = (lo + hi) >> 1; if (qr[mid].now < e.now) lo = mid + 1; else hi = mid; }
+            qi = lo;
+          }
+          const gs_qrow b = qr[qi];
+          arrive_sum = b.arrive_sum; oldest = b.oldest_arrive;
+        }
+        gs_sum_record(p, e, arrive_sum, oldest, v_lo, t_last);
+      }
+    }
+    qbase += total;
+  }
+}
+
+// Block reduction of N 64-bit values: the first NSUM are summed, the next NMIN take the minimum, the rest the maximum;
+// every thread returns with the results.
+template <int N, int NSUM, int NMIN>
+__device__ __forceinline__ long long gs_sum_op(int e, long long a, long long b) {
+  return e < NSUM ? a + b : e < NSUM + NMIN ? (b < a ? b : a) : (b > a ? b : a);
+}
+template <int N, int NSUM, int NMIN>
+__device__ void gs_sum_block_vec(long long (&v)[N]) {
+  __shared__ long long sh[GS_SUM_THREADS / 32][N];
+  __shared__ long long res[N];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+#pragma unroll
+  for (int e = 0; e < N; ++e) {
+    for (int o = 16; o > 0; o >>= 1) {
+      v[e] = gs_sum_op<N, NSUM, NMIN>(e, v[e], __shfl_down_sync(0xffffffffu, v[e], o));
+    }
+    if (lane == 0) sh[warp][e] = v[e];
+  }
+  __syncthreads();
+  if (threadIdx.x < N) {
+    const int e = threadIdx.x;
+    long long a = sh[0][e];
+    for (int w = 1; w < nwarps; ++w) a = gs_sum_op<N, NSUM, NMIN>(e, a, sh[w][e]);
+    res[e] = a;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int e = 0; e < N; ++e) v[e] = res[e];
+  __syncthreads();
+}
+
+// Job part of replicas first .. first + count - 1, one block per replica in turn (grid-stride).  Src supplies
+// finished(r) and job(r, i), the i-th finished job in finish order.  scratch: 3 * pitch ints per block.
+template <class Src>
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_sum_jobs_kernel(Src src, int first, int count, gs_summary *acc,
+                                                                    int *scratch, long long pitch) {
+  __shared__ unsigned hist[GS_SUM_TARGETS * GS_SUM_BINS];
+  __shared__ unsigned long long prefix[GS_SUM_TARGETS];
+  __shared__ long long rank[GS_SUM_TARGETS];
+  __shared__ int leader[GS_SUM_TARGETS];
+  int *vals = scratch + (size_t)blockIdx.x * 3 * (size_t)pitch;
+  for (int b = blockIdx.x; b < count; b += gridDim.x) {
+    const int r = first + b;
+    const long long k = src.finished(r);
+    long long red[11] = {0, 0, 0, 0, 0, 0x7fffffff, 0x7fffffff, 0x7fffffff, -0x80000000ll, -0x80000000ll, -0x80000000ll};
+    for (long long i = threadIdx.x; i < k; i += blockDim.x) {
+      const GsSumJob v = src.job(r, i);
+      vals[i] = v.wait; vals[pitch + i] = v.turn; vals[2 * pitch + i] = v.jct;
+      red[0] += v.wait; red[1] += v.turn; red[2] += v.jct; red[3] += v.preempt; red[4] += (long long)v.gpus * v.jct;
+      red[5] = min(red[5], (long long)v.wait); red[6] = min(red[6], (long long)v.turn); red[7] = min(red[7], (long long)v.jct);
+      red[8] = max(red[8], (long long)v.wait); red[9] = max(red[9], (long long)v.turn); red[10] = max(red[10], (long long)v.jct);
+    }
+    gs_sum_block_vec<11, 5, 3>(red);                        // (its barriers also publish the scratch writes)
+    long long span = 0;
+#pragma unroll
+    for (int m = 0; m < 3; ++m) span = max(span, red[8 + m] - red[5 + m]);
+    const int passes = k > 0 ? gs_sum_passes((unsigned long long)span) : 0;
+    if (threadIdx.x < GS_SUM_TARGETS) {
+      prefix[threadIdx.x] = 0;
+      rank[threadIdx.x] = k > 0 ? gs_sum_rank(gs_sum_permille(threadIdx.x % 5), k) : 0;
+    }
+    for (int p = 0; p < passes; ++p) {
+      const int shift = (passes - 1 - p) * 9;
+      for (int i = threadIdx.x; i < GS_SUM_TARGETS * GS_SUM_BINS; i += blockDim.x) hist[i] = 0;
+      __syncthreads();
+      if (threadIdx.x < GS_SUM_TARGETS) {                  // targets of one value with the same prefix share a histogram
+        const int t = threadIdx.x, m0 = (t / 5) * 5;
+        int L = t;
+        for (int u = m0; u < t; ++u) if (prefix[u] == prefix[t]) { L = u; break; }
+        leader[t] = L;
+      }
+      __syncthreads();
+      for (long long i = threadIdx.x; i < k; i += blockDim.x) {
+#pragma unroll
+        for (int m = 0; m < 3; ++m) {
+          const unsigned long long u = (unsigned long long)((long long)vals[m * pitch + i] - red[5 + m]);
+          const unsigned long long hp = u >> (shift + 9);
+          const unsigned d = (unsigned)(u >> shift) & (GS_SUM_BINS - 1);
+          bool placed = false;
+#pragma unroll
+          for (int q = 0; q < 5; ++q) {
+            const int t = m * 5 + q;
+            if (!placed && leader[t] == t && prefix[t] == hp) { atomicAdd(&hist[t * GS_SUM_BINS + d], 1u); placed = true; }
+          }
+        }
+      }
+      __syncthreads();
+      if (threadIdx.x < GS_SUM_TARGETS) {
+        const int t = threadIdx.x;
+        long long rk = rank[t];
+        const unsigned d = gs_sum_pick(hist + leader[t] * GS_SUM_BINS, rk);
+        rank[t] = rk;
+        prefix[t] = (prefix[t] << 9) | d;
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+      gs_summary &A = acc[r];
+      A.finished = k;
+      A.wait_sum = red[0]; A.turnaround_sum = red[1]; A.jct_sum = red[2]; A.preempt_sum = red[3]; A.gpu_ticks_sum = red[4];
+      for (int t = 0; t < 5; ++t) {
+        A.wait_q[t] = k > 0 ? (int)(red[5] + (long long)prefix[t]) : 0;
+        A.turnaround_q[t] = k > 0 ? (int)(red[6] + (long long)prefix[5 + t]) : 0;
+        A.jct_q[t] = k > 0 ? (int)(red[7] + (long long)prefix[10 + t]) : 0;
+      }
+    }
+    __syncthreads();
+  }
+}
+
+}  // namespace
+#endif  // __CUDACC__

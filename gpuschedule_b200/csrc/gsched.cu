@@ -50,6 +50,7 @@
 #include "gs_policy.cuh"
 #include "gs_aux.cuh"
 #include "gs_switch.cuh"
+#include "gs_summary.cuh"
 
 // ------------------------------------------------------------------ host side
 
@@ -79,6 +80,8 @@ struct SimHost {
   int max_need = 1;
   unsigned char *state_ptr = nullptr;     // the replica's slab: inside the handle's arena or its own allocation (state_slab)
   bool trace_in_arena = false;
+  int64_t sum_rows = 0;                   // gs_summarize: rows folded into the replica's accumulator (its watermark)
+  bool sum_fresh = true;                  // the accumulator is to be zeroed before the next fold (the replica was prepared afresh)
   SimDev dev;
   SimLayout layout;
 };
@@ -112,6 +115,7 @@ struct gs_engine {
   int comm_min_runnable = 0x7fffffff;      // gs_comm_set_min_runnable: no exchange unless the caller asks for one (include/gsched.h)
   unsigned long long comm_epoch = 0, comm_epoch0 = 0;   // exchange counter: continues across runs / value at the last prepare
   bool dirty = true;       // host mirror of SimDev newer than device copy
+  gs_summary *d_sum = nullptr;   // gs_summarize: one accumulator per replica
 };
 
 static std::string g_create_err;
@@ -187,6 +191,7 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->tarena) cudaFree(h->tarena);
   if (h->h_stage) cudaFreeHost(h->h_stage);
   if (h->d_scratch) cudaFree(h->d_scratch);
+  if (h->d_sum) cudaFree(h->d_sum);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
   if (h->comm_buf) cudaFree(h->comm_buf);
   if (h->e0) cudaEventDestroy(h->e0);
@@ -514,6 +519,7 @@ static int bind_sim(gs_handle h, SimHost &s, const SimLayout &L, unsigned char *
   D.blocked = D.nev = D.nq = D.nne = 0;
   D.mem_busy = D.sum_arr = D.span_used = D.events = D.evals = D.started = D.ticks = D.row_first = 0;
   D.need_init = 1;
+  s.sum_rows = 0; s.sum_fresh = true;
   s.prepared = true;
   return GS_OK;
 }
@@ -1030,6 +1036,95 @@ extern "C" int gs_fetch_all(gs_handle h, int sim, int64_t first, int64_t count, 
   if (rc == GS_OK && (jobs_out || finish_order_out)) rc = gs_fetch_jobs(h, sim, jobs_out, finish_order_out);
   if (rc == GS_OK) rc = gs_fetch_spans(h, sim, span_off_out, spans_out, spans_cap, spans_used);
   return rc;
+}
+
+// ------------------------------------------------------------------ run summaries (gs_summary.cuh)
+// Rows of the last window not folded yet (`delta` above the accumulator's watermark), one block per replica.
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_sum_rows_kernel(const SimDev *sims, int first, gs_summary *acc) {
+  const int r = first + blockIdx.x;
+  const SimDev &S = sims[r];
+  gs_summary &A = acc[r];
+  const long long wm = A.rows;
+  const long long lo = wm > S.row_first ? wm : S.row_first, hi = S.ticks;
+  GsSumPart p;
+  gs_sum_zero(p);
+  if (S.policy == GS_SCHED_FIFO) gs_sum_fold_records(p, S.evrows, S.nev, S.qrows, S.nq, S.ticks, wm);
+  else
+    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) gs_sum_row(p, S.rows[i - S.row_first], 0.0);
+  gs_sum_block_reduce(p);
+  if (threadIdx.x == 0) {
+    A.n = S.n; A.done = S.done; A.status = S.status;
+    if (hi > lo) {
+      gs_sum_add_rows(A, p);
+      A.makespan = S.policy == GS_SCHED_FIFO ? hi : S.rows[hi - 1 - S.row_first].now;   // fifo: row i has delta i + 1
+    }
+    A.util_sum = __longlong_as_double(0x7ff8000000000000ll);    // sampled on the host after the run
+  }
+}
+
+// The finished jobs as job.csv prints them (gs_expand_jobs_kernel for fifo, the job records otherwise).
+struct GsSumEngineJobs {
+  const SimDev *sims;
+  __device__ long long finished(int r) const { return sims[r].finished; }
+  __device__ GsSumJob job(int r, long long i) const {
+    const SimDev &S = sims[r];
+    const int j = S.fin[i];
+    const JobIn jb = S.jobs[j];
+    if (S.policy == GS_SCHED_FIFO) {
+      const int st = S.jstart[j];
+      const double d = S.netcost ? S.dur2[j] : jb.dur;
+      const int need = gs_sum_run_length(d > jb.dur ? d : jb.dur);
+      return gs_sum_job(jb.arrive, st, st + need, need, 1, jb.gpus);
+    }
+    const gs_job_rec rec = S.rec[j];
+    return gs_sum_job(jb.arrive, rec.start, rec.end, rec.jct, rec.preempt, jb.gpus);
+  }
+};
+
+extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, double *kernel_ms) {
+  if (!h) return GS_ERR_ARG;
+  if (first < 0 || count < 0 || first + count > h->nsims || (count > 0 && !out)) return fail(h, GS_ERR_ARG, "gs_summarize: bad arguments");
+  if (count == 0) { if (kernel_ms) *kernel_ms = 0.0; return GS_OK; }
+  // every check before anything changes: a refused call leaves the accumulators as they were
+  int64_t kmax = 1;
+  for (int i = first; i < first + count; ++i) {
+    const SimHost &s = h->sims[(size_t)i];
+    if (!s.prepared) return fail(h, GS_ERR_STATE, "gs_summarize: a replica has not run yet");
+    if (s.sum_rows < s.dev.row_first)
+      return fail(h, GS_ERR_STATE, "gs_summarize: a replica ran a window that was not summarised (call gs_summarize after every gs_run)");
+    kmax = std::max(kmax, (int64_t)s.dev.finished);
+  }
+  CU(cudaSetDevice(h->device));
+  if (!h->d_sum) {
+    CU(cudaMalloc(&h->d_sum, sizeof(gs_summary) * (size_t)h->nsims));
+    CU(cudaMemset(h->d_sum, 0, sizeof(gs_summary) * (size_t)h->nsims));
+  }
+  int per_sm = 1, sms = 132;
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_sum_jobs_kernel<GsSumEngineJobs>, GS_SUM_THREADS, 0));
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+  const int grid = std::min(count, std::max(1, per_sm) * sms);
+  const size_t pitch = (size_t)align_up((size_t)kmax, 64);
+  int rc = ensure_scratch(h, 3 * sizeof(int) * pitch * (size_t)grid);
+  if (rc) return rc;
+  for (int i = first; i < first + count; ++i) {
+    SimHost &s = h->sims[(size_t)i];
+    if (s.sum_fresh) { CU(cudaMemsetAsync(h->d_sum + i, 0, sizeof(gs_summary), h->stream)); s.sum_fresh = false; }
+  }
+  CU(cudaEventRecord(h->e0, h->stream));
+  gs_sum_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->d_sum);
+  CU(cudaGetLastError());
+  GsSumEngineJobs src{h->d_sims};
+  gs_sum_jobs_kernel<GsSumEngineJobs><<<(unsigned)grid, GS_SUM_THREADS, 0, h->stream>>>(src, first, count, h->d_sum, (int *)h->d_scratch,
+                                                                                       (long long)pitch);
+  CU(cudaGetLastError());
+  h->launches += 2;
+  CU(cudaEventRecord(h->e1, h->stream));
+  CU(cudaMemcpyAsync(out, h->d_sum + first, sizeof(gs_summary) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  float ms = 0; cudaEventElapsedTime(&ms, h->e0, h->e1);
+  if (kernel_ms) *kernel_ms = ms;
+  for (int i = first; i < first + count; ++i) h->sims[(size_t)i].sum_rows = out[i - first].rows;
+  return GS_OK;
 }
 
 extern "C" int gs_place_batch(gs_handle h, const gs_cluster *cluster, const gs_node *nodes, int32_t m,

@@ -11,7 +11,7 @@ import types
 
 import numpy as np
 
-from . import capi, rngcol
+from . import capi, rngcol, summary
 from .infrastructure import Infrastructure
 from .jobs import JobQueueManager, JobsManager
 from .log_manager import LogManager
@@ -36,11 +36,8 @@ def _is_utilisation_aware(fl):
     return fl.scheme in Scheduler.UTILISATION_AWARE or fl.schedule in Scheduler.UTILISATION_AWARE
 
 
-def run_batched_horus(flag_sets, device=0, out_root="log", chunk=1 << 21, rows_cap=1 << 16):
-    """The horus / horus+ / gandiva configurations of a sweep as replicas of ONE gs_horus launch.  Every replica
-    owns a numpy RandomState (seeded with flags.seed when >= 0, fresh entropy otherwise -- the reference's repeats
-    are unseeded) whose stream it consumes exactly like the single-run path does with numpy's global one, so a
-    seeded replica writes the same bytes as `run_sim.py --seed s`.  Returns [(output_dir, stats)]."""
+def _horus_setup(flag_sets, chunk, rows_cap):
+    """per configuration: infrastructure, jobs, and the replica's own random stream (see run_batched_horus)"""
     sims = []
     for fl in flag_sets:
         infra = Infrastructure(fl)
@@ -49,33 +46,48 @@ def run_batched_horus(flag_sets, device=0, out_root="log", chunk=1 << 21, rows_c
         raw = fl.schedule == "horus+"
         draw = (lambda k, rs=rs: rs.randint(0, 2 ** 32, size=k, dtype=np.uint32)) if raw else (lambda k, rs=rs: rs.standard_normal(k))
         sims.append(dict(fl=fl, infra=infra, jm=jm, raw=raw, draw=draw, stream=draw(chunk), rows_cap=rows_cap))
+    return sims
+
+
+def _horus_run(eng, sims, rows_cap):
+    """configure, load and run every replica to the end; a replica that ran out of rows or of samples starts over
+    with twice the rows / a longer stream while the others keep their results"""
+    for i, sm in enumerate(sims):
+        fl = sm["fl"]
+        eng.config(i, sm["infra"].gs_cluster(), capi.make_horus_params(fl.scheme, fl.schedule, int(fl.num_buffer), int(fl.num_queue)))
+        eng.load_trace(i, sm["jm"].table)
+        (eng.load_words if sm["raw"] else eng.load_stream)(i, sm["stream"])
+    cap = rows_cap
+    while True:
+        for sm in sims:
+            sm["ran_cap"] = cap                           # the row window this launch really gives every replica
+        try:
+            eng.run(rows_cap=cap)
+            return
+        except capi.GsError as e:
+            if e.code != capi.GS_ERR_CAPACITY:
+                raise
+            for i, sm in enumerate(sims):                 # finished replicas keep their results; the short ones start over
+                st = eng.stats(i)
+                if st.status != capi.GS_ERR_CAPACITY:
+                    continue
+                if st.ticks < sm["ran_cap"]:              # ran out of samples: continue this replica's stream
+                    sm["stream"] = np.concatenate([sm["stream"], sm["draw"](len(sm["stream"]))])
+                else:                                     # ran out of rows
+                    sm["rows_cap"] = 2 * sm["ran_cap"]
+                (eng.load_words if sm["raw"] else eng.load_stream)(i, sm["stream"])
+            cap = max(sm["rows_cap"] for sm in sims)
+
+
+def run_batched_horus(flag_sets, device=0, out_root="log", chunk=1 << 21, rows_cap=1 << 16):
+    """The horus / horus+ / gandiva configurations of a sweep as replicas of ONE gs_horus launch.  Every replica
+    owns a numpy RandomState (seeded with flags.seed when >= 0, fresh entropy otherwise -- the reference's repeats
+    are unseeded) whose stream it consumes exactly like the single-run path does with numpy's global one, so a
+    seeded replica writes the same bytes as `run_sim.py --seed s`.  Returns [(output_dir, stats)]."""
+    sims = _horus_setup(flag_sets, chunk, rows_cap)
     results = []
     with capi.HorusEngine(device=device, nsims=len(sims)) as eng:
-        for i, sm in enumerate(sims):
-            fl = sm["fl"]
-            eng.config(i, sm["infra"].gs_cluster(), capi.make_horus_params(fl.scheme, fl.schedule, int(fl.num_buffer), int(fl.num_queue)))
-            eng.load_trace(i, sm["jm"].table)
-            (eng.load_words if sm["raw"] else eng.load_stream)(i, sm["stream"])
-        cap = rows_cap
-        while True:
-            for sm in sims:
-                sm["ran_cap"] = cap                       # the row window this launch really gives every replica
-            try:
-                eng.run(rows_cap=cap)
-                break
-            except capi.GsError as e:
-                if e.code != capi.GS_ERR_CAPACITY:
-                    raise
-                for i, sm in enumerate(sims):             # finished replicas keep their results; the short ones start over
-                    st = eng.stats(i)
-                    if st.status != capi.GS_ERR_CAPACITY:
-                        continue
-                    if st.ticks < sm["ran_cap"]:          # ran out of samples: continue this replica's stream
-                        sm["stream"] = np.concatenate([sm["stream"], sm["draw"](len(sm["stream"]))])
-                    else:                                 # ran out of rows
-                        sm["rows_cap"] = 2 * sm["ran_cap"]
-                    (eng.load_words if sm["raw"] else eng.load_stream)(i, sm["stream"])
-                cap = max(sm["rows_cap"] for sm in sims)
+        _horus_run(eng, sims, rows_cap)
         for i, sm in enumerate(sims):
             fl, infra, jm = sm["fl"], sm["infra"], sm["jm"]
             rows, util, flags_arr, recs, order = eng.fetch(i)
@@ -93,6 +105,23 @@ def run_batched_horus(flag_sets, device=0, out_root="log", chunk=1 << 21, rows_c
     return results
 
 
+def _plain_setup(flag_sets):
+    """per configuration of the fifo / event-driven engine: (flags, infrastructure, jobs, policy)"""
+    sims = []
+    for fl in flag_sets:
+        infra = Infrastructure(fl)
+        jm = JobsManager(fl, JobQueueManager(fl, fl.trace_file))
+        sched = Scheduler(infra, jm, None)
+        sims.append((fl, infra, jm, sched.make_policy(jm.table)))
+    return sims
+
+
+def _plain_load(eng, sims):
+    for i, (fl, infra, jm, pol) in enumerate(sims):
+        eng.config(i, infra.gs_cluster(), pol)
+        eng.load_trace(i, jm.table)
+
+
 def run_batched(flag_sets, device=0, out_root="log"):
     """Run every configuration of `flag_sets` (list of flags namespaces) as one replica each.
     Returns [(output_dir, stats)] in the order of `flag_sets`; the utilisation-aware configurations go through
@@ -107,17 +136,10 @@ def run_batched(flag_sets, device=0, out_root="log"):
             for idx, res in zip(plain, run_batched([flag_sets[i] for i in plain], device, out_root)):
                 out[idx] = res
         return out
-    sims = []
-    for fl in flag_sets:
-        infra = Infrastructure(fl)
-        jm = JobsManager(fl, JobQueueManager(fl, fl.trace_file))
-        sched = Scheduler(infra, jm, None)
-        sims.append((fl, infra, jm, sched.make_policy(jm.table)))
+    sims = _plain_setup(flag_sets)
     results = []
     with capi.Engine(device=device, nsims=len(sims)) as eng:
-        for i, (fl, infra, jm, pol) in enumerate(sims):
-            eng.config(i, infra.gs_cluster(), pol)
-            eng.load_trace(i, jm.table)
+        _plain_load(eng, sims)
         rows_all = eng.run_all()
         for i, (fl, infra, jm, pol) in enumerate(sims):
             recs, order = eng.fetch_jobs(i)
@@ -139,6 +161,41 @@ def run_batched(flag_sets, device=0, out_root="log"):
     return results
 
 
+def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16):
+    """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
+    same configurations and random streams as run_batched, but no row or job record is read back and nothing is
+    written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus."""
+    out = np.zeros(len(flag_sets), dtype=capi.SUMMARY_DTYPE)
+    aware = [i for i, fl in enumerate(flag_sets) if _is_utilisation_aware(fl)]
+    plain = [i for i in range(len(flag_sets)) if i not in set(aware)]
+    if aware:
+        sims = _horus_setup([flag_sets[i] for i in aware], chunk, rows_cap)
+        with capi.HorusEngine(device=device, nsims=len(sims)) as eng:
+            _horus_run(eng, sims, rows_cap)
+            out[aware] = eng.summarize()
+    if plain:
+        sims = _plain_setup([flag_sets[i] for i in plain])
+        with capi.Engine(device=device, nsims=len(sims)) as eng:
+            _plain_load(eng, sims)
+            out[plain] = eng.run_summarized()
+    return out
+
+
+SUMMARY_KEYS = ["trace", "scheme", "schedule", "num_buffer", "num_queue", "seed"]
+
+
+def write_summary_csv(path, flag_sets, records):
+    """one line per configuration: its flags (SUMMARY_KEYS), the summary fields and the derived numbers (summary.py)"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + summary.columns())
+        for fl, rec in zip(flag_sets, records):
+            cl = Infrastructure(fl).gs_cluster()
+            w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed]
+                       + summary.flat(rec, cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib))
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description="run a sweep of simulator configurations as one batched GPU launch")
     ap.add_argument("--trace", nargs="+", required=True, help="trace CSV file(s)")
@@ -150,6 +207,8 @@ def main(argv=None):
     ap.add_argument("--num_queue", type=int, default=4)
     ap.add_argument("--repeats", type=int, default=1)
     ap.add_argument("--seed", type=int, default=-1)
+    ap.add_argument("--summary", default=None, metavar="FILE",
+                    help="write one CSV line of run summary per configuration to FILE instead of the per-run logs")
     a = ap.parse_args(argv)
     sets = []
     for tr in a.trace:
@@ -161,6 +220,10 @@ def main(argv=None):
                                        num_node_p_switch=a.num_node_p_switch, num_queue=a.num_queue, num_buffer=a.num_buffer,
                                        log_path=os.path.join(f"batched_{tag}", f"{scheme}_{sc}"),
                                        seed=a.seed if a.seed < 0 else a.seed + rep))
+    if a.summary:
+        write_summary_csv(a.summary, sets, summarize_batched(sets))
+        print(f"{a.summary}: {len(sets)} configurations")
+        return
     for out_dir, st in run_batched(sets):
         print(f"{out_dir}: ticks={st.ticks} events={st.events} finished={st.finished}")
 

@@ -217,6 +217,38 @@ typedef struct gs_jobin {
   double duration;        /* minutes * scale_factor                              */
 } gs_jobin;
 
+/* One replica's run reduced to the numbers the reference's notebooks compute from its cluster.csv and job.csv
+ * (makespan, mean utilisation, mean pending time, job-level means / medians / spreads).  256 bytes.
+ * "Rows" are the lines of cluster.csv: one per tick for the fifo and horus engines, one per event for the
+ * event-driven policies.  "Jobs" are the lines of job.csv, i.e. the finished jobs.  A job's `arrive` is its
+ * arrival tick gs_jobin.arrive_tick = ceil(normalized_time); job.csv's submit_time is int(normalized_time) and
+ * can be one less.  fifo's start / end / jct / preempt are what job.csv prints: end = start + max(1, ceil(duration))
+ * (duration after the network cost when network costs are on), jct = that run length, preempt = 1.
+ * A summary of a replica that is not done yet covers the rows and finished jobs so far.                        */
+typedef struct gs_summary {
+  int64_t n;                /* jobs in the trace                                                               */
+  int64_t rows;             /* rows folded so far                                                              */
+  int32_t done, status;     /* the replica's done flag and in-kernel status (gs_run_stats)                     */
+  int64_t makespan;         /* `delta` of the last row folded (df.delta.max())                                 */
+  int64_t busy_gpus_sum, running_sum, queued_sum;   /* sums over rows of num_busy_gpus / num_running_jobs / num_queuing_jobs */
+  int32_t busy_gpus_max, running_max, queued_max;   /* their maxima over rows                                            */
+  int32_t pend_max_max;     /* max over rows of max_pending_time                                               */
+  uint64_t pend_sum_lo, pend_sum_hi;   /* sum over rows of the row's pending-time sum (gs_tick_row.pend_sum), 128-bit */
+  uint64_t mem_busy_lo, mem_busy_hi;   /* sum over rows of mem_busy_bytes, 128-bit; mean avg_gpu_memory_allocated =
+                                          this / 2^20 / (M * G * gpu_mem_cap_mib) / rows                              */
+  int64_t pending_rows;     /* rows with avg_pending_time != 0                                                 */
+  double avg_pending_sum;   /* sum of avg_pending_time over those rows, each term pend_sum / (queued + 1e-9)
+                               (log_manager.pending_columns); the mean the notebooks take is this / pending_rows    */
+  double util_sum;          /* horus engine: sum over rows of the sampled avg_gpu_utilization, NaN counted as 0
+                               (the notebooks' fillna(0)); NaN from gs_summarize (that column is sampled on the host) */
+  int64_t finished;         /* lines of job.csv                                                                */
+  int64_t wait_sum, turnaround_sum, jct_sum, preempt_sum, gpu_ticks_sum;  /* sums over finished jobs of start - arrive,
+                               end - arrive, jct, preempt, num_gpu * jct                                          */
+  int32_t wait_q[5], turnaround_q[5], jct_q[5];   /* nearest-rank order statistics at 50 / 90 / 95 / 99 / 100 %: of k
+                               values sorted ascending, rank q (per mille) is element ceil(q * k / 1000) - 1; 0 when k = 0 */
+  int32_t reserved[5];
+} gs_summary;
+
 typedef struct gs_engine *gs_handle;
 
 int gs_abi_version(void);
@@ -343,6 +375,17 @@ int gs_comm_stats(gs_handle h, int64_t *exchanges, double *mean_us);
  * load (the direct table of gs_config_sim) no list we measured -- up to ~7000 runnable jobs -- is evaluated slower by
  * one GPU than an exchange takes (DESIGN section 7 has the numbers); the call is how a caller opts in. */
 int gs_comm_set_min_runnable(gs_handle h, int k);
+
+/* ---- on-device run summaries -------------------------------------------------------------------------
+ * gs_summarize folds, for replicas [first, first + count), the rows of the last gs_run window not folded yet into
+ * per-replica accumulators the handle keeps on the device (gs_result_layout and the result blocks are untouched),
+ * recomputes the job part from the finish order and the per-job results, and copies `count` gs_summary records
+ * to `out` (one copy, synchronous).  Call it after every gs_run to summarise a run of several windows; calling it
+ * twice folds nothing twice.  A replica prepared afresh (first gs_run, gs_reset, a new trace) starts from zero.
+ * kernel_ms (may be NULL) receives the device time of its kernels; gs_run_stats.kernel_ms does not include it.
+ * Errors: GS_ERR_ARG for a bad range, GS_ERR_STATE for a replica that has not run or whose earlier window was
+ * not summarised (nothing is changed then).  util_sum is NaN here.                                        */
+int gs_summarize(gs_handle h, int first, int count, gs_summary *out, double *kernel_ms);
 
 /* Stateless candidate scoring: evaluate b jobs against ONE cluster state.
  * first_node[i] = node of a single-node first fit, or the first node of a

@@ -93,6 +93,12 @@ int gs_horus_stats(gs_horus_handle h, int32_t sim, gs_horus_run_stats *out);
  * array" flag (how str() prints it), and the job records in finish order. */
 int gs_horus_fetch(gs_horus_handle h, int32_t sim, gs_tick_row *rows, double *util, uint8_t *util_is_array,
                    int64_t rows_cap, gs_horus_job_rec *recs, int32_t *finish_order, int64_t *n_rows, int64_t *n_finished);
+/* Run summaries (gs_summary, gsched.h) of replicas [first, first + count), computed on the device from every row the
+ * replicas hold -- [0, ticks): a replica that ran out of rows starts over, so there is no window to carry across --
+ * and from their finished jobs.  util_sum is the sum of the sampled avg_gpu_utilization values (NaN counted as 0).
+ * kernel_ms (may be NULL) receives the device time of the summary kernels.  GS_ERR_ARG for a bad range,
+ * GS_ERR_STATE for a replica that has not run. */
+int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t count, gs_summary *out, double *kernel_ms);
 /* Kernel mapping (no reference counterpart): simulations per warp, 1 (default: lane 0 of each warp) or 32; 0 = one
  * simulation per warp with all 32 lanes scoring a candidate job's devices together (gs_horus_coop_kernel). */
 int gs_horus_set_lanes(gs_horus_handle h, int lanes_per_warp);
