@@ -80,6 +80,9 @@ assert SUMMARY_DTYPE.itemsize == 256
 
 JOBIN_DTYPE = np.dtype([("arrive_tick", "<i4"), ("gpus", "<i4"), ("gpu_per_task", "<i4"), ("ps_count", "<i4"),
                         ("mem_bytes", "<i8"), ("duration", "<f8")])
+# gs_boot_params (include/gsched.h): one bootstrap replica -- Philox key (seed, stream), jobs, gap scale gap_num / gap_den
+BOOT_PARAMS_DTYPE = np.dtype([("seed", "<u8"), ("stream", "<u8"), ("n", "<i8"), ("gap_num", "<i4"), ("gap_den", "<i4")])
+assert BOOT_PARAMS_DTYPE.itemsize == 32
 NODE_DTYPE = np.dtype([("busy_mask", "<u8"), ("cpu_used", "<i4"), ("mem_used", "<i4")])
 JOBREQ_DTYPE = np.dtype([("gpus", "<i4"), ("gpu_per_task", "<i4"), ("mem_bytes", "<i8")])
 
@@ -235,7 +238,11 @@ def load_library():
     lib.gs_result_layout.argtypes = [C.c_void_p, C.c_int, C.POINTER(GsResultLayout)]
     lib.gs_fetch_results.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     lib.gs_summarize.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, f64p]
-    for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize"):
+    lib.gs_boot_population.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+    lib.gs_boot_traces.argtypes = [C.c_void_p, C.c_void_p, f64p]
+    lib.gs_fetch_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
+                 "gs_fetch_trace"):
         getattr(lib, name).restype = C.c_int
     lib.gs_switch_yarn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, f64p, C.c_int64,
                                    C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_int64]
@@ -506,11 +513,11 @@ class Engine:
         mm = arr(table.model_mb, np.float64)
         it = arr(table.iterations, np.float64)
         ps = arr(table.ps_count, np.int32)
-        self._n[sim] = int(table.n)
         self._check(self.lib.gs_load_trace(
             self.h, sim, int(table.n), _ptr(a, C.c_int32), _ptr(g, C.c_int32), _ptr(c, C.c_int32),
             _ptr(d, C.c_double), _ptr(m, C.c_int64), _ptr(mm, C.c_double), _ptr(it, C.c_double),
             _ptr(ps, C.c_int32)), "gs_load_trace")
+        self._n[sim] = int(table.n)                 # only once the replica holds the trace (fetch_trace sizes by it)
 
     def set_engine(self, mode):
         """event-driven policies: 0 / 1 = warp per replica, 2 = thread per replica (the fifo engine has one mapping)"""
@@ -521,9 +528,9 @@ class Engine:
         packed = np.ascontiguousarray(packed, dtype=JOBIN_DTYPE)
         mm = None if model_mb is None else np.ascontiguousarray(model_mb, dtype=np.float64)
         it = None if iterations is None else np.ascontiguousarray(iterations, dtype=np.float64)
-        self._n[sim] = len(packed)
         self._check(self.lib.gs_load_trace_packed(self.h, sim, len(packed), packed.ctypes.data_as(C.c_void_p),
                                                   _ptr(mm, C.c_double), _ptr(it, C.c_double)), "gs_load_trace_packed")
+        self._n[sim] = len(packed)
 
     def fetch_all(self, sim, rows_out, jobs_out, order_out, off_out, spans_out, first=0, count=None):
         """One call: rows of the last window, job records, finish order, spans by job (into caller buffers)."""
@@ -566,11 +573,34 @@ class Engine:
         """every replica's trace from one host block (numpy uint8 / record view; trace i at i * pitch_bytes): one strided upload"""
         n_each = np.ascontiguousarray(n_each, dtype=np.int64)
         assert len(n_each) == self.nsims
-        for i, k in enumerate(n_each.tolist()):
-            self._n[i] = int(k)
         self._keep_block = (block, n_each)
         self._check(self.lib.gs_load_traces_packed(self.h, block.ctypes.data_as(C.c_void_p), int(pitch_bytes), _ptr(n_each, C.c_int64)),
                     "gs_load_traces_packed")
+        self._n = [int(k) for k in n_each.tolist()]
+
+    # ---- bootstrap replicas generated on the device (include/gsched.h: gs_boot_*)
+    def boot_population(self, table_or_packed):
+        """the base trace every replica is drawn from: a JobTable or JOBIN_DTYPE records (validated, copied to the device)"""
+        packed = table_or_packed.packed() if hasattr(table_or_packed, "packed") else table_or_packed
+        packed = np.ascontiguousarray(packed, dtype=JOBIN_DTYPE)
+        self._check(self.lib.gs_boot_population(self.h, packed.ctypes.data_as(C.c_void_p), len(packed)), "gs_boot_population")
+
+    def boot_traces(self, params, with_time=False):
+        """draw every replica's trace from the population: `params` holds one BOOT_PARAMS_DTYPE record per replica.
+        with_time: returns the generator's kernel milliseconds"""
+        params = np.ascontiguousarray(params, dtype=BOOT_PARAMS_DTYPE)
+        if params.shape != (self.nsims,):
+            raise ValueError(f"boot_traces: one parameter record per replica ({self.nsims}), got shape {params.shape}")
+        ms = C.c_double(0.0)
+        self._check(self.lib.gs_boot_traces(self.h, params.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces")
+        self._n = [int(k) for k in params["n"].tolist()]
+        return ms.value if with_time else None
+
+    def fetch_trace(self, sim=0):
+        """the JOBIN_DTYPE records of the trace replica `sim` holds on the device (loaded or generated)"""
+        out = np.zeros(max(self._n[sim], 1), dtype=JOBIN_DTYPE)
+        self._check(self.lib.gs_fetch_trace(self.h, sim, out.ctypes.data_as(C.c_void_p)), "gs_fetch_trace")
+        return out[:self._n[sim]]
 
     def result_layout(self, sim=0) -> GsResultLayout:
         lay = GsResultLayout()

@@ -1,0 +1,156 @@
+// gs_boot.cuh -- bootstrap replicas of a trace generated on the device (gs_boot_population / gs_boot_traces,
+// include/gsched.h), included by gsched.cu.
+//
+// A replica is drawn from one base trace, the population P (K records in admission order) and its K - 1 inter-arrival
+// gaps D.  Job j of replica (seed, stream) takes the four words w0..w3 of the Philox4x64-10 block with key
+// (seed, stream) and counter (j + 1, 0, 0, 0) -- numpy.random.Philox(key=[seed, stream], counter=[j, 0, 0, 0])
+// .random_raw(4), since numpy increments its counter before it generates -- and then
+//   source row  r_j = floor(w0 * K / 2^64)
+//   gap         g_0 = 0, g_j = D[floor(w1 * (K - 1) / 2^64)] (0 when K = 1)
+//   arrival     arrive_j = floor((g_0 + ... + g_j) * gap_num / gap_den), exact integers
+//   record      {arrive_j, P[r_j].gpus, P[r_j].gpu_per_task, 0, P[r_j].mem_bytes, P[r_j].duration}
+// w2 and w3 are unused.  The generator, the pick and the arithmetic are __host__ __device__: tests/emu/boot_emu.cpp
+// runs them with g++, and tracegen.bootstrap_packed is their numpy mirror.
+//
+// gs_boot_kernel: one block per replica walks its jobs in chunks of the block size -- a Philox block per job, a gather
+// of the population row, a block-wide inclusive int64 scan of the gaps with a carry between chunks -- and writes the
+// chunk's 32-byte records through shared memory into the replica's slot of the trace arena with contiguous 16-byte
+// stores.  The same pass reduces the replica's span-pool bound (sum of min(tasks, M)) and last arrival tick.
+#pragma once
+
+#include <stdint.h>
+
+#include "gsched.h"
+
+#ifndef __CUDACC__
+#ifndef __host__
+#define __host__
+#endif
+#ifndef __device__
+#define __device__
+#endif
+#endif
+
+#define GS_BOOT_HD static __host__ __device__ inline
+#define GS_BOOT_THREADS 256
+
+static_assert(sizeof(gs_boot_params) == 32, "gs_boot_params is 32 bytes");
+
+// high 64 bits of the 128-bit product a * b
+GS_BOOT_HD uint64_t gs_boot_mulhi(uint64_t a, uint64_t b) {
+#ifdef __CUDA_ARCH__
+  return __umul64hi(a, b);
+#else
+  return (uint64_t)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+
+struct GsPhilox { uint64_t w[4]; };
+
+// Philox4x64-10 (Salmon et al., SC'11; the constants of Random123 and numpy)
+GS_BOOT_HD GsPhilox gs_boot_philox(uint64_t k0, uint64_t k1, uint64_t c0, uint64_t c1, uint64_t c2, uint64_t c3) {
+  const uint64_t M0 = 0xD2E7470EE14C6C93ull, M1 = 0xCA5A826395121157ull;
+  const uint64_t W0 = 0x9E3779B97F4A7C15ull, W1 = 0xBB67AE8584CAA73Bull;
+#ifdef __CUDA_ARCH__
+#pragma unroll
+#endif
+  for (int r = 0; r < 10; ++r) {
+    if (r > 0) { k0 += W0; k1 += W1; }
+    const uint64_t hi0 = gs_boot_mulhi(M0, c0), lo0 = M0 * c0;
+    const uint64_t hi1 = gs_boot_mulhi(M1, c2), lo1 = M1 * c2;
+    c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+  }
+  GsPhilox b;
+  b.w[0] = c0; b.w[1] = c1; b.w[2] = c2; b.w[3] = c3;
+  return b;
+}
+
+// Source row and gap index (-1: no gap, g_j = 0) of job j of a population of K records.
+GS_BOOT_HD void gs_boot_pick(uint64_t seed, uint64_t stream, long long j, long long K, long long &row, long long &gap) {
+  const GsPhilox b = gs_boot_philox(seed, stream, (uint64_t)j + 1u, 0, 0, 0);
+  row = (long long)gs_boot_mulhi(b.w[0], (uint64_t)K);
+  gap = (j > 0 && K > 1) ? (long long)gs_boot_mulhi(b.w[1], (uint64_t)(K - 1)) : -1;
+}
+
+// arrive = floor(S * gap_num / gap_den) for a gap sum S >= 0.  The caller bounds S * gap_num below 2^62
+// (gs_boot_arrive_bound), so the product fits in 64 bits.
+GS_BOOT_HD int gs_boot_arrive(long long S, int gap_num, int gap_den) { return (int)(S * (long long)gap_num / gap_den); }
+
+// Largest arrival tick any replica of n jobs can reach: floor((n - 1) * max_gap * gap_num / gap_den), exactly.
+GS_BOOT_HD long long gs_boot_arrive_bound(long long n, long long max_gap, int gap_num, int gap_den) {
+  if (n <= 1) return 0;
+  const __int128 x = (__int128)(n - 1) * max_gap * gap_num / gap_den;
+  return x > (__int128)0x7fffffffffffffffll ? 0x7fffffffffffffffll : (long long)x;
+}
+
+#ifdef __CUDACC__
+namespace {
+
+struct GsBootRep {        // one replica's parameters as the kernel reads them
+  uint64_t seed, stream;
+  long long n;
+  int gap_num, gap_den, M, pad;
+};
+
+// out[2 b] = sum over the jobs of min(tasks, M), out[2 b + 1] = last arrival tick (0 without jobs)
+__global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRep *reps, const JobIn *pop, const int *gaps, long long K,
+                                                                 JobIn *arena, long long stride_recs, long long *out) {
+  __shared__ int4 stage[2 * GS_BOOT_THREADS];
+  __shared__ long long warp_tot[GS_BOOT_THREADS / 32];
+  __shared__ long long red[2][GS_BOOT_THREADS / 32];
+  const GsBootRep R = reps[blockIdx.x];
+  int4 *dst = reinterpret_cast<int4 *>(arena + stride_recs * (long long)blockIdx.x);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  long long carry = 0, spans = 0, last = 0;
+  for (long long j0 = 0; j0 < R.n; j0 += blockDim.x) {
+    const long long j = j0 + threadIdx.x;
+    const bool in = j < R.n;
+    long long g = 0;
+    int4 lo = make_int4(0, 0, 0, 0), hi = make_int4(0, 0, 0, 0);
+    if (in) {
+      long long row, gi;
+      gs_boot_pick(R.seed, R.stream, j, K, row, gi);
+      const int4 *src = reinterpret_cast<const int4 *>(pop + row);
+      lo = __ldg(src); hi = __ldg(src + 1);
+      if (gi >= 0) g = __ldg(gaps + gi);
+    }
+    long long x = g;                                   // inclusive scan: lanes, then warps, then the carry
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long y = __shfl_up_sync(0xffffffffu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_tot[warp] = x;
+    __syncthreads();
+    long long before = carry, chunk = 0;
+    for (int w = 0; w < nwarps; ++w) { const long long t = warp_tot[w]; before += w < warp ? t : 0; chunk += t; }
+    carry += chunk;
+    if (in) {
+      const int arrive = gs_boot_arrive(before + x, R.gap_num, R.gap_den);
+      const long long tasks = lo.y / lo.z;
+      spans += tasks < R.M ? tasks : R.M;
+      last = arrive;                                   // arrivals do not decrease: the thread's latest job is its largest
+      stage[2 * threadIdx.x] = make_int4(arrive, lo.y, lo.z, 0);
+      stage[2 * threadIdx.x + 1] = hi;
+    }
+    __syncthreads();
+    const long long cnt = R.n - j0 < (long long)blockDim.x ? R.n - j0 : (long long)blockDim.x;
+    for (int k = threadIdx.x; k < 2 * cnt; k += blockDim.x) dst[2 * j0 + k] = stage[k];
+    __syncthreads();                                   // stage and warp_tot are rewritten by the next chunk
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    spans += __shfl_down_sync(0xffffffffu, spans, o);
+    last = max(last, __shfl_down_sync(0xffffffffu, last, o));
+  }
+  if (lane == 0) { red[0][warp] = spans; red[1][warp] = last; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < nwarps; ++w) { spans += red[0][w]; last = max(last, red[1][w]); }
+    out[2 * blockIdx.x] = spans;
+    out[2 * blockIdx.x + 1] = last;
+  }
+}
+
+}  // namespace
+#endif  // __CUDACC__

@@ -51,6 +51,7 @@
 #include "gs_aux.cuh"
 #include "gs_switch.cuh"
 #include "gs_summary.cuh"
+#include "gs_boot.cuh"
 
 // ------------------------------------------------------------------ host side
 
@@ -116,6 +117,8 @@ struct gs_engine {
   unsigned long long comm_epoch = 0, comm_epoch0 = 0;   // exchange counter: continues across runs / value at the last prepare
   bool dirty = true;       // host mirror of SimDev newer than device copy
   gs_summary *d_sum = nullptr;   // gs_summarize: one accumulator per replica
+  // gs_boot_population: the records of the base trace, then its k - 1 gaps (int32)
+  void *d_pop = nullptr; int64_t pop_k = 0; int64_t pop_max_gap = 0; double pop_max_need = 1.0;
 };
 
 static std::string g_create_err;
@@ -192,6 +195,7 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->h_stage) cudaFreeHost(h->h_stage);
   if (h->d_scratch) cudaFree(h->d_scratch);
   if (h->d_sum) cudaFree(h->d_sum);
+  if (h->d_pop) cudaFree(h->d_pop);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
   if (h->comm_buf) cudaFree(h->comm_buf);
   if (h->e0) cudaEventDestroy(h->e0);
@@ -766,6 +770,35 @@ extern "C" int gs_fetch_compact(gs_handle h, int sim, gs_evrow *ev_out, gs_qrow 
   return GS_OK;
 }
 
+// The trace arena holds the traces of all replicas side by side, one stride apart (gs_load_traces_packed,
+// gs_boot_traces).  reserve_trace_arena makes room for traces of up to nmax records each (h->tarena_stride);
+// bind_arena_trace then points replica i at its slot: loaded, not prepared, the span budget applied.
+static int reserve_trace_arena(gs_handle h, int64_t nmax) {
+  const size_t stride = align_up(sizeof(JobIn) * (size_t)nmax, 512);
+  const size_t need = stride * (size_t)h->nsims;
+  CU(wait_stream(h));                                   // earlier work may still read the old traces
+  if (h->tarena_bytes < need) {
+    if (h->tarena) cudaFree(h->tarena);
+    h->tarena = nullptr; h->tarena_bytes = 0;
+    CU(cudaMalloc(&h->tarena, need));
+    h->tarena_bytes = need;
+  }
+  h->tarena_stride = stride;
+  return GS_OK;
+}
+
+static void bind_arena_trace(gs_handle h, int i, int64_t n, int64_t span_cap, double max_need, int64_t last_arrive) {
+  SimHost &s = h->sims[(size_t)i];
+  SimDev &D = s.dev;
+  memset(&D, 0, sizeof(D));
+  D.jobs = (const JobIn *)((unsigned char *)h->tarena + h->tarena_stride * (size_t)i);
+  if (h->span_budget > 0) { const int64_t lim = (int64_t)(h->span_budget * (double)n) + 4096; if (span_cap > lim) span_cap = lim; }
+  s.n = n; s.span_cap = span_cap > 0 ? span_cap : 1;
+  s.max_need = (int)max_need + 2;
+  s.last_arrive = last_arrive;
+  s.loaded = true; s.prepared = false; s.trace_in_arena = true;
+}
+
 // Every replica of the handle at once, from ONE host block (record i*pitch_bytes is the trace of replica i): the traces
 // go into a device arena with one stride and travel as a single strided copy.  With gs_set_async and a page-locked
 // block nothing is staged and the call returns before the copy completes (keep the block until gs_run / gs_sync).
@@ -790,16 +823,9 @@ extern "C" int gs_load_traces_packed(gs_handle h, const gs_jobin *jobs, size_t p
     if (rc) return rc;
     if (max_need[(size_t)i] > (double)(1 << 26)) return fail(h, GS_ERR_ARG, "gs_load_trace: job duration exceeds 2^26 ticks");
   }
-  const size_t stride = align_up(sizeof(JobIn) * (size_t)nmax, 512);
-  const size_t need = stride * (size_t)h->nsims;
-  CU(wait_stream(h));                                   // earlier work may still read the old traces
-  if (h->tarena_bytes < need) {
-    if (h->tarena) cudaFree(h->tarena);
-    h->tarena = nullptr; h->tarena_bytes = 0;
-    CU(cudaMalloc(&h->tarena, need));
-    h->tarena_bytes = need;
-  }
-  h->tarena_stride = stride;
+  int rc = reserve_trace_arena(h, nmax);
+  if (rc) return rc;
+  const size_t stride = h->tarena_stride;
   bool direct = false;
   if (h->async) {
     cudaPointerAttributes at;
@@ -808,7 +834,7 @@ extern "C" int gs_load_traces_packed(gs_handle h, const gs_jobin *jobs, size_t p
   }
   const void *src = jobs;
   if (!direct) {
-    int rc = ensure_stage(h, pitch_bytes * (size_t)h->nsims);
+    rc = ensure_stage(h, pitch_bytes * (size_t)h->nsims);
     if (rc) return rc;
     memcpy(h->h_stage, jobs, pitch_bytes * (size_t)h->nsims);
     src = h->h_stage;
@@ -822,17 +848,8 @@ extern "C" int gs_load_traces_packed(gs_handle h, const gs_jobin *jobs, size_t p
     h->h2d_ms += ms;
   }
   for (int i = 0; i < h->nsims; ++i) {
-    SimHost &s = h->sims[(size_t)i];
     const JobIn *ji = reinterpret_cast<const JobIn *>(reinterpret_cast<const unsigned char *>(jobs) + pitch_bytes * (size_t)i);
-    SimDev &D = s.dev;
-    memset(&D, 0, sizeof(D));
-    D.jobs = (const JobIn *)((unsigned char *)h->tarena + stride * (size_t)i);
-    int64_t sc = span_cap[(size_t)i];
-    if (h->span_budget > 0) { const int64_t lim = (int64_t)(h->span_budget * (double)n_each[i]) + 4096; if (sc > lim) sc = lim; }
-    s.n = n_each[i]; s.span_cap = sc > 0 ? sc : 1;
-    s.max_need = (int)max_need[(size_t)i] + 2;
-    s.last_arrive = n_each[i] > 0 ? ji[n_each[i] - 1].arrive : 0;
-    s.loaded = true; s.prepared = false; s.trace_in_arena = true;
+    bind_arena_trace(h, i, n_each[i], span_cap[(size_t)i], max_need[(size_t)i], n_each[i] > 0 ? ji[n_each[i] - 1].arrive : 0);
   }
   h->dirty = true;
   return GS_OK;
@@ -1125,6 +1142,94 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
   if (kernel_ms) *kernel_ms = ms;
   for (int i = first; i < first + count; ++i) h->sims[(size_t)i].sum_rows = out[i - first].rows;
   return GS_OK;
+}
+
+// ------------------------------------------------------------------ bootstrap replicas (gs_boot.cuh)
+extern "C" int gs_boot_population(gs_handle h, const gs_jobin *trace, int64_t k) {
+  if (!h) return GS_ERR_ARG;
+  if (!trace || k < 1 || k >= (1ll << 31) - 64) return fail(h, GS_ERR_ARG, "gs_boot_population: bad arguments (1 <= k < 2^31 - 64)");
+  const JobIn *ji = reinterpret_cast<const JobIn *>(trace);
+  SimHost probe;                                        // the load rules do not depend on the cluster without network costs
+  memset(&probe.cl, 0, sizeof(probe.cl));
+  probe.cl.num_switch = probe.cl.num_node_p_switch = 1;
+  int64_t spans = 0;
+  double max_need = 1.0;
+  int rc = scan_trace(h, probe, k, ji, false, nullptr, nullptr, &spans, &max_need);
+  if (rc) return rc;
+  if (max_need > (double)(1 << 26)) return fail(h, GS_ERR_ARG, "gs_boot_population: job duration exceeds 2^26 ticks");
+  std::vector<int32_t> gaps((size_t)(k > 1 ? k - 1 : 1), 0);
+  int64_t max_gap = 0;
+  for (int64_t i = 0; i + 1 < k; ++i) {
+    gaps[(size_t)i] = ji[i + 1].arrive - ji[i].arrive;
+    max_gap = std::max(max_gap, (int64_t)gaps[(size_t)i]);
+  }
+  CU(cudaSetDevice(h->device));
+  const size_t off_gaps = align_up(sizeof(JobIn) * (size_t)k);
+  void *d = nullptr;
+  CU(cudaMalloc(&d, off_gaps + 4 * gaps.size()));
+  cudaError_t e1 = cudaMemcpy(d, ji, sizeof(JobIn) * (size_t)k, cudaMemcpyHostToDevice);
+  cudaError_t e2 = cudaMemcpy((unsigned char *)d + off_gaps, gaps.data(), 4 * gaps.size(), cudaMemcpyHostToDevice);
+  if (e1 != cudaSuccess || e2 != cudaSuccess) { cudaFree(d); return fail(h, GS_ERR_CUDA, "gs_boot_population: upload failed"); }
+  if (h->d_pop) { CU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_pop); }
+  h->d_pop = d; h->pop_k = k; h->pop_max_gap = max_gap; h->pop_max_need = max_need;
+  return GS_OK;
+}
+
+extern "C" int gs_boot_traces(gs_handle h, const gs_boot_params *params, double *kernel_ms) {
+  if (!h) return GS_ERR_ARG;
+  if (!params) return fail(h, GS_ERR_ARG, "gs_boot_traces: params is NULL");
+  if (!h->d_pop) return fail(h, GS_ERR_STATE, "gs_boot_traces: call gs_boot_population first");
+  // every check before anything changes: a refused call leaves the replicas' traces as they were
+  std::vector<GsBootRep> reps((size_t)h->nsims);
+  int64_t nmax = 1;
+  for (int i = 0; i < h->nsims; ++i) {
+    const SimHost &s = h->sims[(size_t)i];
+    const gs_boot_params &p = params[i];
+    if (!s.configured) return fail(h, GS_ERR_STATE, "gs_boot_traces: call gs_config_sim for every replica first");
+    if (s.cl.enable_network_costs) return fail(h, GS_ERR_ARG, "gs_boot_traces: traces with network columns go through gs_load_trace");
+    if (p.n < 0 || p.n >= (1ll << 31) - 64) return fail(h, GS_ERR_ARG, "gs_boot_traces: n out of range");
+    if (p.gap_num < 0 || p.gap_den < 1) return fail(h, GS_ERR_ARG, "gs_boot_traces: the gap scale needs gap_num >= 0 and gap_den >= 1");
+    if (gs_boot_arrive_bound(p.n, h->pop_max_gap, p.gap_num, p.gap_den) >= 0x7fffffffll)
+      return fail(h, GS_ERR_ARG, "gs_boot_traces: the last arrival tick can reach 2^31 - 1 (fewer jobs or a smaller gap scale)");
+    GsBootRep &r = reps[(size_t)i];
+    r.seed = p.seed; r.stream = p.stream; r.n = p.n; r.gap_num = p.gap_num; r.gap_den = p.gap_den;
+    r.M = s.cl.num_switch * s.cl.num_node_p_switch; r.pad = 0;
+    nmax = std::max(nmax, p.n);
+  }
+  CU(cudaSetDevice(h->device));
+  int rc = reserve_trace_arena(h, nmax);
+  if (rc) return rc;
+  const size_t off_out = align_up(sizeof(GsBootRep) * reps.size());
+  rc = ensure_scratch(h, off_out + 16 * reps.size());
+  if (rc) return rc;
+  unsigned char *d = (unsigned char *)h->d_scratch;
+  std::vector<long long> res(2 * reps.size());
+  const JobIn *pop = (const JobIn *)h->d_pop;
+  const int *gaps = (const int *)((unsigned char *)h->d_pop + align_up(sizeof(JobIn) * (size_t)h->pop_k));
+  CU(cudaMemcpyAsync(d, reps.data(), sizeof(GsBootRep) * reps.size(), cudaMemcpyHostToDevice, h->stream));
+  CU(cudaEventRecord(h->e0, h->stream));
+  gs_boot_kernel<<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>((const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena,
+                                                                       (long long)(h->tarena_stride / sizeof(JobIn)), (long long *)(d + off_out));
+  CU(cudaGetLastError());
+  h->launches += 1;
+  CU(cudaEventRecord(h->e1, h->stream));
+  CU(cudaMemcpyAsync(res.data(), d + off_out, 16 * reps.size(), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  float ms = 0; cudaEventElapsedTime(&ms, h->e0, h->e1);
+  if (kernel_ms) *kernel_ms = ms;
+  for (int i = 0; i < h->nsims; ++i) bind_arena_trace(h, i, params[i].n, res[2 * (size_t)i], h->pop_max_need, res[2 * (size_t)i + 1]);
+  h->dirty = true;
+  return GS_OK;
+}
+
+extern "C" int gs_fetch_trace(gs_handle h, int sim, gs_jobin *out) {
+  if (!h) return GS_ERR_ARG;
+  if (sim < 0 || sim >= h->nsims) return fail(h, GS_ERR_ARG, "gs_fetch_trace: sim index out of range");
+  const SimHost &s = h->sims[(size_t)sim];
+  if (!s.loaded) return fail(h, GS_ERR_STATE, "gs_fetch_trace: the replica holds no trace");
+  if (s.n > 0 && !out) return fail(h, GS_ERR_ARG, "gs_fetch_trace: NULL output");
+  CU(cudaSetDevice(h->device));
+  return timed_d2h(h, out, s.dev.jobs, sizeof(JobIn) * (size_t)s.n);
 }
 
 extern "C" int gs_place_batch(gs_handle h, const gs_cluster *cluster, const gs_node *nodes, int32_t m,

@@ -7,10 +7,16 @@ log_manager: every number follows from the record and the cluster shape.
     pending_mean       avg_pending_sum / pending_rows                      mean of avg_pending_time where it is non-zero
     wait_mean, turnaround_mean, jct_mean                                   means over the lines of job.csv
     util_mean          util_sum / rows (horus engine; NaN otherwise)       mean of avg_gpu_utilization, NaN as 0
+
+`spread` takes many records of one configuration (bootstrap replicas, sweep.summarize_bootstrap) and gives, for the
+makespan and each derived number, the mean, the sample standard deviation and a nearest-rank percentile interval.
 """
 from __future__ import annotations
 
 import math
+from fractions import Fraction
+
+import numpy as np
 
 QUANTILES = (50, 90, 95, 99, 100)
 
@@ -38,6 +44,53 @@ def derived(rec, n_nodes, gpus_per_node, gpu_mem_cap_mib):
         jct_mean=_div(int(rec["jct_sum"]), k),
         util_mean=_div(float(rec["util_sum"]), rows),
     )
+
+
+SPREAD_METRICS = ("makespan", "gpu_share", "mem_mean", "pending_mean", "wait_mean", "turnaround_mean", "jct_mean", "util_mean")
+SPREAD_STATS = ("mean", "std", "lo", "hi")
+
+
+def nearest_rank(q, k):
+    """index of the element at fraction q (a Fraction, or a number taken by its decimal text) of k > 0 sorted values:
+    ceil(q * k) - 1, at least 0 -- gs_summary's rule, where q is given in per mille"""
+    q = q if isinstance(q, Fraction) else Fraction(str(q))
+    return max(-((-q.numerator * k) // q.denominator) - 1, 0)
+
+
+def spread(records, n_nodes, gpus_per_node, gpu_mem_cap_mib, level=0.95):
+    """Spread across replicas (e.g. bootstrap replicas of one configuration) of the makespan and of every derived
+    number: {metric: {mean, std (sample, ddof 1), lo, hi}}, where [lo, hi] is the nearest-rank interval holding the
+    central `level` of the replicas' values.  A metric that is NaN for any replica is NaN throughout; std is NaN for
+    fewer than two replicas."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    cols = {m: [] for m in SPREAD_METRICS}
+    for rec in records:
+        d = derived(rec, n_nodes, gpus_per_node, gpu_mem_cap_mib)
+        cols["makespan"].append(float(rec["makespan"]))
+        for m in SPREAD_METRICS[1:]:
+            cols[m].append(d[m])
+    out = {}
+    for m, vals in cols.items():
+        v = np.asarray(vals, dtype=np.float64)
+        k = len(v)
+        if k == 0 or np.isnan(v).any():
+            out[m] = dict.fromkeys(SPREAD_STATS, math.nan)
+            continue
+        s = np.sort(v)
+        out[m] = dict(mean=float(v.mean()), std=float(v.std(ddof=1)) if k > 1 else math.nan,
+                      lo=float(s[nearest_rank((1 - level) / 2, k)]), hi=float(s[nearest_rank((1 + level) / 2, k)]))
+    return out
+
+
+def spread_columns():
+    """names of the flat columns of a spread, in the order `spread_flat` returns them"""
+    return [f"{m}_{s}" for m in SPREAD_METRICS for s in SPREAD_STATS]
+
+
+def spread_flat(sp):
+    return [sp[m][s] for m in SPREAD_METRICS for s in SPREAD_STATS]
 
 
 def columns():

@@ -6,8 +6,10 @@ from __future__ import annotations
 
 import argparse
 import datetime
+import math
 import os
 import types
+from fractions import Fraction
 
 import numpy as np
 
@@ -181,6 +183,93 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16):
     return out
 
 
+def load_gap_scale(load):
+    """offered load L as the gap scale 1/L of gs_boot_params: (gap_num, gap_den)"""
+    f = Fraction(1.0 / float(load)).limit_denominator(65535)
+    return f.numerator, f.denominator
+
+
+def _check_bootstrap_args(flag_sets, replicas, loads, n):
+    if int(replicas) < 1:
+        raise ValueError("bootstrap: replicas must be >= 1")
+    if not len(loads) or not all(math.isfinite(float(L)) and float(L) > 0 for L in loads):
+        raise ValueError("bootstrap: loads must be positive and finite")
+    if any(load_gap_scale(L)[0] > 2 ** 31 - 1 for L in loads):
+        raise ValueError("bootstrap: a load is too small to be expressed as a gap scale")
+    if n is not None and not 0 <= int(n) < 2 ** 31 - 64:
+        raise ValueError("bootstrap: n out of range")
+    aware = [fl.schedule for fl in flag_sets if _is_utilisation_aware(fl)]
+    if aware:
+        raise ValueError(f"bootstrap: the utilisation-aware engine ({', '.join(sorted(set(aware)))}) has no generated traces")
+
+
+def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0):
+    """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
+    its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
+    (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
+    summarised on the device.  A replica has `n` jobs (default: as many as its base trace).  The same replica index
+    draws the same jobs and gaps under every configuration and load (common random numbers), so configurations can be
+    compared replica by replica.  Returns SUMMARY_DTYPE records of shape (len(flag_sets), len(loads), replicas).
+
+    One engine handle per base trace file.  A gittins replica takes its index table from the base trace (the
+    replica's own trace never reaches the host).  Utilisation-aware configurations are an argument error, as are
+    replicas < 1 and non-positive loads; every argument is checked before a trace is read or an engine created."""
+    _check_bootstrap_args(flag_sets, replicas, loads, n)
+    R, loads = int(replicas), [float(L) for L in loads]
+    out = np.zeros((len(flag_sets), len(loads), R), dtype=capi.SUMMARY_DTYPE)
+    by_trace = {}
+    for c, fl in enumerate(flag_sets):
+        by_trace.setdefault(fl.trace_file, []).append(c)
+    for configs in by_trace.values():
+        sims = _plain_setup([flag_sets[c] for c in configs])
+        base = sims[0][2].table
+        jobs = base.n if n is None else int(n)
+        params = np.zeros(len(configs) * len(loads) * R, dtype=capi.BOOT_PARAMS_DTYPE)
+        with capi.Engine(device=device, nsims=len(params)) as eng:
+            i = 0
+            for fl, infra, jm, pol in sims:
+                for L in loads:
+                    num, den = load_gap_scale(L)
+                    for r in range(R):
+                        eng.config(i, infra.gs_cluster(), pol)
+                        params[i] = (seed, r, jobs, num, den)
+                        i += 1
+            eng.boot_population(base)
+            eng.boot_traces(params)
+            recs = eng.run_summarized()
+        for k, c in enumerate(configs):
+            out[c] = recs[k * len(loads) * R:(k + 1) * len(loads) * R].reshape(len(loads), R)
+    return out
+
+
+def write_bootstrap_csv(path, flag_sets, loads, records):
+    """one line per (configuration, load, replica): replica, load, the configuration's flags, the summary columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(["replica", "load"] + SUMMARY_KEYS + summary.columns())
+        for fl, per_load in zip(flag_sets, records):
+            cl = Infrastructure(fl).gs_cluster()
+            shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
+            for L, recs in zip(loads, per_load):
+                for r, rec in enumerate(recs):
+                    w.writerow([r, L, fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + summary.flat(rec, *shape))
+
+
+def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95):
+    """one line per (configuration, load): the flags, the load, the replica count and summary.spread's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["load", "replicas", "level"] + summary.spread_columns())
+        for fl, per_load in zip(flag_sets, records):
+            cl = Infrastructure(fl).gs_cluster()
+            shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
+            for L, recs in zip(loads, per_load):
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, len(recs), level]
+                           + summary.spread_flat(summary.spread(recs, *shape, level=level)))
+
+
 SUMMARY_KEYS = ["trace", "scheme", "schedule", "num_buffer", "num_queue", "seed"]
 
 
@@ -209,7 +298,22 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=-1)
     ap.add_argument("--summary", default=None, metavar="FILE",
                     help="write one CSV line of run summary per configuration to FILE instead of the per-run logs")
+    ap.add_argument("--bootstrap", type=int, default=None, metavar="R",
+                    help="run R bootstrap replicas of every configuration, drawn on the GPU from its trace (needs --summary; "
+                         "the Philox key is (--seed, or 0 when it is negative, replica index))")
+    ap.add_argument("--load", type=float, nargs="+", default=None, metavar="L",
+                    help="with --bootstrap: offered loads, the trace's inter-arrival gaps scaled by 1/L (default 1)")
+    ap.add_argument("--jobs", type=int, default=None, metavar="N", help="with --bootstrap: jobs per replica (default: the trace's)")
+    ap.add_argument("--summary-ci", default=None, metavar="FILE",
+                    help="with --bootstrap: one CSV line per (configuration, load) with the mean, std and 95%% interval across replicas")
     a = ap.parse_args(argv)
+    if a.bootstrap is None and (a.load is not None or a.jobs is not None or a.summary_ci is not None):
+        ap.error("--load, --jobs and --summary-ci need --bootstrap")
+    if a.bootstrap is not None:
+        if not a.summary:
+            ap.error("--bootstrap needs --summary FILE")
+        if a.repeats != 1:
+            ap.error("--bootstrap replaces --repeats")
     sets = []
     for tr in a.trace:
         for sc in a.schedule:
@@ -220,6 +324,18 @@ def main(argv=None):
                                        num_node_p_switch=a.num_node_p_switch, num_queue=a.num_queue, num_buffer=a.num_buffer,
                                        log_path=os.path.join(f"batched_{tag}", f"{scheme}_{sc}"),
                                        seed=a.seed if a.seed < 0 else a.seed + rep))
+    if a.bootstrap is not None:
+        loads = a.load or [1.0]
+        try:
+            _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs)
+        except ValueError as e:
+            ap.error(str(e))
+        recs = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs)
+        write_bootstrap_csv(a.summary, sets, loads, recs)
+        if a.summary_ci:
+            write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs)
+        print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads x {a.bootstrap} replicas")
+        return
     if a.summary:
         write_summary_csv(a.summary, sets, summarize_batched(sets))
         print(f"{a.summary}: {len(sets)} configurations")

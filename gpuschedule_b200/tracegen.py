@@ -76,6 +76,87 @@ def synth_columns(n_jobs: int, seed: int = 1, rate: float = 0.5,
     return cols
 
 
+# ---- bootstrap replicas: the host mirror of gs_boot_traces (gpuschedule_b200/csrc/gs_boot.cuh), bit for bit
+_PHILOX_M = (np.uint64(0xD2E7470EE14C6C93), np.uint64(0xCA5A826395121157))
+_PHILOX_W = (np.uint64(0x9E3779B97F4A7C15), np.uint64(0xBB67AE8584CAA73B))
+_LO32 = np.uint64(0xFFFFFFFF)
+_S32 = np.uint64(32)
+
+
+def mulhi64(a, b):
+    """high 64 bits of the 128-bit products a * b (uint64 arrays, broadcast)"""
+    a, b = np.asarray(a, dtype=np.uint64), np.asarray(b, dtype=np.uint64)
+    a_lo, a_hi, b_lo, b_hi = a & _LO32, a >> _S32, b & _LO32, b >> _S32
+    lh, hl = a_lo * b_hi, a_hi * b_lo
+    mid = ((a_lo * b_lo) >> _S32) + (lh & _LO32) + (hl & _LO32)
+    return a_hi * b_hi + (lh >> _S32) + (hl >> _S32) + (mid >> _S32)
+
+
+def philox4x64(seed, stream, counters):
+    """Philox4x64-10 blocks with key (seed, stream) at `counters` (uint64, shape (..., 4)); returns the four words of
+    each block, shape (..., 4).  numpy.random.Philox(key=[seed, stream], counter=c).random_raw(4) is the block at c + 1."""
+    c = np.array(counters, dtype=np.uint64)
+    if c.shape[-1:] != (4,):
+        raise ValueError("counters must have shape (..., 4)")
+    c0, c1, c2, c3 = (c[..., i] for i in range(4))
+    k0, k1 = np.array(seed, dtype=np.uint64), np.array(stream, dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        for r in range(10):
+            if r:
+                k0, k1 = k0 + _PHILOX_W[0], k1 + _PHILOX_W[1]
+            hi0, lo0 = mulhi64(_PHILOX_M[0], c0), _PHILOX_M[0] * c0
+            hi1, lo1 = mulhi64(_PHILOX_M[1], c2), _PHILOX_M[1] * c2
+            c0, c1, c2, c3 = hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0
+    return np.stack([c0, c1, c2, c3], axis=-1)
+
+
+def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1):
+    """Replica (seed, stream) of `n` jobs drawn from `population` (JOBIN_DTYPE records of one trace in admission order):
+    job j resamples a row and an inter-arrival gap of the population with the Philox4x64-10 block at counter
+    (j + 1, 0, 0, 0), and its arrival is floor(gap sum * gap_num / gap_den) (include/gsched.h, gs_boot_traces).
+    Returns (JOBIN_DTYPE records, source rows)."""
+    from .capi import JOBIN_DTYPE
+    pop = np.ascontiguousarray(population, dtype=JOBIN_DTYPE)
+    k, n, gap_num, gap_den = len(pop), int(n), int(gap_num), int(gap_den)
+    if k < 1 or not 0 <= n < 2 ** 31 - 64 or gap_num < 0 or gap_den < 1:
+        raise ValueError("bootstrap_packed: needs a population of at least one record, 0 <= n < 2^31 - 64, gap_num >= 0, gap_den >= 1")
+    gaps = np.diff(pop["arrive_tick"].astype(np.int64))
+    max_gap = int(gaps.max()) if len(gaps) else 0
+    if n > 1 and (n - 1) * max_gap * gap_num // gap_den >= 2 ** 31 - 1:
+        raise ValueError("bootstrap_packed: the last arrival tick can reach 2^31 - 1")
+    ctr = np.zeros((n, 4), dtype=np.uint64)
+    ctr[:, 0] = np.arange(1, n + 1, dtype=np.uint64)
+    w = philox4x64(seed, stream, ctr)
+    rows = mulhi64(w[:, 0], np.uint64(k)).astype(np.int64)
+    g = np.zeros(n, dtype=np.int64)
+    if k > 1 and n > 1:
+        g[1:] = gaps[mulhi64(w[1:, 1], np.uint64(k - 1)).astype(np.int64)]
+    out = np.zeros(n, dtype=JOBIN_DTYPE)
+    out["arrive_tick"] = np.cumsum(g) * gap_num // gap_den       # below 2^62 by the bound checked above
+    src = pop[rows]
+    for f in ("gpus", "gpu_per_task", "mem_bytes", "duration"):
+        out[f] = src[f]
+    return out, rows
+
+
+def bootstrap_table(base_table, seed, stream, n, gap_num=1, gap_den=1):
+    """bootstrap_packed of a JobTable as a JobTable of its own (labels 0..n-1, the source rows' num_gpu_text and
+    utilisation columns, submit = arrive), so that a generated replica can go through the ordinary upload path and
+    the ordinary log writers."""
+    from .ingest import JobTable
+    recs, rows = bootstrap_packed(base_table.packed(), seed, stream, n, gap_num, gap_den)
+    pick = lambda a: None if a is None else np.ascontiguousarray(np.asarray(a)[rows])
+    t = JobTable(
+        n=len(recs), label=[str(i) for i in range(len(recs))],
+        num_gpu_text=None if base_table.num_gpu_text is None else [base_table.num_gpu_text[r] for r in rows.tolist()],
+        arrive_tick=recs["arrive_tick"].copy(), submit=recs["arrive_tick"].copy(), gpus=recs["gpus"].copy(),
+        gpu_per_task=recs["gpu_per_task"].copy(), duration=recs["duration"].copy(), mem_bytes=recs["mem_bytes"].copy(),
+        util_avg=pick(base_table.util_avg), util_max=pick(base_table.util_max))
+    if "mem_avg_mib" in base_table.extra:
+        t.extra["mem_avg_mib"] = pick(base_table.extra["mem_avg_mib"])
+    return t
+
+
 def synth_frame(n_jobs: int, **kw):
     import pandas as pd
     return pd.DataFrame(synth_columns(n_jobs, **kw))

@@ -387,6 +387,31 @@ int gs_comm_set_min_runnable(gs_handle h, int k);
  * not summarised (nothing is changed then).  util_sum is NaN here.                                        */
 int gs_summarize(gs_handle h, int first, int count, gs_summary *out, double *kernel_ms);
 
+/* ---- bootstrap replicas generated on the device ---------------------------------------------------------
+ * gs_boot_population gives the handle one base trace P of k >= 1 records (admission order, the gs_load_trace rules;
+ * validated once, copied to the device); D holds its k - 1 inter-arrival gaps D[i] = P[i+1].arrive_tick - P[i].arrive_tick.
+ * gs_boot_traces then draws a trace for EVERY replica of the handle from params[sim] (nsims entries): job j takes the
+ * words w0..w3 of the Philox4x64-10 block with key (seed, stream) and counter (j + 1, 0, 0, 0) -- numpy's
+ * Philox(key=[seed, stream], counter=[j, 0, 0, 0]).random_raw(4) -- and becomes
+ *   {floor(S_j * gap_num / gap_den), P[r].gpus, P[r].gpu_per_task, 0, P[r].mem_bytes, P[r].duration}
+ * with r = floor(w0 * k / 2^64), S_j = g_0 + ... + g_j, g_0 = 0, g_j = D[floor(w1 * (k - 1) / 2^64)] (0 when k = 1).
+ * gap_num / gap_den = 1 / 1 keeps the base trace's arrival rate in expectation, 1 / 2 doubles the offered load; the same
+ * (seed, stream) draws the same rows and gaps at every load (common random numbers).  Afterwards every replica is in the
+ * state gs_load_traces_packed leaves (loaded, not prepared, span budget applied); kernel_ms (may be NULL) receives the
+ * generator's device time.  gs_fetch_trace copies the n records of any resident trace of one replica (synchronous).
+ * Errors (nothing changes): GS_ERR_ARG for a NULL argument, k < 1 or a record that breaks the load rules, n outside
+ * gs_load_traces_packed's range, gap_num < 0 or gap_den < 1, a replica whose cluster has network costs, or a worst-case
+ * last arrival floor((n - 1) * max(D) * gap_num / gap_den) of 2^31 - 1 or more; GS_ERR_STATE without a population, for
+ * a replica not configured with gs_config_sim, or (gs_fetch_trace) for a replica that holds no trace.          */
+typedef struct gs_boot_params {
+  uint64_t seed, stream;    /* Philox key                                                                     */
+  int64_t n;                /* jobs                                                                           */
+  int32_t gap_num, gap_den; /* gap scale: gap_num >= 0, gap_den >= 1                                          */
+} gs_boot_params;           /* 32 bytes */
+int gs_boot_population(gs_handle h, const gs_jobin *trace, int64_t k);
+int gs_boot_traces(gs_handle h, const gs_boot_params *params /* nsims */, double *kernel_ms);
+int gs_fetch_trace(gs_handle h, int sim, gs_jobin *out /* n records */);
+
 /* Stateless candidate scoring: evaluate b jobs against ONE cluster state.
  * first_node[i] = node of a single-node first fit, or the first node of a
  * cross-node fill, or -1 if the job cannot be placed; task_node (optional)
