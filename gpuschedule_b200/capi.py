@@ -77,6 +77,15 @@ SUMMARY_DTYPE = np.dtype([("n", "<i8"), ("rows", "<i8"), ("done", "<i4"), ("stat
                           ("gpu_ticks_sum", "<i8"), ("wait_q", "<i4", (5,)), ("turnaround_q", "<i4", (5,)), ("jct_q", "<i4", (5,)),
                           ("reserved", "<i4", (5,))])
 assert SUMMARY_DTYPE.itemsize == 256
+# gs_tbin (include/gsched.h): one bin of a replica's timeline -- gs_summary's row part restricted to the rows with
+# min(delta // W, B - 1) == bin, their smallest / largest delta and the `finished` counter of the bin's last row
+TBIN_DTYPE = np.dtype([("rows", "<i8"), ("busy_gpus_sum", "<i8"), ("running_sum", "<i8"), ("queued_sum", "<i8"),
+                       ("busy_gpus_max", "<i4"), ("running_max", "<i4"), ("queued_max", "<i4"), ("pend_max_max", "<i4"),
+                       ("pend_sum_lo", "<u8"), ("pend_sum_hi", "<u8"), ("mem_busy_lo", "<u8"), ("mem_busy_hi", "<u8"),
+                       ("pending_rows", "<i8"), ("avg_pending_sum", "<f8"), ("util_sum", "<f8"),
+                       ("delta_min", "<i8"), ("delta_max", "<i8"), ("finished_last", "<i8")])
+assert TBIN_DTYPE.itemsize == 128
+TIMELINE_MAX_BINS = 1024
 
 JOBIN_DTYPE = np.dtype([("arrive_tick", "<i4"), ("gpus", "<i4"), ("gpu_per_task", "<i4"), ("ps_count", "<i4"),
                         ("mem_bytes", "<i8"), ("duration", "<f8")])
@@ -180,7 +189,9 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_last_error.restype = C.c_char_p
     lib.gs_horus_build_tag.restype = C.c_char_p
     lib.gs_horus_summarize.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, f64p]
-    for name in ("gs_horus_summarize", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
+    lib.gs_horus_set_timeline.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
+    lib.gs_horus_fetch_timeline.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+    for name in ("gs_horus_summarize", "gs_horus_set_timeline", "gs_horus_fetch_timeline", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
                  "gs_horus_run", "gs_horus_stats", "gs_horus_fetch"):
         getattr(lib, name).restype = C.c_int
     return lib
@@ -241,8 +252,10 @@ def load_library():
     lib.gs_boot_population.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
     lib.gs_boot_traces.argtypes = [C.c_void_p, C.c_void_p, f64p]
     lib.gs_fetch_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    lib.gs_set_timeline.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
+    lib.gs_fetch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
-                 "gs_fetch_trace"):
+                 "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline"):
         getattr(lib, name).restype = C.c_int
     lib.gs_switch_yarn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, f64p, C.c_int64,
                                    C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_int64]
@@ -463,6 +476,24 @@ class HorusEngine:
         self._check(self.lib.gs_horus_summarize(self.h, int(first), count, out.ctypes.data_as(C.c_void_p), C.byref(ms)),
                     "gs_horus_summarize")
         return (out[:count], ms.value) if with_time else out[:count]
+
+    def set_timeline(self, width, nbins):
+        """bin every summarised row by min(delta // width, nbins - 1) on the device; nbins = 0 turns it off
+        (include/gsched_horus.h: gs_horus_set_timeline)"""
+        self._check(self.lib.gs_horus_set_timeline(self.h, int(width), int(nbins)), "gs_horus_set_timeline")
+        self._tl_nbins = int(nbins)
+
+    def timeline(self, first=0, count=None):
+        """TBIN_DTYPE bins of replicas [first, first+count) as of the last summarize(): shape (count, nbins)"""
+        return _fetch_timeline(self, self.lib.gs_horus_fetch_timeline, "gs_horus_fetch_timeline", first, count)
+
+
+def _fetch_timeline(eng, fn, what, first, count):
+    count = eng.nsims - first if count is None else int(count)
+    b = getattr(eng, "_tl_nbins", 0)
+    out = np.zeros((max(count, 1), max(b, 1)), dtype=TBIN_DTYPE)
+    eng._check(fn(eng.h, int(first), count, out.ctypes.data_as(C.c_void_p)), what)
+    return out[:count, :b]
 
 
 class Engine:
@@ -741,6 +772,16 @@ class Engine:
         ms = C.c_double(0.0)
         self._check(self.lib.gs_summarize(self.h, int(first), count, out.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_summarize")
         return (out[:count], ms.value) if with_time else out[:count]
+
+    def set_timeline(self, width, nbins):
+        """while nbins > 0, every summarize() also bins the rows it folds by min(delta // width, nbins - 1) on the
+        device; nbins = 0 turns it off.  Set it before the first summarize() of a run (include/gsched.h: gs_set_timeline)"""
+        self._check(self.lib.gs_set_timeline(self.h, int(width), int(nbins)), "gs_set_timeline")
+        self._tl_nbins = int(nbins)
+
+    def timeline(self, first=0, count=None):
+        """TBIN_DTYPE bins of replicas [first, first+count) as of the last summarize(): shape (count, nbins)"""
+        return _fetch_timeline(self, self.lib.gs_fetch_timeline, "gs_fetch_timeline", first, count)
 
     def run_summarized(self, rows_cap=0):
         """Run every replica to its exit condition, summarising after every launch and fetching no rows; returns

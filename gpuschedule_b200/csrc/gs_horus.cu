@@ -64,6 +64,13 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_hsum_rows_kernel(const HSim
   }
 }
 
+// Timeline of gs_horus_summarize: the same rows [0, ticks) with the sampled utilisation, into zeroed bins.
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_htl_rows_kernel(const HSim *sims, int first, gs_tbin *bins, long long W, int B) {
+  const int r = first + blockIdx.x;
+  const HSim &S = sims[r];
+  gs_tl_fold_rows(bins + (size_t)r * (size_t)B, B, W, S.rows, S.util, 0, 0, S.ticks);
+}
+
 struct GsSumHorusJobs {
   const HSim *sims;
   __device__ long long finished(int r) const { return sims[r].nfin; }
@@ -86,6 +93,7 @@ struct WordStream {                 // raw MT19937 words + the per-position samp
 };
 struct HorusSimHost {
   bool configured = false, loaded = false, prepared = false;
+  bool tl_done = false;             // summarised with the timeline on since it was prepared
   gs_cluster cl{};
   gs_horus_params par{};
   std::vector<HJob> jobs;
@@ -110,6 +118,8 @@ struct gs_horus_handle_s {
   long long launches = 0;
   gs_summary *d_sum = nullptr;      // gs_horus_summarize: one record per replica
   int *d_sum_scratch = nullptr; size_t sum_scratch_bytes = 0;
+  gs_tbin *d_tl = nullptr; size_t tl_bytes = 0;   // gs_horus_set_timeline: nsims x tl_nbins bins
+  int64_t tl_width = 0; int tl_nbins = 0;
   std::string err;
   std::vector<double> shared;       // one stream consumed by every replica that did not get its own
   double *d_shared = nullptr; size_t shared_cap = 0; bool shared_dirty = false;
@@ -158,6 +168,7 @@ extern "C" int gs_horus_destroy(gs_horus_handle h) {
   if (h->d_sims) cudaFree(h->d_sims);
   if (h->d_sum) cudaFree(h->d_sum);
   if (h->d_sum_scratch) cudaFree(h->d_sum_scratch);
+  if (h->d_tl) cudaFree(h->d_tl);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -347,7 +358,7 @@ static int prepare(gs_horus_handle h, HorusSimHost &s, long long rows_cap) {
   D.rows_cap = rows_cap;
   D.current_remaining = (long long)n; D.running_jobs = 0;
   s.rows_cap = rows_cap;
-  s.prepared = true;
+  s.prepared = true; s.tl_done = false;
   return GS_OK;
 }
 
@@ -451,6 +462,8 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   HCU(cudaSetDevice(h->device));
   if (!h->d_sum) HCU(cudaMalloc(&h->d_sum, sizeof(gs_summary) * (size_t)nsims));
   HCU(cudaMemsetAsync(h->d_sum + first, 0, sizeof(gs_summary) * (size_t)count, h->stream));
+  const int B = h->tl_nbins;
+  if (B > 0) HCU(cudaMemsetAsync(h->d_tl + (size_t)first * B, 0, sizeof(gs_tbin) * (size_t)B * (size_t)count, h->stream));
 #ifdef __CUDACC__
   int per_sm = 1, sms = 132;
   HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_sum_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
@@ -470,6 +483,11 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
                                                                                       h->d_sum_scratch, (long long)pitch);
   HCU(cudaGetLastError());
   h->launches += 2;
+  if (B > 0) {
+    gs_htl_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->d_tl, (long long)h->tl_width, B);
+    HCU(cudaGetLastError());
+    h->launches += 1;
+  }
   HCU(cudaEventRecord(h->ev1, h->stream));
 #else   // host build for tests/emu: the same folds, one replica after the other
   for (int r = first; r < first + count; ++r) {
@@ -487,6 +505,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
       jobs[(size_t)i] = gs_sum_job(S.jobs[j].arrive, S.recs[j].start, S.recs[j].end, S.recs[j].jct, S.recs[j].preempt, S.jobs[j].gpus);
     }
     gs_sum_jobs_serial(jobs.data(), S.nfin, A);
+    if (B > 0) gs_tl_fold_rows_serial(h->d_tl + (size_t)r * B, B, (long long)h->tl_width, S.rows, S.util, 0, 0, S.ticks);
   }
   (void)kmax;
 #endif
@@ -497,5 +516,40 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   HCU(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   if (kernel_ms) *kernel_ms = ms;
 #endif
+  if (B > 0) for (int i = first; i < first + count; ++i) h->sims[(size_t)i].tl_done = true;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_set_timeline(gs_horus_handle h, int64_t bin_width, int32_t nbins) {
+  if (!h) return GS_ERR_ARG;
+  if (nbins < 0 || nbins > GS_TIMELINE_MAX_BINS || (nbins > 0 && (bin_width < 1 || bin_width > (1ll << 40))))
+    return hfail(h, GS_ERR_ARG, "gs_horus_set_timeline: nbins must be in 0..1024 and, when it is not 0, bin_width in 1..2^40");
+  const size_t need = sizeof(gs_tbin) * h->sims.size() * (size_t)nbins;
+  if (need > h->tl_bytes) {
+    HCU(cudaSetDevice(h->device));
+    gs_tbin *d = nullptr;
+    HCU(cudaMalloc(&d, need));
+    if (h->d_tl) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_tl); }
+    h->d_tl = d; h->tl_bytes = need;
+  }
+  h->tl_width = nbins > 0 ? bin_width : 0;
+  h->tl_nbins = nbins;
+  for (auto &s : h->sims) s.tl_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_fetch_timeline(gs_horus_handle h, int32_t first, int32_t count, gs_tbin *out) {
+  if (!h) return GS_ERR_ARG;
+  const int nsims = (int)h->sims.size();
+  if (first < 0 || count < 0 || first > nsims - count || (count > 0 && !out)) return hfail(h, GS_ERR_ARG, "gs_horus_fetch_timeline: bad arguments");
+  if (h->tl_nbins == 0) return hfail(h, GS_ERR_STATE, "gs_horus_fetch_timeline: the timeline is off (gs_horus_set_timeline)");
+  for (int i = first; i < first + count; ++i)
+    if (!h->sims[(size_t)i].prepared || !h->sims[(size_t)i].tl_done)
+      return hfail(h, GS_ERR_STATE, "gs_horus_fetch_timeline: a replica has not been summarised with the timeline on since it was prepared");
+  if (count == 0) return GS_OK;
+  HCU(cudaSetDevice(h->device));
+  const size_t B = (size_t)h->tl_nbins;
+  HCU(cudaMemcpyAsync(out, h->d_tl + (size_t)first * B, sizeof(gs_tbin) * B * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
   return GS_OK;
 }

@@ -122,6 +122,84 @@ GS_SUM_HD void gs_sum_add_rows(gs_summary &s, const GsSumPart &p) {
   s.pending_rows += p.pending_rows; s.avg_pending_sum += p.avg; s.util_sum += p.util;
 }
 
+// ---- timeline (gs_tbin): the row fold above, keyed by bin = min(floor(delta / W), B - 1)
+static_assert(sizeof(gs_tbin) == 128, "gs_tbin is 128 bytes");
+
+// Partial fold of some rows of ONE bin.  `last` orders rows (row index, or `delta` for the fifo records, which are
+// monotone): `fin` is the `finished` counter of the row with the largest `last`.
+struct GsTlPart {
+  GsSumPart s;
+  long long dmin, dmax, last, fin;
+};
+
+GS_SUM_HD int gs_tl_bin(long long delta, long long W, int B) {
+  if (delta < 0) return 0;
+  const long long b = delta / W;
+  return b < B - 1 ? (int)b : B - 1;
+}
+
+GS_SUM_HD void gs_tl_zero(GsTlPart &p) {
+  gs_sum_zero(p.s);
+  p.dmin = 0x7fffffffffffffffll; p.dmax = -0x7fffffffffffffffll - 1; p.last = -1; p.fin = 0;
+}
+
+GS_SUM_HD void gs_tl_row(GsTlPart &p, const gs_tick_row &r, double util, long long index) {
+  gs_sum_row(p.s, r, util);
+  p.dmin = r.now < p.dmin ? r.now : p.dmin; p.dmax = r.now > p.dmax ? r.now : p.dmax;
+  if (index > p.last) { p.last = index; p.fin = r.finished; }
+}
+
+// The rows v_lo .. v_hi of one fifo record (already clipped to the bin and to the watermark; nothing if empty).
+GS_SUM_HD void gs_tl_record(GsTlPart &p, const gs_evrow &e, long long arrive_sum, int oldest, long long v_lo, long long v_hi) {
+  if (v_hi < v_lo) return;
+  gs_sum_record(p.s, e, arrive_sum, oldest, v_lo, v_hi);
+  p.dmin = v_lo < p.dmin ? v_lo : p.dmin; p.dmax = v_hi > p.dmax ? v_hi : p.dmax;
+  if (v_hi > p.last) { p.last = v_hi; p.fin = e.finished; }
+}
+
+GS_SUM_HD void gs_tl_merge(GsTlPart &a, const GsTlPart &b) {
+  gs_sum_merge(a.s, b.s);
+  a.dmin = b.dmin < a.dmin ? b.dmin : a.dmin; a.dmax = b.dmax > a.dmax ? b.dmax : a.dmax;
+  if (b.last > a.last) { a.last = b.last; a.fin = b.fin; }
+}
+
+// Add a partial to a bin.  Partials reach a bin in row order (later windows, later runs of rows), so the newest one
+// carries the bin's last row.
+GS_SUM_HD void gs_tl_add(gs_tbin &t, const GsTlPart &p) {
+  if (p.s.rows == 0) return;
+  if (t.rows == 0) { t.delta_min = p.dmin; t.delta_max = p.dmax; }
+  else { t.delta_min = p.dmin < t.delta_min ? p.dmin : t.delta_min; t.delta_max = p.dmax > t.delta_max ? p.dmax : t.delta_max; }
+  t.finished_last = p.fin;
+  t.rows += p.s.rows;
+  t.busy_gpus_sum += p.s.busy; t.running_sum += p.s.running; t.queued_sum += p.s.queued;
+  t.busy_gpus_max = gs_sum_imax(t.busy_gpus_max, p.s.busy_max); t.running_max = gs_sum_imax(t.running_max, p.s.running_max);
+  t.queued_max = gs_sum_imax(t.queued_max, p.s.queued_max); t.pend_max_max = gs_sum_imax(t.pend_max_max, p.s.pend_max);
+  gs_sum_add128(t.pend_sum_lo, t.pend_sum_hi, p.s.pend);
+  gs_sum_add128(t.mem_busy_lo, t.mem_busy_hi, p.s.mem);
+  t.pending_rows += p.s.pending_rows; t.avg_pending_sum += p.s.avg; t.util_sum += p.s.util;
+}
+
+// Rows lo .. hi - 1 (rows[i - base]; util may be NULL) in row order, one partial per run of rows that share a bin.
+// Any order of `delta` is binned correctly.  The bin kernel's path for rows whose `delta` is not monotone (run by one
+// thread) and the host-emulation build's horus timeline.
+GS_SUM_HD void gs_tl_fold_rows_serial(gs_tbin *bins, int B, long long W, const gs_tick_row *rows, const double *util,
+                                      long long base, long long lo, long long hi) {
+  GsTlPart p;
+  gs_tl_zero(p);
+  int cur = -1;
+  for (long long i = lo; i < hi; ++i) {
+    const gs_tick_row &r = rows[i - base];
+    const int b = gs_tl_bin(r.now, W, B);
+    if (b != cur) {
+      if (cur >= 0) gs_tl_add(bins[cur], p);
+      gs_tl_zero(p);
+      cur = b;
+    }
+    gs_tl_row(p, r, util ? util[i - base] : 0.0, i);
+  }
+  if (cur >= 0) gs_tl_add(bins[cur], p);
+}
+
 // ---- jobs
 struct GsSumJob { int wait, turn, jct, preempt, gpus; };
 
@@ -275,6 +353,137 @@ __device__ void gs_sum_fold_records(GsSumPart &p, const gs_evrow *ev, int nev, c
     }
     qbase += total;
   }
+}
+
+// ---- timeline bin kernels' block functions.  Every bin is folded by ONE warp (bins b = warp, warp + 8, ...): lanes
+// stride over the bin's rows / records, a fixed shuffle tree merges the lanes, lane 0 adds the result to the bin.  So
+// each fp64 sum has one fixed order and the same call gives the same bits.  The bins' row ranges come from one pass
+// that writes, for every bin b, the first row (record) whose bin is >= b -- which needs rows ordered by `delta`.
+__device__ __forceinline__ GsTlPart gs_tl_shfl_down(const GsTlPart &p, int o) {
+  GsTlPart q;
+  q.s = gs_sum_shfl_down(p.s, o);
+  q.dmin = __shfl_down_sync(0xffffffffu, p.dmin, o); q.dmax = __shfl_down_sync(0xffffffffu, p.dmax, o);
+  q.last = __shfl_down_sync(0xffffffffu, p.last, o); q.fin = __shfl_down_sync(0xffffffffu, p.fin, o);
+  return q;
+}
+
+__device__ __forceinline__ void gs_tl_warp_add(gs_tbin &t, GsTlPart &p) {
+  for (int o = 16; o > 0; o >>= 1) { const GsTlPart q = gs_tl_shfl_down(p, o); gs_tl_merge(p, q); }
+  if ((threadIdx.x & 31) == 0) gs_tl_add(t, p);
+}
+
+// Rows lo .. hi - 1 (rows[i - base], util may be NULL) into bins[0 .. B).  Rows whose `delta` never decreases take the
+// warp-per-bin path; otherwise thread 0 folds them in row order (gs_tl_fold_rows_serial).  Block-cooperative.
+__device__ void gs_tl_fold_rows(gs_tbin *bins, int B, long long W, const gs_tick_row *rows, const double *util, long long base,
+                                long long lo, long long hi) {
+  __shared__ int start[GS_TIMELINE_MAX_BINS + 1];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  int down = 0;
+  for (long long i = lo + 1 + threadIdx.x; i < hi; i += blockDim.x) down |= rows[i - base].now < rows[i - 1 - base].now;
+  if (__syncthreads_or(down)) {
+    if (threadIdx.x == 0) gs_tl_fold_rows_serial(bins, B, W, rows, util, base, lo, hi);
+    return;
+  }
+  for (int b = threadIdx.x; b <= B; b += blockDim.x) start[b] = (int)(hi - lo);
+  __syncthreads();
+  for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+    const int k = gs_tl_bin(rows[i - base].now, W, B), kp = i > lo ? gs_tl_bin(rows[i - 1 - base].now, W, B) : -1;
+    for (int b = kp + 1; b <= k; ++b) start[b] = (int)(i - lo);
+  }
+  __syncthreads();
+  for (int b = warp; b < B; b += nwarps) {
+    const long long s = lo + start[b], e = lo + start[b + 1];
+    if (s >= e) continue;                                   // (warp-uniform)
+    GsTlPart p;
+    gs_tl_zero(p);
+    for (long long i = s + lane; i < e; i += 32) gs_tl_row(p, rows[i - base], util ? util[i - base] : 0.0, i);
+    gs_tl_warp_add(bins[b], p);
+  }
+}
+
+// fifo: the window's records into bins[0 .. B), rows with `delta` <= wm skipped (gs_sum_fold_records' rows).  A record
+// covers the ticks now_k .. t_last_k; bin b takes the records from the first one with bin(t_last) >= b up to and
+// including the first one with bin(t_last) > b, each clipped to the bin's ticks with gs_sum_record -- a record that
+// straddles a boundary is split there.  The gs_qrow of a record with a queue is found by counting such records (the
+// pass that finds the ranges also stores each bin's count), checked, and searched for by `now` should it not match.
+__device__ void gs_tl_fold_records(gs_tbin *bins, int B, long long W, const gs_evrow *ev, int nev, const gs_qrow *qr, int nq,
+                                   long long ticks, long long wm) {
+  __shared__ int start[GS_TIMELINE_MAX_BINS + 1], qstart[GS_TIMELINE_MAX_BINS + 1];
+  __shared__ int warp_cnt[GS_SUM_THREADS / 32];
+  __shared__ int k0_sh;
+  if (ticks <= wm || nev == 0) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  auto t_last = [&](int k) -> long long { return k + 1 < nev ? (long long)ev[k + 1].now - 1 : ticks; };
+  if (threadIdx.x == 0) {                                   // first record with ticks past the watermark
+    int a = 0, z = nev - 1;
+    while (a < z) { const int mid = (a + z) >> 1; if (t_last(mid) > wm) z = mid; else a = mid + 1; }
+    k0_sh = a;
+  }
+  for (int b = threadIdx.x; b <= B; b += blockDim.x) { start[b] = nev; qstart[b] = 0; }
+  __syncthreads();
+  const int k0 = k0_sh;
+  int qbase = 0;
+  for (int t0 = 0; t0 < nev; t0 += blockDim.x) {
+    const int k = t0 + threadIdx.x;
+    const bool in = k < nev;
+    const bool hasq = in && ev[k].queued > 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, hasq);
+    if (lane == 0) warp_cnt[warp] = __popc(bal);
+    __syncthreads();
+    int off = __popc(bal & ((1u << lane) - 1u)), total = 0;
+    for (int w = 0; w < nwarps; ++w) { const int c = warp_cnt[w]; off += w < warp ? c : 0; total += c; }
+    __syncthreads();
+    if (in && k >= k0) {
+      const int kh = gs_tl_bin(t_last(k), W, B), kp = k > k0 ? gs_tl_bin(t_last(k - 1), W, B) : -1;
+      for (int b = kp + 1; b <= kh; ++b) { start[b] = k; qstart[b] = qbase + off; }
+    }
+    qbase += total;
+  }
+  __syncthreads();
+  for (int b = warp; b < B; b += nwarps) {
+    const int s = start[b];
+    if (s >= nev) continue;                                 // (warp-uniform)
+    const int e = start[b + 1] < nev - 1 ? start[b + 1] : nev - 1;
+    const long long b_lo = (long long)b * W, b_hi = b == B - 1 ? 0x7fffffffffffffffll : ((long long)b + 1) * W - 1;
+    GsTlPart p;
+    gs_tl_zero(p);
+    int qb = qstart[b];
+    for (int c = s; c <= e; c += 32) {
+      const int k = c + lane;
+      const bool in = k <= e;
+      gs_evrow rec;
+      if (in) rec = ev[k];
+      const bool hasq = in && rec.queued > 0;
+      const unsigned bal = __ballot_sync(0xffffffffu, hasq);
+      if (in) {
+        long long v_lo = rec.now > wm + 1 ? (long long)rec.now : wm + 1;
+        v_lo = v_lo > b_lo ? v_lo : b_lo;
+        const long long tl = t_last(k), v_hi = tl < b_hi ? tl : b_hi;
+        if (v_hi >= v_lo) {
+          long long arrive_sum = 0; int oldest = 0;
+          if (hasq) {
+            int qi = qb + __popc(bal & ((1u << lane) - 1u));
+            if (qi >= nq || qr[qi].now != rec.now) {
+              int a = 0, z = nq - 1;
+              while (a < z) { const int mid = (a + z) >> 1; if (qr[mid].now < rec.now) a = mid + 1; else z = mid; }
+              qi = a;
+            }
+            const gs_qrow q = qr[qi];
+            arrive_sum = q.arrive_sum; oldest = q.oldest_arrive;
+          }
+          gs_tl_record(p, rec, arrive_sum, oldest, v_lo, v_hi);
+        }
+      }
+      qb += __popc(bal);
+    }
+    gs_tl_warp_add(bins[b], p);
+  }
+}
+
+// util_sum of bins[0 .. B) = NaN (gs_summarize: the column is sampled on the host).  After the fold, block-cooperative.
+__device__ void gs_tl_util_nan(gs_tbin *bins, int B) {
+  __syncthreads();
+  for (int b = threadIdx.x; b < B; b += blockDim.x) bins[b].util_sum = __longlong_as_double(0x7ff8000000000000ll);
 }
 
 // Block reduction of N 64-bit values: the first NSUM are summed, the next NMIN take the minimum, the rest the maximum;

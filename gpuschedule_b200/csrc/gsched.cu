@@ -83,6 +83,8 @@ struct SimHost {
   bool trace_in_arena = false;
   int64_t sum_rows = 0;                   // gs_summarize: rows folded into the replica's accumulator (its watermark)
   bool sum_fresh = true;                  // the accumulator is to be zeroed before the next fold (the replica was prepared afresh)
+  bool tl_fresh = true;                   // gs_set_timeline: the bins are to be zeroed before the next fold
+  bool tl_done = false;                   // summarised with the timeline on since it was prepared
   SimDev dev;
   SimLayout layout;
 };
@@ -117,6 +119,8 @@ struct gs_engine {
   unsigned long long comm_epoch = 0, comm_epoch0 = 0;   // exchange counter: continues across runs / value at the last prepare
   bool dirty = true;       // host mirror of SimDev newer than device copy
   gs_summary *d_sum = nullptr;   // gs_summarize: one accumulator per replica
+  gs_tbin *d_tl = nullptr; size_t tl_bytes = 0;   // gs_set_timeline: nsims x tl_nbins bins
+  int64_t tl_width = 0; int tl_nbins = 0;
   // gs_boot_population: the records of the base trace, then its k - 1 gaps (int32)
   void *d_pop = nullptr; int64_t pop_k = 0; int64_t pop_max_gap = 0; double pop_max_need = 1.0;
 };
@@ -195,6 +199,7 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->h_stage) cudaFreeHost(h->h_stage);
   if (h->d_scratch) cudaFree(h->d_scratch);
   if (h->d_sum) cudaFree(h->d_sum);
+  if (h->d_tl) cudaFree(h->d_tl);
   if (h->d_pop) cudaFree(h->d_pop);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
   if (h->comm_buf) cudaFree(h->comm_buf);
@@ -524,6 +529,7 @@ static int bind_sim(gs_handle h, SimHost &s, const SimLayout &L, unsigned char *
   D.mem_busy = D.sum_arr = D.span_used = D.events = D.evals = D.started = D.ticks = D.row_first = 0;
   D.need_init = 1;
   s.sum_rows = 0; s.sum_fresh = true;
+  s.tl_fresh = true; s.tl_done = false;
   s.prepared = true;
   return GS_OK;
 }
@@ -1079,6 +1085,19 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_sum_rows_kernel(const SimDe
   }
 }
 
+// Timeline: the same rows as gs_sum_rows_kernel into the replica's bins.  Launched before it, so `acc[r].rows` is still
+// the watermark of the rows folded before this call.
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_tl_rows_kernel(const SimDev *sims, int first, const gs_summary *acc, gs_tbin *bins,
+                                                                    long long W, int B) {
+  const int r = first + blockIdx.x;
+  const SimDev &S = sims[r];
+  const long long wm = acc[r].rows;
+  gs_tbin *T = bins + (size_t)r * (size_t)B;
+  if (S.policy == GS_SCHED_FIFO) gs_tl_fold_records(T, B, W, S.evrows, S.nev, S.qrows, S.nq, S.ticks, wm);
+  else gs_tl_fold_rows(T, B, W, S.rows, nullptr, S.row_first, wm > S.row_first ? wm : S.row_first, S.ticks);
+  gs_tl_util_nan(T, B);
+}
+
 // The finished jobs as job.csv prints them (gs_expand_jobs_kernel for fifo, the job records otherwise).
 struct GsSumEngineJobs {
   const SimDev *sims;
@@ -1123,11 +1142,18 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
   const size_t pitch = (size_t)align_up((size_t)kmax, 64);
   int rc = ensure_scratch(h, 3 * sizeof(int) * pitch * (size_t)grid);
   if (rc) return rc;
+  const int B = h->tl_nbins;
   for (int i = first; i < first + count; ++i) {
     SimHost &s = h->sims[(size_t)i];
     if (s.sum_fresh) { CU(cudaMemsetAsync(h->d_sum + i, 0, sizeof(gs_summary), h->stream)); s.sum_fresh = false; }
+    if (B > 0 && s.tl_fresh) { CU(cudaMemsetAsync(h->d_tl + (size_t)i * B, 0, sizeof(gs_tbin) * (size_t)B, h->stream)); s.tl_fresh = false; }
   }
   CU(cudaEventRecord(h->e0, h->stream));
+  if (B > 0) {            // before gs_sum_rows_kernel, which advances the watermark
+    gs_tl_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->d_sum, h->d_tl, (long long)h->tl_width, B);
+    CU(cudaGetLastError());
+    h->launches += 1;
+  }
   gs_sum_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->d_sum);
   CU(cudaGetLastError());
   GsSumEngineJobs src{h->d_sims};
@@ -1140,7 +1166,47 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
   CU(cudaStreamSynchronize(h->stream));
   float ms = 0; cudaEventElapsedTime(&ms, h->e0, h->e1);
   if (kernel_ms) *kernel_ms = ms;
-  for (int i = first; i < first + count; ++i) h->sims[(size_t)i].sum_rows = out[i - first].rows;
+  for (int i = first; i < first + count; ++i) {
+    h->sims[(size_t)i].sum_rows = out[i - first].rows;
+    if (B > 0) h->sims[(size_t)i].tl_done = true;
+  }
+  return GS_OK;
+}
+
+extern "C" int gs_set_timeline(gs_handle h, int64_t bin_width, int32_t nbins) {
+  if (!h) return GS_ERR_ARG;
+  if (nbins < 0 || nbins > GS_TIMELINE_MAX_BINS || (nbins > 0 && (bin_width < 1 || bin_width > (1ll << 40))))
+    return fail(h, GS_ERR_ARG, "gs_set_timeline: nbins must be in 0..1024 and, when it is not 0, bin_width in 1..2^40");
+  for (const SimHost &s : h->sims)
+    if (s.prepared && !s.sum_fresh && s.sum_rows > 0)
+      return fail(h, GS_ERR_STATE, "gs_set_timeline: a replica has already folded rows (set the timeline before summarising a run, or after gs_reset)");
+  const size_t need = sizeof(gs_tbin) * (size_t)h->nsims * (size_t)nbins;
+  if (need > h->tl_bytes) {
+    CU(cudaSetDevice(h->device));
+    gs_tbin *d = nullptr;
+    CU(cudaMalloc(&d, need));
+    if (h->d_tl) { CU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_tl); }
+    h->d_tl = d; h->tl_bytes = need;
+  }
+  h->tl_width = nbins > 0 ? bin_width : 0;
+  h->tl_nbins = nbins;
+  for (SimHost &s : h->sims) { s.tl_fresh = true; s.tl_done = false; }
+  return GS_OK;
+}
+
+extern "C" int gs_fetch_timeline(gs_handle h, int first, int count, gs_tbin *out) {
+  if (!h) return GS_ERR_ARG;
+  if (first < 0 || count < 0 || first + count > h->nsims || (count > 0 && !out)) return fail(h, GS_ERR_ARG, "gs_fetch_timeline: bad arguments");
+  if (h->tl_nbins == 0) return fail(h, GS_ERR_STATE, "gs_fetch_timeline: the timeline is off (gs_set_timeline)");
+  for (int i = first; i < first + count; ++i) {
+    const SimHost &s = h->sims[(size_t)i];
+    if (!s.prepared || !s.tl_done) return fail(h, GS_ERR_STATE, "gs_fetch_timeline: a replica has not been summarised with the timeline on since it was prepared");
+  }
+  if (count == 0) return GS_OK;
+  CU(cudaSetDevice(h->device));
+  const size_t B = (size_t)h->tl_nbins;
+  CU(cudaMemcpyAsync(out, h->d_tl + (size_t)first * B, sizeof(gs_tbin) * B * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  CU(wait_stream(h));
   return GS_OK;
 }
 

@@ -10,6 +10,10 @@ log_manager: every number follows from the record and the cluster shape.
 
 `spread` takes many records of one configuration (bootstrap replicas, sweep.summarize_bootstrap) and gives, for the
 makespan and each derived number, the mean, the sample standard deviation and a nearest-rank percentile interval.
+
+Timelines (capi.TBIN_DTYPE bins from Engine.timeline / HorusEngine.timeline): `timeline_derived` gives the same kind
+of numbers per bin -- the curves the notebooks plot against `delta` -- and `timeline_spread` their spread per bin over
+the replicas that have rows in that bin (what groupby("delta").mean() averages over).
 """
 from __future__ import annotations
 
@@ -71,17 +75,17 @@ def spread(records, n_nodes, gpus_per_node, gpu_mem_cap_mib, level=0.95):
         cols["makespan"].append(float(rec["makespan"]))
         for m in SPREAD_METRICS[1:]:
             cols[m].append(d[m])
-    out = {}
-    for m, vals in cols.items():
-        v = np.asarray(vals, dtype=np.float64)
-        k = len(v)
-        if k == 0 or np.isnan(v).any():
-            out[m] = dict.fromkeys(SPREAD_STATS, math.nan)
-            continue
-        s = np.sort(v)
-        out[m] = dict(mean=float(v.mean()), std=float(v.std(ddof=1)) if k > 1 else math.nan,
-                      lo=float(s[nearest_rank((1 - level) / 2, k)]), hi=float(s[nearest_rank((1 + level) / 2, k)]))
-    return out
+    return {m: _spread_of(np.asarray(vals, dtype=np.float64), level) for m, vals in cols.items()}
+
+
+def _spread_of(v, level):
+    """mean, sample std and nearest-rank interval of the values v (level: a Fraction); NaN throughout if any is NaN"""
+    k = len(v)
+    if k == 0 or np.isnan(v).any():
+        return dict.fromkeys(SPREAD_STATS, math.nan)
+    s = np.sort(v)
+    return dict(mean=float(v.mean()), std=float(v.std(ddof=1)) if k > 1 else math.nan,
+                lo=float(s[nearest_rank((1 - level) / 2, k)]), hi=float(s[nearest_rank((1 + level) / 2, k)]))
 
 
 def spread_columns():
@@ -119,3 +123,98 @@ def flat(rec, n_nodes, gpus_per_node, gpu_mem_cap_mib):
         vals += [int(v) for v in rec[col]]
     d = derived(rec, n_nodes, gpus_per_node, gpu_mem_cap_mib)
     return vals + [d[k] for k in ("gpu_share", "mem_mean", "pending_mean", "wait_mean", "turnaround_mean", "jct_mean", "util_mean")]
+
+
+# ---------------------------------------------------------------- timelines
+TIMELINE_METRICS = ("gpu_share", "running_mean", "queued_mean", "mem_mean", "pending_mean_all", "pending_mean_nz", "pend_max",
+                    "util_mean", "finished_last")
+
+
+def _u128_float(lo, hi):
+    """float64 of 128-bit fields, elementwise (exactly rounded, as float(u128(lo, hi)))"""
+    lo, hi = np.asarray(lo, dtype=np.uint64), np.asarray(hi, dtype=np.uint64)
+    out = lo.astype(np.float64)
+    for idx in zip(*np.nonzero(hi)):
+        out[idx] = float(u128(lo[idx], hi[idx]))
+    return out
+
+
+def timeline_derived(bins, n_nodes, gpus_per_node, gpu_mem_cap_mib):
+    """Per-bin numbers of TBIN_DTYPE bins (any shape; every array has that shape).  NaN where a bin has no rows:
+        delta_min, delta_max   the bin's smallest / largest `delta` (its tick range)
+        rows                   its rows (int)
+        gpu_share              busy_gpus_sum / (rows * M * G)
+        running_mean, queued_mean   mean num_running_jobs / num_queuing_jobs
+        mem_mean               mean avg_gpu_memory_allocated
+        pending_mean_all       avg_pending_sum / rows: mean avg_pending_time over all rows (the time plots' curve)
+        pending_mean_nz        avg_pending_sum / pending_rows: over the rows where it is non-zero (the bar charts')
+        pend_max               max max_pending_time
+        util_mean              util_sum / rows (horus engine; NaN otherwise)
+        finished_last          jobs finished by the bin's last row"""
+    bins = np.asarray(bins)
+    rows = bins["rows"].astype(np.int64)
+    empty = rows == 0
+    r = np.where(empty, np.nan, rows.astype(np.float64))
+    mg = n_nodes * gpus_per_node
+    with np.errstate(invalid="ignore", divide="ignore"):
+        pr = bins["pending_rows"].astype(np.float64)
+        mem = _u128_float(bins["mem_busy_lo"], bins["mem_busy_hi"])
+        out = dict(
+            delta_min=np.where(empty, np.nan, bins["delta_min"].astype(np.float64)),
+            delta_max=np.where(empty, np.nan, bins["delta_max"].astype(np.float64)),
+            rows=rows,
+            gpu_share=bins["busy_gpus_sum"].astype(np.float64) / (r * mg),
+            running_mean=bins["running_sum"].astype(np.float64) / r,
+            queued_mean=bins["queued_sum"].astype(np.float64) / r,
+            mem_mean=mem / 1048576.0 / (mg * gpu_mem_cap_mib) / r,
+            pending_mean_all=bins["avg_pending_sum"] / r,
+            pending_mean_nz=np.where(pr > 0, bins["avg_pending_sum"] / np.where(pr > 0, pr, 1.0), np.nan),   # (empty bins have none)
+            pend_max=np.where(empty, np.nan, bins["pend_max_max"].astype(np.float64)),
+            util_mean=bins["util_sum"] / r,
+            finished_last=np.where(empty, np.nan, bins["finished_last"].astype(np.float64)),
+        )
+    return out
+
+
+def timeline_spread(bins, n_nodes, gpus_per_node, gpu_mem_cap_mib, level=0.95):
+    """Spread per bin across replicas: `bins` has shape (replicas, B).  For every bin, over the replicas that have rows
+    in it: {"replicas": int array (B,), metric: {mean, std, lo, hi: float arrays (B,)}} for every TIMELINE_METRICS
+    entry, with spread's rules (sample std, nearest-rank interval holding the central `level`; NaN throughout where a
+    value is NaN for any of those replicas or none has rows)."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    bins = np.asarray(bins)
+    if bins.ndim != 2:
+        raise ValueError("timeline_spread: bins must have shape (replicas, bins)")
+    d = timeline_derived(bins, n_nodes, gpus_per_node, gpu_mem_cap_mib)
+    reach = d["rows"] > 0
+    nb = bins.shape[1]
+    out = {"replicas": reach.sum(axis=0).astype(np.int64)}
+    for m in TIMELINE_METRICS:
+        cols = [_spread_of(d[m][reach[:, b], b], level) for b in range(nb)]
+        out[m] = {s: np.array([c[s] for c in cols], dtype=np.float64) for s in SPREAD_STATS}
+    return out
+
+
+def timeline_columns():
+    """names of the flat per-bin columns `timeline_flat` returns, in order"""
+    return ["delta_min", "delta_max", "rows"] + list(TIMELINE_METRICS)
+
+
+def timeline_flat(d, b):
+    """bin b of a timeline_derived dict as a list of Python values (ints for counts, NaN kept)"""
+    vals = []
+    for name in timeline_columns():
+        v = d[name][b]
+        vals.append(int(v) if name == "rows" or (name in ("delta_min", "delta_max", "pend_max", "finished_last") and not np.isnan(v))
+                    else float(v))
+    return vals
+
+
+def timeline_spread_columns():
+    return [f"{m}_{s}" for m in TIMELINE_METRICS for s in SPREAD_STATS]
+
+
+def timeline_spread_flat(sp, b):
+    return [float(sp[m][s][b]) for m in TIMELINE_METRICS for s in SPREAD_STATS]

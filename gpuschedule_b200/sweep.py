@@ -163,10 +163,28 @@ def run_batched(flag_sets, device=0, out_root="log"):
     return results
 
 
-def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16):
+def check_timeline(timeline):
+    """(bin width W, bins B) of a timeline argument, or ValueError"""
+    try:
+        W, B = (int(x) for x in timeline)
+    except (TypeError, ValueError):
+        raise ValueError("timeline: expected (bin width, bins)") from None
+    if not 1 <= W <= 2 ** 40:
+        raise ValueError("timeline: the bin width must be in 1..2^40 ticks")
+    if not 1 <= B <= capi.TIMELINE_MAX_BINS:
+        raise ValueError(f"timeline: the bin count must be in 1..{capi.TIMELINE_MAX_BINS}")
+    return W, B
+
+
+def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None):
     """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
     same configurations and random streams as run_batched, but no row or job record is read back and nothing is
-    written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus."""
+    written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus.
+    timeline=(W, B): also bin every replica's rows on the device (gs_set_timeline) and return (summaries,
+    TBIN_DTYPE bins of shape (len(flag_sets), B))."""
+    if timeline is not None:
+        W, B = check_timeline(timeline)
+        bins = np.zeros((len(flag_sets), B), dtype=capi.TBIN_DTYPE)
     out = np.zeros(len(flag_sets), dtype=capi.SUMMARY_DTYPE)
     aware = [i for i, fl in enumerate(flag_sets) if _is_utilisation_aware(fl)]
     plain = [i for i in range(len(flag_sets)) if i not in set(aware)]
@@ -174,13 +192,21 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16):
         sims = _horus_setup([flag_sets[i] for i in aware], chunk, rows_cap)
         with capi.HorusEngine(device=device, nsims=len(sims)) as eng:
             _horus_run(eng, sims, rows_cap)
+            if timeline is not None:
+                eng.set_timeline(W, B)
             out[aware] = eng.summarize()
+            if timeline is not None:
+                bins[aware] = eng.timeline()
     if plain:
         sims = _plain_setup([flag_sets[i] for i in plain])
         with capi.Engine(device=device, nsims=len(sims)) as eng:
             _plain_load(eng, sims)
+            if timeline is not None:
+                eng.set_timeline(W, B)
             out[plain] = eng.run_summarized()
-    return out
+            if timeline is not None:
+                bins[plain] = eng.timeline()
+    return out if timeline is None else (out, bins)
 
 
 def load_gap_scale(load):
@@ -203,7 +229,7 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n):
         raise ValueError(f"bootstrap: the utilisation-aware engine ({', '.join(sorted(set(aware)))}) has no generated traces")
 
 
-def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0):
+def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -213,10 +239,16 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
 
     One engine handle per base trace file.  A gittins replica takes its index table from the base trace (the
     replica's own trace never reaches the host).  Utilisation-aware configurations are an argument error, as are
-    replicas < 1 and non-positive loads; every argument is checked before a trace is read or an engine created."""
+    replicas < 1 and non-positive loads; every argument is checked before a trace is read or an engine created.
+    timeline=(W, B): also bin every replica's rows on the device and return (summaries, TBIN_DTYPE bins of shape
+    (len(flag_sets), len(loads), replicas, B))."""
     _check_bootstrap_args(flag_sets, replicas, loads, n)
+    if timeline is not None:
+        W, B = check_timeline(timeline)
     R, loads = int(replicas), [float(L) for L in loads]
     out = np.zeros((len(flag_sets), len(loads), R), dtype=capi.SUMMARY_DTYPE)
+    if timeline is not None:
+        bins = np.zeros((len(flag_sets), len(loads), R, B), dtype=capi.TBIN_DTYPE)
     by_trace = {}
     for c, fl in enumerate(flag_sets):
         by_trace.setdefault(fl.trace_file, []).append(c)
@@ -236,10 +268,15 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
                         i += 1
             eng.boot_population(base)
             eng.boot_traces(params)
+            if timeline is not None:
+                eng.set_timeline(W, B)
             recs = eng.run_summarized()
+            tl = eng.timeline() if timeline is not None else None
         for k, c in enumerate(configs):
             out[c] = recs[k * len(loads) * R:(k + 1) * len(loads) * R].reshape(len(loads), R)
-    return out
+            if tl is not None:
+                bins[c] = tl[k * len(loads) * R:(k + 1) * len(loads) * R].reshape(len(loads), R, B)
+    return out if timeline is None else (out, bins)
 
 
 def write_bootstrap_csv(path, flag_sets, loads, records):
@@ -271,6 +308,42 @@ def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95):
 
 
 SUMMARY_KEYS = ["trace", "scheme", "schedule", "num_buffer", "num_queue", "seed"]
+
+
+def _bin_bounds(b, W, B):
+    """first tick of bin b and the first tick after it ("inf" for the open-ended last bin)"""
+    return [b * W, "inf" if b == B - 1 else (b + 1) * W]
+
+
+def write_timeline_csv(path, flag_sets, bins, width):
+    """one line per (configuration, bin): the flags, the bin, its tick range and summary.timeline_derived's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["bin", "bin_start", "bin_end"] + summary.timeline_columns())
+        for fl, tb in zip(flag_sets, bins):
+            cl = Infrastructure(fl).gs_cluster()
+            d = summary.timeline_derived(tb, cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
+            for b in range(len(tb)):
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, b]
+                           + _bin_bounds(b, width, len(tb)) + summary.timeline_flat(d, b))
+
+
+def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95):
+    """one line per (configuration, load, bin): the flags, the load, the bin, its tick range, the number of replicas
+    with rows in it and summary.timeline_spread's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["load", "bin", "bin_start", "bin_end", "replicas", "level"] + summary.timeline_spread_columns())
+        for fl, per_load in zip(flag_sets, bins):
+            cl = Infrastructure(fl).gs_cluster()
+            shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
+            for L, tb in zip(loads, per_load):
+                sp = summary.timeline_spread(tb, *shape, level=level)
+                for b in range(tb.shape[1]):
+                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, b]
+                               + _bin_bounds(b, width, tb.shape[1]) + [int(sp["replicas"][b]), level] + summary.timeline_spread_flat(sp, b))
 
 
 def write_summary_csv(path, flag_sets, records):
@@ -306,7 +379,25 @@ def main(argv=None):
     ap.add_argument("--jobs", type=int, default=None, metavar="N", help="with --bootstrap: jobs per replica (default: the trace's)")
     ap.add_argument("--summary-ci", default=None, metavar="FILE",
                     help="with --bootstrap: one CSV line per (configuration, load) with the mean, std and 95%% interval across replicas")
+    ap.add_argument("--timeline", default=None, metavar="FILE",
+                    help="with --summary: also bin every run's rows by delta on the GPU and write one CSV line per (configuration, bin) "
+                         "to FILE; with --bootstrap one line per (configuration, load, bin) with the spread across replicas")
+    ap.add_argument("--bin-width", type=int, default=None, metavar="W", help="with --timeline: ticks of delta per bin")
+    ap.add_argument("--bins", type=int, default=None, metavar="B",
+                    help=f"with --timeline: bins (1..{capi.TIMELINE_MAX_BINS}, default 128); the last one is open-ended")
     a = ap.parse_args(argv)
+    timeline = None
+    if a.timeline is not None:
+        if not a.summary:
+            ap.error("--timeline needs --summary FILE")
+        if a.bin_width is None:
+            ap.error("--timeline needs --bin-width W")
+        try:
+            timeline = check_timeline((a.bin_width, 128 if a.bins is None else a.bins))
+        except ValueError as e:
+            ap.error(str(e))
+    elif a.bin_width is not None or a.bins is not None:
+        ap.error("--bin-width and --bins need --timeline FILE")
     if a.bootstrap is None and (a.load is not None or a.jobs is not None or a.summary_ci is not None):
         ap.error("--load, --jobs and --summary-ci need --bootstrap")
     if a.bootstrap is not None:
@@ -330,14 +421,21 @@ def main(argv=None):
             _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs)
         except ValueError as e:
             ap.error(str(e))
-        recs = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs)
+        recs = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline)
+        if timeline is not None:
+            recs, bins = recs
+            write_timeline_ci_csv(a.timeline, sets, loads, bins, timeline[0])
         write_bootstrap_csv(a.summary, sets, loads, recs)
         if a.summary_ci:
             write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs)
         print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads x {a.bootstrap} replicas")
         return
     if a.summary:
-        write_summary_csv(a.summary, sets, summarize_batched(sets))
+        recs = summarize_batched(sets, timeline=timeline)
+        if timeline is not None:
+            recs, bins = recs
+            write_timeline_csv(a.timeline, sets, bins, timeline[0])
+        write_summary_csv(a.summary, sets, recs)
         print(f"{a.summary}: {len(sets)} configurations")
         return
     for out_dir, st in run_batched(sets):

@@ -387,6 +387,37 @@ int gs_comm_set_min_runnable(gs_handle h, int k);
  * not summarised (nothing is changed then).  util_sum is NaN here.                                        */
 int gs_summarize(gs_handle h, int first, int count, gs_summary *out, double *kernel_ms);
 
+/* ---- binned time series of a run's rows (timeline) -----------------------------------------------------
+ * A timeline of bin width W >= 1 (ticks of `delta`) and B bins (1 <= B <= GS_TIMELINE_MAX_BINS) puts a row into bin
+ * min(floor(delta / W), B - 1) (a negative `delta` into bin 0): the last bin is open-ended, so the bins of a replica
+ * together hold exactly the rows its gs_summary holds.  A bin holds the row part of gs_summary restricted to its
+ * rows, the smallest and largest `delta` folded into it and the `finished` counter of its last row in row order.
+ * The fields of a bin without rows are 0 (util_sum: NaN from gs_summarize).  128 bytes.                    */
+#define GS_TIMELINE_MAX_BINS 1024
+typedef struct gs_tbin {
+  int64_t rows;
+  int64_t busy_gpus_sum, running_sum, queued_sum;
+  int32_t busy_gpus_max, running_max, queued_max, pend_max_max;
+  uint64_t pend_sum_lo, pend_sum_hi;   /* 128-bit, as in gs_summary */
+  uint64_t mem_busy_lo, mem_busy_hi;
+  int64_t pending_rows;
+  double avg_pending_sum;
+  double util_sum;
+  int64_t delta_min, delta_max;        /* the smallest / largest `delta` of the bin's rows                          */
+  int64_t finished_last;               /* `finished` of the bin's last row in row order                              */
+} gs_tbin;
+/* gs_set_timeline: while nbins > 0, every gs_summarize also folds the rows it folds (the same rows past the same
+ * watermark) into per-replica bins on the device; nbins = 0 (the default) turns the timeline off, and bin_width is
+ * then ignored.  Every replica starts again from zero bins.  GS_ERR_ARG for a bad width or count, GS_ERR_STATE when a
+ * replica has folded rows since it was last prepared (set the timeline before the first gs_summarize of a run, or
+ * after gs_reset); nothing changes on an error.
+ * gs_fetch_timeline copies count * nbins records (replica-major) as of the last gs_summarize (synchronous).
+ * GS_ERR_ARG for a bad range, GS_ERR_STATE when the timeline is off or a replica has not been summarised since it was
+ * prepared with the timeline on.  A replica prepared afresh (first gs_run, gs_reset, a new trace, gs_boot_traces)
+ * starts from zero bins.                                                                                   */
+int gs_set_timeline(gs_handle h, int64_t bin_width, int32_t nbins);
+int gs_fetch_timeline(gs_handle h, int first, int count, gs_tbin *out);
+
 /* ---- bootstrap replicas generated on the device ---------------------------------------------------------
  * gs_boot_population gives the handle one base trace P of k >= 1 records (admission order, the gs_load_trace rules;
  * validated once, copied to the device); D holds its k - 1 inter-arrival gaps D[i] = P[i+1].arrive_tick - P[i].arrive_tick.

@@ -99,6 +99,11 @@ int gs_horus_fetch(gs_horus_handle h, int32_t sim, gs_tick_row *rows, double *ut
  * kernel_ms (may be NULL) receives the device time of the summary kernels.  GS_ERR_ARG for a bad range,
  * GS_ERR_STATE for a replica that has not run. */
 int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t count, gs_summary *out, double *kernel_ms);
+/* Timeline (gs_tbin, gsched.h) filled by gs_horus_summarize from the same rows [0, ticks) with the sampled utilisation
+ * (util_sum).  gs_horus_summarize folds every row again on every call, so the timeline may be set at any time; setting
+ * it marks every replica as not summarised.  Errors as gs_set_timeline / gs_fetch_timeline.                 */
+int gs_horus_set_timeline(gs_horus_handle h, int64_t bin_width, int32_t nbins);
+int gs_horus_fetch_timeline(gs_horus_handle h, int32_t first, int32_t count, gs_tbin *out);
 /* Kernel mapping (no reference counterpart): simulations per warp, 1 (default: lane 0 of each warp) or 32; 0 = one
  * simulation per warp with all 32 lanes scoring a candidate job's devices together (gs_horus_coop_kernel). */
 int gs_horus_set_lanes(gs_horus_handle h, int lanes_per_warp);
