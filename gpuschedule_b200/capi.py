@@ -86,6 +86,15 @@ TBIN_DTYPE = np.dtype([("rows", "<i8"), ("busy_gpus_sum", "<i8"), ("running_sum"
                        ("delta_min", "<i8"), ("delta_max", "<i8"), ("finished_last", "<i8")])
 assert TBIN_DTYPE.itemsize == 128
 TIMELINE_MAX_BINS = 1024
+# gs_jclass (include/gsched.h): one job-size class of a replica's finished jobs -- gs_summary's job part restricted to
+# the class, with exact 128-bit sums of squares; CDF counts come separately as uint32 (replica, class, 3, E + 1)
+JCLASS_DTYPE = np.dtype([("jobs", "<i8"), ("wait_sum", "<i8"), ("turnaround_sum", "<i8"), ("jct_sum", "<i8"), ("preempt_sum", "<i8"),
+                         ("gpu_ticks_sum", "<i8"), ("wait_sq_lo", "<u8"), ("wait_sq_hi", "<u8"), ("turnaround_sq_lo", "<u8"),
+                         ("turnaround_sq_hi", "<u8"), ("jct_sq_lo", "<u8"), ("jct_sq_hi", "<u8"),
+                         ("wait_q", "<i4", (5,)), ("turnaround_q", "<i4", (5,)), ("jct_q", "<i4", (5,)), ("reserved", "<i4")])
+assert JCLASS_DTYPE.itemsize == 160
+JOBDIST_MAX_CLASSES = 8
+JOBDIST_MAX_EDGES = 255
 
 JOBIN_DTYPE = np.dtype([("arrive_tick", "<i4"), ("gpus", "<i4"), ("gpu_per_task", "<i4"), ("ps_count", "<i4"),
                         ("mem_bytes", "<i8"), ("duration", "<f8")])
@@ -191,7 +200,9 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_summarize.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, f64p]
     lib.gs_horus_set_timeline.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
     lib.gs_horus_fetch_timeline.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
-    for name in ("gs_horus_summarize", "gs_horus_set_timeline", "gs_horus_fetch_timeline", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
+    lib.gs_horus_set_jobdist.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
+    lib.gs_horus_fetch_jobdist.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    for name in ("gs_horus_summarize", "gs_horus_set_timeline", "gs_horus_fetch_timeline", "gs_horus_set_jobdist", "gs_horus_fetch_jobdist", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
                  "gs_horus_run", "gs_horus_stats", "gs_horus_fetch"):
         getattr(lib, name).restype = C.c_int
     return lib
@@ -254,8 +265,10 @@ def load_library():
     lib.gs_fetch_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.gs_set_timeline.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
     lib.gs_fetch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    lib.gs_set_jobdist.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
+    lib.gs_fetch_jobdist.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
-                 "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline"):
+                 "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
         getattr(lib, name).restype = C.c_int
     lib.gs_switch_yarn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, f64p, C.c_int64,
                                    C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_int64]
@@ -487,6 +500,15 @@ class HorusEngine:
         """TBIN_DTYPE bins of replicas [first, first+count) as of the last summarize(): shape (count, nbins)"""
         return _fetch_timeline(self, self.lib.gs_horus_fetch_timeline, "gs_horus_fetch_timeline", first, count)
 
+    def set_jobdist(self, bounds, edges):
+        """job statistics by job size, filled by every summarize(): len(bounds) + 1 classes by num_gpu, CDF counts at
+        `edges`; bounds=None turns it off (include/gsched_horus.h: gs_horus_set_jobdist)"""
+        _set_jobdist(self, self.lib.gs_horus_set_jobdist, "gs_horus_set_jobdist", bounds, edges)
+
+    def jobdist(self, first=0, count=None):
+        """(JCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3, E + 1)) as of the last summarize()"""
+        return _fetch_jobdist(self, self.lib.gs_horus_fetch_jobdist, "gs_horus_fetch_jobdist", first, count)
+
 
 def _fetch_timeline(eng, fn, what, first, count):
     count = eng.nsims - first if count is None else int(count)
@@ -494,6 +516,30 @@ def _fetch_timeline(eng, fn, what, first, count):
     out = np.zeros((max(count, 1), max(b, 1)), dtype=TBIN_DTYPE)
     eng._check(fn(eng.h, int(first), count, out.ctypes.data_as(C.c_void_p)), what)
     return out[:count, :b]
+
+
+def _set_jobdist(eng, fn, what, bounds, edges):
+    if bounds is None:
+        eng._check(fn(eng.h, 0, None, 0, None), what)
+        eng._jd_shape = (0, 0)
+        return
+    b = np.ascontiguousarray(np.asarray(bounds, dtype=np.int64).reshape(-1))
+    e = np.ascontiguousarray(np.asarray(edges, dtype=np.int64).reshape(-1))
+    if (b.size and (b.min() < -2 ** 31 or b.max() >= 2 ** 31)) or (e.size and (e.min() < -2 ** 31 or e.max() >= 2 ** 31)):
+        raise GsError(f"{what}: bounds and edges must be int32", GS_ERR_ARG)
+    b, e = b.astype(np.int32), e.astype(np.int32)
+    eng._check(fn(eng.h, len(b) + 1, b.ctypes.data_as(C.c_void_p) if len(b) else None, len(e),
+                  e.ctypes.data_as(C.c_void_p) if len(e) else None), what)
+    eng._jd_shape = (len(b) + 1, len(e))
+
+
+def _fetch_jobdist(eng, fn, what, first, count):
+    count = eng.nsims - first if count is None else int(count)
+    nc, ne = getattr(eng, "_jd_shape", (0, 0))
+    classes = np.zeros((max(count, 1), max(nc, 1)), dtype=JCLASS_DTYPE)
+    hist = np.zeros((max(count, 1), max(nc, 1), 3, ne + 1), dtype=np.uint32)
+    eng._check(fn(eng.h, int(first), count, classes.ctypes.data_as(C.c_void_p), hist.ctypes.data_as(C.c_void_p)), what)
+    return classes[:count, :nc], hist[:count, :nc]
 
 
 class Engine:
@@ -782,6 +828,17 @@ class Engine:
     def timeline(self, first=0, count=None):
         """TBIN_DTYPE bins of replicas [first, first+count) as of the last summarize(): shape (count, nbins)"""
         return _fetch_timeline(self, self.lib.gs_fetch_timeline, "gs_fetch_timeline", first, count)
+
+    def set_jobdist(self, bounds, edges):
+        """while set, every summarize() also computes per-replica job statistics by job size on the device:
+        len(bounds) + 1 classes (a job's class is the number of bounds <= its num_gpu) and CDF counts of wait /
+        turnaround / jct at `edges`; bounds=None turns it off.  May be called at any time (include/gsched.h: gs_set_jobdist)"""
+        _set_jobdist(self, self.lib.gs_set_jobdist, "gs_set_jobdist", bounds, edges)
+
+    def jobdist(self, first=0, count=None):
+        """(JCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3, E + 1)) of replicas [first, first+count)
+        as of the last summarize(); count[..., m, b] = #(value m <= edges[b]) - #(value m <= edges[b - 1])"""
+        return _fetch_jobdist(self, self.lib.gs_fetch_jobdist, "gs_fetch_jobdist", first, count)
 
     def run_summarized(self, rows_cap=0):
         """Run every replica to its exit condition, summarising after every launch and fetching no rows; returns

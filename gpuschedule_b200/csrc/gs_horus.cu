@@ -94,6 +94,7 @@ struct WordStream {                 // raw MT19937 words + the per-position samp
 struct HorusSimHost {
   bool configured = false, loaded = false, prepared = false;
   bool tl_done = false;             // summarised with the timeline on since it was prepared
+  bool jd_done = false;             // summarised with the current jobdist setting since it was prepared
   gs_cluster cl{};
   gs_horus_params par{};
   std::vector<HJob> jobs;
@@ -120,6 +121,9 @@ struct gs_horus_handle_s {
   int *d_sum_scratch = nullptr; size_t sum_scratch_bytes = 0;
   gs_tbin *d_tl = nullptr; size_t tl_bytes = 0;   // gs_horus_set_timeline: nsims x tl_nbins bins
   int64_t tl_width = 0; int tl_nbins = 0;
+  gs_jclass *d_jd = nullptr; size_t jd_bytes = 0;       // gs_horus_set_jobdist: nsims x C class records
+  unsigned *d_jd_hist = nullptr; size_t jd_hist_bytes = 0;   // and nsims x C x 3 x (E + 1) CDF counts
+  GsJdCfg jd{};                                          // jd.nclasses = 0: off
   std::string err;
   std::vector<double> shared;       // one stream consumed by every replica that did not get its own
   double *d_shared = nullptr; size_t shared_cap = 0; bool shared_dirty = false;
@@ -169,6 +173,8 @@ extern "C" int gs_horus_destroy(gs_horus_handle h) {
   if (h->d_sum) cudaFree(h->d_sum);
   if (h->d_sum_scratch) cudaFree(h->d_sum_scratch);
   if (h->d_tl) cudaFree(h->d_tl);
+  if (h->d_jd) cudaFree(h->d_jd);
+  if (h->d_jd_hist) cudaFree(h->d_jd_hist);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -358,7 +364,7 @@ static int prepare(gs_horus_handle h, HorusSimHost &s, long long rows_cap) {
   D.rows_cap = rows_cap;
   D.current_remaining = (long long)n; D.running_jobs = 0;
   s.rows_cap = rows_cap;
-  s.prepared = true; s.tl_done = false;
+  s.prepared = true; s.tl_done = false; s.jd_done = false;
   return GS_OK;
 }
 
@@ -464,6 +470,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   HCU(cudaMemsetAsync(h->d_sum + first, 0, sizeof(gs_summary) * (size_t)count, h->stream));
   const int B = h->tl_nbins;
   if (B > 0) HCU(cudaMemsetAsync(h->d_tl + (size_t)first * B, 0, sizeof(gs_tbin) * (size_t)B * (size_t)count, h->stream));
+  const int C = h->jd.nclasses;
 #ifdef __CUDACC__
   int per_sm = 1, sms = 132;
   HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_sum_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
@@ -483,6 +490,15 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
                                                                                       h->d_sum_scratch, (long long)pitch);
   HCU(cudaGetLastError());
   h->launches += 2;
+  if (C > 0) {            // after gs_sum_jobs_kernel, on the same scratch
+    int per_jd = 1;
+    HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_jd, gs_jd_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
+    const int grid_jd = std::min(grid, std::max(1, per_jd) * sms);
+    gs_jd_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid_jd, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->jd,
+                                                                                          h->d_jd, h->d_jd_hist, h->d_sum_scratch, (long long)pitch);
+    HCU(cudaGetLastError());
+    h->launches += 1;
+  }
   if (B > 0) {
     gs_htl_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->d_tl, (long long)h->tl_width, B);
     HCU(cudaGetLastError());
@@ -505,6 +521,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
       jobs[(size_t)i] = gs_sum_job(S.jobs[j].arrive, S.recs[j].start, S.recs[j].end, S.recs[j].jct, S.recs[j].preempt, S.jobs[j].gpus);
     }
     gs_sum_jobs_serial(jobs.data(), S.nfin, A);
+    if (C > 0) gs_jd_jobs_serial(jobs.data(), S.nfin, h->jd, h->d_jd + (size_t)r * C, h->d_jd_hist + (size_t)r * C * 3 * (h->jd.nedges + 1));
     if (B > 0) gs_tl_fold_rows_serial(h->d_tl + (size_t)r * B, B, (long long)h->tl_width, S.rows, S.util, 0, 0, S.ticks);
   }
   (void)kmax;
@@ -516,7 +533,10 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   HCU(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   if (kernel_ms) *kernel_ms = ms;
 #endif
-  if (B > 0) for (int i = first; i < first + count; ++i) h->sims[(size_t)i].tl_done = true;
+  for (int i = first; i < first + count; ++i) {
+    if (B > 0) h->sims[(size_t)i].tl_done = true;
+    if (C > 0) h->sims[(size_t)i].jd_done = true;
+  }
   return GS_OK;
 }
 
@@ -550,6 +570,52 @@ extern "C" int gs_horus_fetch_timeline(gs_horus_handle h, int32_t first, int32_t
   HCU(cudaSetDevice(h->device));
   const size_t B = (size_t)h->tl_nbins;
   HCU(cudaMemcpyAsync(out, h->d_tl + (size_t)first * B, sizeof(gs_tbin) * B * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
+  return GS_OK;
+}
+
+extern "C" int gs_horus_set_jobdist(gs_horus_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges) {
+  if (!h) return GS_ERR_ARG;
+  GsJdCfg cfg;
+  const char *why = nullptr;
+  if (!gs_jd_make_cfg(nclasses, bounds, nedges, edges, cfg, &why)) return hfail(h, GS_ERR_ARG, std::string("gs_horus_set_jobdist: ") + why);
+  const size_t need = sizeof(gs_jclass) * h->sims.size() * (size_t)cfg.nclasses;
+  const size_t need_hist = sizeof(unsigned) * h->sims.size() * (size_t)cfg.nclasses * 3 * (size_t)(cfg.nedges + 1);
+  if (need > h->jd_bytes || need_hist > h->jd_hist_bytes) {
+    HCU(cudaSetDevice(h->device));
+    gs_jclass *d = nullptr;
+    unsigned *dh = nullptr;
+    HCU(cudaMalloc(&d, std::max(need, h->jd_bytes)));
+    if (cudaMalloc(&dh, std::max(need_hist, h->jd_hist_bytes)) != cudaSuccess) {
+      cudaFree(d);
+      return hfail(h, GS_ERR_CUDA, "gs_horus_set_jobdist: cudaMalloc failed");
+    }
+    HCU(cudaStreamSynchronize(h->stream));
+    if (h->d_jd) cudaFree(h->d_jd);
+    if (h->d_jd_hist) cudaFree(h->d_jd_hist);
+    h->d_jd = d; h->jd_bytes = std::max(need, h->jd_bytes);
+    h->d_jd_hist = dh; h->jd_hist_bytes = std::max(need_hist, h->jd_hist_bytes);
+  }
+  h->jd = cfg;
+  for (auto &s : h->sims) s.jd_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t count, gs_jclass *classes_out, uint32_t *hist_out) {
+  if (!h) return GS_ERR_ARG;
+  const int nsims = (int)h->sims.size();
+  if (first < 0 || count < 0 || first > nsims - count) return hfail(h, GS_ERR_ARG, "gs_horus_fetch_jobdist: bad arguments");
+  if (h->jd.nclasses == 0) return hfail(h, GS_ERR_STATE, "gs_horus_fetch_jobdist: the job statistics are off (gs_horus_set_jobdist)");
+  for (int i = first; i < first + count; ++i)
+    if (!h->sims[(size_t)i].prepared || !h->sims[(size_t)i].jd_done)
+      return hfail(h, GS_ERR_STATE, "gs_horus_fetch_jobdist: a replica has not been summarised with this setting since it was prepared");
+  if (count == 0) return GS_OK;
+  HCU(cudaSetDevice(h->device));
+  const size_t C = (size_t)h->jd.nclasses, per = C * 3 * (size_t)(h->jd.nedges + 1);
+  if (classes_out)
+    HCU(cudaMemcpyAsync(classes_out, h->d_jd + (size_t)first * C, sizeof(gs_jclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  if (hist_out)
+    HCU(cudaMemcpyAsync(hist_out, h->d_jd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   HCU(cudaStreamSynchronize(h->stream));
   return GS_OK;
 }

@@ -239,6 +239,53 @@ GS_SUM_HD unsigned gs_sum_pick(const unsigned *hist, long long &rank) {
   return d;
 }
 
+// ---- job statistics by job size (gs_jclass, include/gsched.h)
+static_assert(sizeof(gs_jclass) == 160, "gs_jclass is 160 bytes");
+
+// A jobdist setting, passed to the kernel by value (1 KB of parameters; the edges are staged in shared memory).
+struct GsJdCfg {
+  int nclasses, nedges;
+  int bounds[GS_JOBDIST_MAX_CLASSES - 1];
+  int edges[GS_JOBDIST_MAX_EDGES];
+};
+
+// Class of a job with `gpus` GPUs: the number of the nb = C - 1 increasing bounds that are <= gpus.
+GS_SUM_HD int gs_jd_class(const int *bounds, int nb, int gpus) {
+  int c = 0;
+  while (c < nb && bounds[c] <= gpus) ++c;
+  return c;
+}
+
+// CDF bin of a value: #{i : edges[i] < v} over E increasing edges (binary search).
+GS_SUM_HD int gs_jd_bin(const int *edges, int E, int v) {
+  int lo = 0, hi = E;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (edges[mid] < v) lo = mid + 1; else hi = mid; }
+  return lo;
+}
+
+// A jobdist setting from the C ABI's arrays, or false (the message in *why) when it is not valid.
+static inline bool gs_jd_make_cfg(int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges, GsJdCfg &cfg, const char **why) {
+  *why = "nclasses must be in 0..8 and nedges in 0..255";
+  if (nclasses < 0 || nclasses > GS_JOBDIST_MAX_CLASSES || nedges < 0 || nedges > GS_JOBDIST_MAX_EDGES) return false;
+  cfg = GsJdCfg{};
+  if (nclasses == 0) return true;
+  *why = "a NULL array with a positive count";
+  if ((nclasses > 1 && !bounds) || (nedges > 0 && !edges)) return false;
+  *why = "the class bounds must be >= 1 and strictly increasing";
+  for (int i = 0; i < nclasses - 1; ++i)
+    if (bounds[i] < 1 || (i > 0 && bounds[i] <= bounds[i - 1])) return false;
+  *why = "the edges must be strictly increasing";
+  for (int i = 1; i < nedges; ++i)
+    if (edges[i] <= edges[i - 1]) return false;
+  cfg.nclasses = nclasses; cfg.nedges = nedges;
+  for (int i = 0; i < nclasses - 1; ++i) cfg.bounds[i] = bounds[i];
+  for (int i = 0; i < nedges; ++i) cfg.edges[i] = edges[i];
+  return true;
+}
+
+// v * v (< 2^62 for any int32 v) added to a 128-bit sum of squares.
+GS_SUM_HD void gs_jd_add_sq(uint64_t &lo, uint64_t &hi, int v) { gs_sum_add128(lo, hi, (gs_i128)((long long)v * v)); }
+
 #ifndef __CUDACC__
 // Host forms of the job part (the host-emulation build of gs_horus.cu, CPU tests): the same sums, and the same radix
 // select run serially, one target at a time.
@@ -277,6 +324,50 @@ static inline void gs_sum_jobs_serial(const GsSumJob *jobs, long long k, gs_summ
   gs_sum_select_serial(vals, k, s.wait_q);
   gs_sum_select_serial(vals + k, k, s.turnaround_q);
   gs_sum_select_serial(vals + 2 * k, k, s.jct_q);
+  delete[] vals;
+}
+
+// jobdist of k finished jobs: classes[0 .. C) and hist[C][3][E + 1] (overwritten).  The kernel's steps, serially:
+// count per class, write the values into per-class segments, fold each segment, select within it.
+static inline void gs_jd_jobs_serial(const GsSumJob *jobs, long long k, const GsJdCfg &cfg, gs_jclass *classes, uint32_t *hist) {
+  const int C = cfg.nclasses, nb = cfg.nedges + 1;
+  long long off[GS_JOBDIST_MAX_CLASSES + 1] = {0};
+  for (int c = 0; c < C; ++c) classes[c] = gs_jclass{};
+  for (long long i = 0; i < (long long)C * 3 * nb; ++i) hist[i] = 0;
+  for (long long i = 0; i < k; ++i) off[gs_jd_class(cfg.bounds, C - 1, jobs[i].gpus) + 1] += 1;
+  for (int c = 0; c < C; ++c) off[c + 1] += off[c];
+  const long long pitch = k > 0 ? k : 1;
+  int *vals = new int[(size_t)(3 * pitch)];
+  long long cur[GS_JOBDIST_MAX_CLASSES];
+  for (int c = 0; c < C; ++c) cur[c] = off[c];
+  for (long long i = 0; i < k; ++i) {
+    const GsSumJob &v = jobs[i];
+    const int c = gs_jd_class(cfg.bounds, C - 1, v.gpus);
+    gs_jclass &J = classes[c];
+    J.preempt_sum += v.preempt; J.gpu_ticks_sum += (long long)v.gpus * v.jct;
+    const long long pos = cur[c]++;
+    vals[pos] = v.wait; vals[pitch + pos] = v.turn; vals[2 * pitch + pos] = v.jct;
+  }
+  for (int c = 0; c < C; ++c) {
+    gs_jclass &J = classes[c];
+    const long long kc = off[c + 1] - off[c];
+    const int *seg = vals + off[c];
+    J.jobs = kc;
+    uint32_t *hc = hist + (size_t)c * 3 * nb;
+    for (long long i = 0; i < kc; ++i) {
+      const int w = seg[i], t = seg[pitch + i], j = seg[2 * pitch + i];
+      J.wait_sum += w; J.turnaround_sum += t; J.jct_sum += j;
+      gs_jd_add_sq(J.wait_sq_lo, J.wait_sq_hi, w);
+      gs_jd_add_sq(J.turnaround_sq_lo, J.turnaround_sq_hi, t);
+      gs_jd_add_sq(J.jct_sq_lo, J.jct_sq_hi, j);
+      hc[gs_jd_bin(cfg.edges, cfg.nedges, w)] += 1;
+      hc[nb + gs_jd_bin(cfg.edges, cfg.nedges, t)] += 1;
+      hc[2 * nb + gs_jd_bin(cfg.edges, cfg.nedges, j)] += 1;
+    }
+    gs_sum_select_serial(seg, kc, J.wait_q);
+    gs_sum_select_serial(seg + pitch, kc, J.turnaround_q);
+    gs_sum_select_serial(seg + 2 * pitch, kc, J.jct_q);
+  }
   delete[] vals;
 }
 #endif
@@ -517,6 +608,57 @@ __device__ void gs_sum_block_vec(long long (&v)[N]) {
   __syncthreads();
 }
 
+// Radix select of the 15 order statistics (3 value columns x 5 ranks) of k values per column, vals[m * pitch + i]
+// (i < k), whose column minima are mn[0 .. 3) and whose largest column range is `span`.  prefix[t] (shared) receives
+// target t's value minus its column's minimum; hist: GS_SUM_TARGETS * GS_SUM_BINS shared counters.  k = 0: no pass is
+// run and prefix is not to be read.  Block-cooperative: every thread calls it with the same arguments, and the
+// scratch writes it reads must be published by a barrier before the call.
+__device__ __forceinline__ void gs_sum_select(unsigned *hist, unsigned long long *prefix, const int *vals, long long pitch, long long k,
+                                              const long long *mn, long long span) {
+  __shared__ long long rank[GS_SUM_TARGETS];
+  __shared__ int leader[GS_SUM_TARGETS];
+  const int passes = k > 0 ? gs_sum_passes((unsigned long long)span) : 0;
+  if (threadIdx.x < GS_SUM_TARGETS) {
+    prefix[threadIdx.x] = 0;
+    rank[threadIdx.x] = k > 0 ? gs_sum_rank(gs_sum_permille(threadIdx.x % 5), k) : 0;
+  }
+  for (int p = 0; p < passes; ++p) {
+    const int shift = (passes - 1 - p) * 9;
+    for (int i = threadIdx.x; i < GS_SUM_TARGETS * GS_SUM_BINS; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    if (threadIdx.x < GS_SUM_TARGETS) {                    // targets of one value with the same prefix share a histogram
+      const int t = threadIdx.x, m0 = (t / 5) * 5;
+      int L = t;
+      for (int u = m0; u < t; ++u) if (prefix[u] == prefix[t]) { L = u; break; }
+      leader[t] = L;
+    }
+    __syncthreads();
+    for (long long i = threadIdx.x; i < k; i += blockDim.x) {
+#pragma unroll
+      for (int m = 0; m < 3; ++m) {
+        const unsigned long long u = (unsigned long long)((long long)vals[m * pitch + i] - mn[m]);
+        const unsigned long long hp = u >> (shift + 9);
+        const unsigned d = (unsigned)(u >> shift) & (GS_SUM_BINS - 1);
+        bool placed = false;
+#pragma unroll
+        for (int q = 0; q < 5; ++q) {
+          const int t = m * 5 + q;
+          if (!placed && leader[t] == t && prefix[t] == hp) { atomicAdd(&hist[t * GS_SUM_BINS + d], 1u); placed = true; }
+        }
+      }
+    }
+    __syncthreads();
+    if (threadIdx.x < GS_SUM_TARGETS) {
+      const int t = threadIdx.x;
+      long long rk = rank[t];
+      const unsigned d = gs_sum_pick(hist + leader[t] * GS_SUM_BINS, rk);
+      rank[t] = rk;
+      prefix[t] = (prefix[t] << 9) | d;
+    }
+    __syncthreads();
+  }
+}
+
 // Job part of replicas first .. first + count - 1, one block per replica in turn (grid-stride).  Src supplies
 // finished(r) and job(r, i), the i-th finished job in finish order.  scratch: 3 * pitch ints per block.
 template <class Src>
@@ -524,8 +666,6 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_sum_jobs_kernel(Src src, in
                                                                     int *scratch, long long pitch) {
   __shared__ unsigned hist[GS_SUM_TARGETS * GS_SUM_BINS];
   __shared__ unsigned long long prefix[GS_SUM_TARGETS];
-  __shared__ long long rank[GS_SUM_TARGETS];
-  __shared__ int leader[GS_SUM_TARGETS];
   int *vals = scratch + (size_t)blockIdx.x * 3 * (size_t)pitch;
   for (int b = blockIdx.x; b < count; b += gridDim.x) {
     const int r = first + b;
@@ -542,46 +682,7 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_sum_jobs_kernel(Src src, in
     long long span = 0;
 #pragma unroll
     for (int m = 0; m < 3; ++m) span = max(span, red[8 + m] - red[5 + m]);
-    const int passes = k > 0 ? gs_sum_passes((unsigned long long)span) : 0;
-    if (threadIdx.x < GS_SUM_TARGETS) {
-      prefix[threadIdx.x] = 0;
-      rank[threadIdx.x] = k > 0 ? gs_sum_rank(gs_sum_permille(threadIdx.x % 5), k) : 0;
-    }
-    for (int p = 0; p < passes; ++p) {
-      const int shift = (passes - 1 - p) * 9;
-      for (int i = threadIdx.x; i < GS_SUM_TARGETS * GS_SUM_BINS; i += blockDim.x) hist[i] = 0;
-      __syncthreads();
-      if (threadIdx.x < GS_SUM_TARGETS) {                  // targets of one value with the same prefix share a histogram
-        const int t = threadIdx.x, m0 = (t / 5) * 5;
-        int L = t;
-        for (int u = m0; u < t; ++u) if (prefix[u] == prefix[t]) { L = u; break; }
-        leader[t] = L;
-      }
-      __syncthreads();
-      for (long long i = threadIdx.x; i < k; i += blockDim.x) {
-#pragma unroll
-        for (int m = 0; m < 3; ++m) {
-          const unsigned long long u = (unsigned long long)((long long)vals[m * pitch + i] - red[5 + m]);
-          const unsigned long long hp = u >> (shift + 9);
-          const unsigned d = (unsigned)(u >> shift) & (GS_SUM_BINS - 1);
-          bool placed = false;
-#pragma unroll
-          for (int q = 0; q < 5; ++q) {
-            const int t = m * 5 + q;
-            if (!placed && leader[t] == t && prefix[t] == hp) { atomicAdd(&hist[t * GS_SUM_BINS + d], 1u); placed = true; }
-          }
-        }
-      }
-      __syncthreads();
-      if (threadIdx.x < GS_SUM_TARGETS) {
-        const int t = threadIdx.x;
-        long long rk = rank[t];
-        const unsigned d = gs_sum_pick(hist + leader[t] * GS_SUM_BINS, rk);
-        rank[t] = rk;
-        prefix[t] = (prefix[t] << 9) | d;
-      }
-      __syncthreads();
-    }
+    gs_sum_select(hist, prefix, vals, pitch, k, red + 5, span);
     if (threadIdx.x == 0) {
       gs_summary &A = acc[r];
       A.finished = k;
@@ -593,6 +694,115 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_sum_jobs_kernel(Src src, in
       }
     }
     __syncthreads();
+  }
+}
+
+// jobdist of replicas first .. first + count - 1 (the jobs of gs_sum_jobs_kernel, whose scratch it reuses), one block
+// per replica in turn (grid-stride): (1) per-class job counts and preempt / gpu-tick sums, kept in registers per class
+// and block-reduced; (2) class offsets; (3) every job's three values written to its class's segment of the scratch
+// through shared per-class cursors (warp-aggregated; the order inside a segment is free, nothing depends on it);
+// (4) per class in turn: sums, 128-bit sums of squares (as sums of 32-bit halves of the squares) and min / max
+// block-reduced, CDF counts by binary search over the shared edges into 3 * (E + 1) shared counters, then
+// (5) gs_sum_select over the segment.  Outputs: classes[r * C + c], hists[((r * C + c) * 3 + m) * (E + 1) + bin].
+template <class Src>
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_jd_jobs_kernel(Src src, int first, int count, GsJdCfg cfg, gs_jclass *classes,
+                                                                   unsigned *hists, int *scratch, long long pitch) {
+  __shared__ unsigned hist[GS_SUM_TARGETS * GS_SUM_BINS];
+  __shared__ unsigned long long prefix[GS_SUM_TARGETS];
+  __shared__ unsigned cdf[3 * (GS_JOBDIST_MAX_EDGES + 1)];
+  __shared__ int edges[GS_JOBDIST_MAX_EDGES];
+  __shared__ long long cls_sum[3][GS_JOBDIST_MAX_CLASSES];    // jobs, preempt_sum, gpu_ticks_sum per class
+  __shared__ long long cursor[GS_JOBDIST_MAX_CLASSES];
+  const int C = cfg.nclasses, E = cfg.nedges, nb = E + 1;
+  const int lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < E; i += blockDim.x) edges[i] = cfg.edges[i];
+  int *vals = scratch + (size_t)blockIdx.x * 3 * (size_t)pitch;
+  for (int b = blockIdx.x; b < count; b += gridDim.x) {
+    const int r = first + b;
+    const long long k = src.finished(r);
+    long long red[3 * GS_JOBDIST_MAX_CLASSES];
+#pragma unroll
+    for (int e = 0; e < 3 * GS_JOBDIST_MAX_CLASSES; ++e) red[e] = 0;
+    for (long long i = threadIdx.x; i < k; i += blockDim.x) {
+      const GsSumJob v = src.job(r, i);
+      const int c = gs_jd_class(cfg.bounds, C - 1, v.gpus);
+#pragma unroll
+      for (int u = 0; u < GS_JOBDIST_MAX_CLASSES; ++u) {
+        if (c == u) { red[u] += 1; red[GS_JOBDIST_MAX_CLASSES + u] += v.preempt; red[2 * GS_JOBDIST_MAX_CLASSES + u] += (long long)v.gpus * v.jct; }
+      }
+    }
+    gs_sum_block_vec<3 * GS_JOBDIST_MAX_CLASSES, 3 * GS_JOBDIST_MAX_CLASSES, 0>(red);
+    if (threadIdx.x < GS_JOBDIST_MAX_CLASSES) {
+      const int c = threadIdx.x;
+      long long off = 0;
+#pragma unroll
+      for (int u = 0; u < GS_JOBDIST_MAX_CLASSES; ++u) off += u < c ? red[u] : 0;
+#pragma unroll
+      for (int u = 0; u < GS_JOBDIST_MAX_CLASSES; ++u) {
+        if (u == c) { cls_sum[0][c] = red[u]; cls_sum[1][c] = red[GS_JOBDIST_MAX_CLASSES + u]; cls_sum[2][c] = red[2 * GS_JOBDIST_MAX_CLASSES + u]; }
+      }
+      cursor[c] = off;
+    }
+    __syncthreads();
+    for (long long i0 = 0; i0 < k; i0 += blockDim.x) {     // (warp-uniform trip count: the shuffles see full warps)
+      const long long i = i0 + threadIdx.x;
+      const bool in = i < k;
+      GsSumJob v;
+      int c = -1;
+      if (in) { v = src.job(r, i); c = gs_jd_class(cfg.bounds, C - 1, v.gpus); }
+      const unsigned peers = __match_any_sync(0xffffffffu, c);
+      const int head = __ffs(peers) - 1;
+      long long base = 0;
+      if (in && lane == head) base = atomicAdd((unsigned long long *)&cursor[c], (unsigned long long)__popc(peers));
+      base = __shfl_sync(0xffffffffu, base, head);
+      if (in) {
+        const long long pos = base + __popc(peers & ((1u << lane) - 1u));
+        vals[pos] = v.wait; vals[pitch + pos] = v.turn; vals[2 * pitch + pos] = v.jct;
+      }
+    }
+    __syncthreads();
+    long long off = 0;
+    for (int c = 0; c < C; ++c) {
+      const long long kc = cls_sum[0][c];
+      const int *seg = vals + off;
+      for (int i = threadIdx.x; i < 3 * nb; i += blockDim.x) cdf[i] = 0;
+      __syncthreads();
+      // sums; squares as the sums of their high and low 32-bit halves (each fits 64 bits); minima; maxima
+      long long s[15] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0x7fffffff, 0x7fffffff, 0x7fffffff, -0x80000000ll, -0x80000000ll, -0x80000000ll};
+      for (long long i = threadIdx.x; i < kc; i += blockDim.x) {
+#pragma unroll
+        for (int m = 0; m < 3; ++m) {
+          const int v = seg[m * pitch + i];
+          const unsigned long long sq = (unsigned long long)((long long)v * v);
+          s[m] += v; s[3 + m] += (long long)(sq >> 32); s[6 + m] += (long long)(sq & 0xffffffffull);
+          s[9 + m] = min(s[9 + m], (long long)v); s[12 + m] = max(s[12 + m], (long long)v);
+          atomicAdd(&cdf[m * nb + gs_jd_bin(edges, E, v)], 1u);
+        }
+      }
+      gs_sum_block_vec<15, 9, 3>(s);                        // (its barriers also publish the CDF counts)
+      unsigned *hout = hists + ((size_t)r * C + c) * 3 * (size_t)nb;
+      for (int i = threadIdx.x; i < 3 * nb; i += blockDim.x) hout[i] = cdf[i];
+      long long span = 0;
+#pragma unroll
+      for (int m = 0; m < 3; ++m) span = max(span, s[12 + m] - s[9 + m]);
+      gs_sum_select(hist, prefix, seg, pitch, kc, s + 9, span);
+      if (threadIdx.x == 0) {
+        gs_jclass J = {};
+        J.jobs = kc; J.wait_sum = s[0]; J.turnaround_sum = s[1]; J.jct_sum = s[2];
+        J.preempt_sum = cls_sum[1][c]; J.gpu_ticks_sum = cls_sum[2][c];
+        gs_sum_add128(J.wait_sq_lo, J.wait_sq_hi, ((gs_i128)s[3] << 32) + s[6]);
+        gs_sum_add128(J.turnaround_sq_lo, J.turnaround_sq_hi, ((gs_i128)s[4] << 32) + s[7]);
+        gs_sum_add128(J.jct_sq_lo, J.jct_sq_hi, ((gs_i128)s[5] << 32) + s[8]);
+        for (int t = 0; t < 5; ++t) {
+          J.wait_q[t] = kc > 0 ? (int)(s[9] + (long long)prefix[t]) : 0;
+          J.turnaround_q[t] = kc > 0 ? (int)(s[10] + (long long)prefix[5 + t]) : 0;
+          J.jct_q[t] = kc > 0 ? (int)(s[11] + (long long)prefix[10 + t]) : 0;
+        }
+        classes[(size_t)r * C + c] = J;
+      }
+      __syncthreads();
+      off += kc;
+    }
   }
 }
 

@@ -85,6 +85,7 @@ struct SimHost {
   bool sum_fresh = true;                  // the accumulator is to be zeroed before the next fold (the replica was prepared afresh)
   bool tl_fresh = true;                   // gs_set_timeline: the bins are to be zeroed before the next fold
   bool tl_done = false;                   // summarised with the timeline on since it was prepared
+  bool jd_done = false;                   // summarised with the current jobdist setting since it was prepared
   SimDev dev;
   SimLayout layout;
 };
@@ -121,6 +122,9 @@ struct gs_engine {
   gs_summary *d_sum = nullptr;   // gs_summarize: one accumulator per replica
   gs_tbin *d_tl = nullptr; size_t tl_bytes = 0;   // gs_set_timeline: nsims x tl_nbins bins
   int64_t tl_width = 0; int tl_nbins = 0;
+  gs_jclass *d_jd = nullptr; size_t jd_bytes = 0;       // gs_set_jobdist: nsims x C class records
+  unsigned *d_jd_hist = nullptr; size_t jd_hist_bytes = 0;   // and nsims x C x 3 x (E + 1) CDF counts
+  GsJdCfg jd{};                                          // jd.nclasses = 0: off
   // gs_boot_population: the records of the base trace, then its k - 1 gaps (int32)
   void *d_pop = nullptr; int64_t pop_k = 0; int64_t pop_max_gap = 0; double pop_max_need = 1.0;
 };
@@ -200,6 +204,8 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->d_scratch) cudaFree(h->d_scratch);
   if (h->d_sum) cudaFree(h->d_sum);
   if (h->d_tl) cudaFree(h->d_tl);
+  if (h->d_jd) cudaFree(h->d_jd);
+  if (h->d_jd_hist) cudaFree(h->d_jd_hist);
   if (h->d_pop) cudaFree(h->d_pop);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
   if (h->comm_buf) cudaFree(h->comm_buf);
@@ -529,7 +535,7 @@ static int bind_sim(gs_handle h, SimHost &s, const SimLayout &L, unsigned char *
   D.mem_busy = D.sum_arr = D.span_used = D.events = D.evals = D.started = D.ticks = D.row_first = 0;
   D.need_init = 1;
   s.sum_rows = 0; s.sum_fresh = true;
-  s.tl_fresh = true; s.tl_done = false;
+  s.tl_fresh = true; s.tl_done = false; s.jd_done = false;
   s.prepared = true;
   return GS_OK;
 }
@@ -1161,6 +1167,16 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
                                                                                        (long long)pitch);
   CU(cudaGetLastError());
   h->launches += 2;
+  const int C = h->jd.nclasses;
+  if (C > 0) {            // after gs_sum_jobs_kernel, on the same scratch
+    int per_jd = 1;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_jd, gs_jd_jobs_kernel<GsSumEngineJobs>, GS_SUM_THREADS, 0));
+    const int grid_jd = std::min(grid, std::max(1, per_jd) * sms);
+    gs_jd_jobs_kernel<GsSumEngineJobs><<<(unsigned)grid_jd, GS_SUM_THREADS, 0, h->stream>>>(src, first, count, h->jd, h->d_jd, h->d_jd_hist,
+                                                                                           (int *)h->d_scratch, (long long)pitch);
+    CU(cudaGetLastError());
+    h->launches += 1;
+  }
   CU(cudaEventRecord(h->e1, h->stream));
   CU(cudaMemcpyAsync(out, h->d_sum + first, sizeof(gs_summary) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
@@ -1169,6 +1185,7 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
   for (int i = first; i < first + count; ++i) {
     h->sims[(size_t)i].sum_rows = out[i - first].rows;
     if (B > 0) h->sims[(size_t)i].tl_done = true;
+    if (C > 0) h->sims[(size_t)i].jd_done = true;
   }
   return GS_OK;
 }
@@ -1206,6 +1223,53 @@ extern "C" int gs_fetch_timeline(gs_handle h, int first, int count, gs_tbin *out
   CU(cudaSetDevice(h->device));
   const size_t B = (size_t)h->tl_nbins;
   CU(cudaMemcpyAsync(out, h->d_tl + (size_t)first * B, sizeof(gs_tbin) * B * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  CU(wait_stream(h));
+  return GS_OK;
+}
+
+extern "C" int gs_set_jobdist(gs_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges) {
+  if (!h) return GS_ERR_ARG;
+  GsJdCfg cfg;
+  const char *why = nullptr;
+  if (!gs_jd_make_cfg(nclasses, bounds, nedges, edges, cfg, &why)) return fail(h, GS_ERR_ARG, std::string("gs_set_jobdist: ") + why);
+  const size_t need = sizeof(gs_jclass) * (size_t)h->nsims * (size_t)cfg.nclasses;
+  const size_t need_hist = sizeof(unsigned) * (size_t)h->nsims * (size_t)cfg.nclasses * 3 * (size_t)(cfg.nedges + 1);
+  if (need > h->jd_bytes || need_hist > h->jd_hist_bytes) {
+    CU(cudaSetDevice(h->device));
+    gs_jclass *d = nullptr;
+    unsigned *dh = nullptr;
+    CU(cudaMalloc(&d, std::max(need, h->jd_bytes)));
+    if (cudaMalloc(&dh, std::max(need_hist, h->jd_hist_bytes)) != cudaSuccess) {
+      cudaFree(d);
+      return fail(h, GS_ERR_CUDA, "gs_set_jobdist: cudaMalloc failed");
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    if (h->d_jd) cudaFree(h->d_jd);
+    if (h->d_jd_hist) cudaFree(h->d_jd_hist);
+    h->d_jd = d; h->jd_bytes = std::max(need, h->jd_bytes);
+    h->d_jd_hist = dh; h->jd_hist_bytes = std::max(need_hist, h->jd_hist_bytes);
+  }
+  h->jd = cfg;
+  for (SimHost &s : h->sims) s.jd_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_fetch_jobdist(gs_handle h, int first, int count, gs_jclass *classes_out, uint32_t *hist_out) {
+  if (!h) return GS_ERR_ARG;
+  if (first < 0 || count < 0 || first + count > h->nsims) return fail(h, GS_ERR_ARG, "gs_fetch_jobdist: bad arguments");
+  if (h->jd.nclasses == 0) return fail(h, GS_ERR_STATE, "gs_fetch_jobdist: the job statistics are off (gs_set_jobdist)");
+  for (int i = first; i < first + count; ++i) {
+    const SimHost &s = h->sims[(size_t)i];
+    if (!s.prepared || !s.jd_done)
+      return fail(h, GS_ERR_STATE, "gs_fetch_jobdist: a replica has not been summarised with this setting since it was prepared");
+  }
+  if (count == 0) return GS_OK;
+  CU(cudaSetDevice(h->device));
+  const size_t C = (size_t)h->jd.nclasses, per = C * 3 * (size_t)(h->jd.nedges + 1);
+  if (classes_out)
+    CU(cudaMemcpyAsync(classes_out, h->d_jd + (size_t)first * C, sizeof(gs_jclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  if (hist_out)
+    CU(cudaMemcpyAsync(hist_out, h->d_jd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(wait_stream(h));
   return GS_OK;
 }

@@ -14,6 +14,12 @@ makespan and each derived number, the mean, the sample standard deviation and a 
 Timelines (capi.TBIN_DTYPE bins from Engine.timeline / HorusEngine.timeline): `timeline_derived` gives the same kind
 of numbers per bin -- the curves the notebooks plot against `delta` -- and `timeline_spread` their spread per bin over
 the replicas that have rows in that bin (what groupby("delta").mean() averages over).
+
+Job statistics by job size (capi.JCLASS_DTYPE records and CDF counts from Engine.jobdist / HorusEngine.jobdist):
+`jobdist_derived` gives per class the job count, the mean, sample std (pandas' .std()) and five quantiles of wait,
+turnaround and jct, and their CDF at every edge -- job_analysis.ipynb's breakdown by used_gpus and
+scheduler_analysis.ipynb's mean / median / std -- and `jobdist_spread` their spread per class over the replicas that
+have jobs in that class.
 """
 from __future__ import annotations
 
@@ -218,3 +224,92 @@ def timeline_spread_columns():
 
 def timeline_spread_flat(sp, b):
     return [float(sp[m][s][b]) for m in TIMELINE_METRICS for s in SPREAD_STATS]
+
+
+# ---------------------------------------------------------------- job statistics by job size
+JOBDIST_QUANTITIES = ("wait", "turnaround", "jct")
+JOBDIST_STATS = ("mean", "std") + tuple(f"p{q}" for q in QUANTILES)
+JOBDIST_METRICS = tuple(f"{m}_{s}" for m in JOBDIST_QUANTITIES for s in JOBDIST_STATS)
+
+
+def _jclass_numbers(rec):
+    """the JOBDIST_METRICS of one JCLASS_DTYPE record as a dict of floats (NaN for an empty class; std NaN below two
+    jobs).  The sample variance (n * sumsq - sum^2) / (n * (n - 1)) is exact in Python ints and rounded once."""
+    n = int(rec["jobs"])
+    out = {}
+    for m in JOBDIST_QUANTITIES:
+        s, sq = int(rec[m + "_sum"]), u128(rec[m + "_sq_lo"], rec[m + "_sq_hi"])
+        out[m + "_mean"] = s / n if n else math.nan
+        out[m + "_std"] = math.sqrt(float(Fraction(n * sq - s * s, n * (n - 1)))) if n > 1 else math.nan
+        for q, v in zip(QUANTILES, rec[m + "_q"].tolist()):
+            out[f"{m}_p{q}"] = float(v) if n else math.nan
+    return out
+
+
+def jobdist_derived(classes, hist, edges):
+    """Per class of one replica: `classes` JCLASS_DTYPE (C,), `hist` CDF counts (C, 3, E + 1), `edges` the E edges.
+    Returns {"jobs": int array (C,), metric: float array (C,) for every JOBDIST_METRICS entry,
+    "<quantity>_cdf": float array (C, E) = #(value <= edge) / jobs}; NaN for an empty class."""
+    classes, hist = np.asarray(classes), np.asarray(hist, dtype=np.int64)
+    if classes.ndim != 1 or hist.shape != (len(classes), 3, len(edges) + 1):
+        raise ValueError("jobdist_derived: expected classes (C,) and hist (C, 3, len(edges) + 1)")
+    jobs = classes["jobs"].astype(np.int64)
+    out = {"jobs": jobs}
+    nums = [_jclass_numbers(rec) for rec in classes]
+    for name in JOBDIST_METRICS:
+        out[name] = np.array([d[name] for d in nums], dtype=np.float64)
+    cum = np.cumsum(hist, axis=2)[:, :, :len(edges)]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        for i, m in enumerate(JOBDIST_QUANTITIES):
+            out[m + "_cdf"] = np.where(jobs[:, None] > 0, cum[:, i, :] / np.where(jobs > 0, jobs, 1)[:, None], np.nan)
+    return out
+
+
+def jobdist_spread(classes, hist, edges, level=0.95):
+    """Spread per class across replicas: `classes` (replicas, C), `hist` (replicas, C, 3, E + 1).  For every class,
+    over the replicas that have at least one job in it: {"replicas": int array (C,), metric: {mean, std, lo, hi: float
+    arrays (C,)} for every JOBDIST_METRICS entry, "<quantity>_cdf": {mean, std, lo, hi: float arrays (C, E)}}, with
+    spread's rules (sample std, nearest-rank interval holding the central `level`, NaN where a value is NaN for any
+    of those replicas or no replica has jobs in the class)."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    classes, hist = np.asarray(classes), np.asarray(hist)
+    if classes.ndim != 2 or hist.shape != classes.shape + (3, len(edges) + 1):
+        raise ValueError("jobdist_spread: expected classes (replicas, C) and hist (replicas, C, 3, len(edges) + 1)")
+    per = [jobdist_derived(classes[r], hist[r], edges) for r in range(classes.shape[0])]
+    nc, ne = classes.shape[1], len(edges)
+    reach = classes["jobs"] > 0
+    out = {"replicas": reach.sum(axis=0).astype(np.int64)}
+    for name in JOBDIST_METRICS:
+        cols = [_spread_of(np.array([d[name][c] for r, d in enumerate(per) if reach[r, c]], dtype=np.float64), level) for c in range(nc)]
+        out[name] = {s: np.array([col[s] for col in cols], dtype=np.float64) for s in SPREAD_STATS}
+    for m in JOBDIST_QUANTITIES:
+        st = {s: np.full((nc, ne), math.nan) for s in SPREAD_STATS}
+        cdf = np.stack([d[m + "_cdf"] for d in per]) if per else np.zeros((0, nc, ne))
+        for c in range(nc):
+            sub = cdf[reach[:, c], c, :]
+            for e in range(ne):
+                sp = _spread_of(sub[:, e], level)
+                for s in SPREAD_STATS:
+                    st[s][c, e] = sp[s]
+        out[m + "_cdf"] = st
+    return out
+
+
+def jobdist_columns():
+    """names of the flat per-class columns `jobdist_flat` returns, in order"""
+    return ["jobs"] + list(JOBDIST_METRICS)
+
+
+def jobdist_flat(d, c):
+    """class c of a jobdist_derived dict as a list of Python values"""
+    return [int(d["jobs"][c])] + [float(d[name][c]) for name in JOBDIST_METRICS]
+
+
+def jobdist_spread_columns():
+    return [f"{name}_{s}" for name in JOBDIST_METRICS for s in SPREAD_STATS]
+
+
+def jobdist_spread_flat(sp, c):
+    return [float(sp[name][s][c]) for name in JOBDIST_METRICS for s in SPREAD_STATS]

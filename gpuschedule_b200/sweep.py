@@ -176,15 +176,43 @@ def check_timeline(timeline):
     return W, B
 
 
-def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None):
+DEFAULT_CDF_EDGES = tuple(2 ** i for i in range(31))
+
+
+def check_jobdist(jobdist):
+    """(class bounds, CDF edges) of a jobdist argument as tuples of ints, or ValueError"""
+    try:
+        bounds, edges = jobdist
+        bounds, edges = [int(x) for x in bounds], [int(x) for x in edges]
+    except (TypeError, ValueError):
+        raise ValueError("jobdist: expected (class bounds, CDF edges), two sequences of ints") from None
+    if len(bounds) > capi.JOBDIST_MAX_CLASSES - 1:
+        raise ValueError(f"jobdist: at most {capi.JOBDIST_MAX_CLASSES - 1} class bounds")
+    if any(b < 1 or b >= 2 ** 31 for b in bounds) or any(b <= a for a, b in zip(bounds, bounds[1:])):
+        raise ValueError("jobdist: the class bounds must be >= 1, int32 and strictly increasing")
+    if len(edges) > capi.JOBDIST_MAX_EDGES:
+        raise ValueError(f"jobdist: at most {capi.JOBDIST_MAX_EDGES} CDF edges")
+    if any(not -2 ** 31 <= e < 2 ** 31 for e in edges) or any(b <= a for a, b in zip(edges, edges[1:])):
+        raise ValueError("jobdist: the CDF edges must be int32 and strictly increasing")
+    return tuple(bounds), tuple(edges)
+
+
+def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None):
     """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
     same configurations and random streams as run_batched, but no row or job record is read back and nothing is
     written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus.
     timeline=(W, B): also bin every replica's rows on the device (gs_set_timeline) and return (summaries,
-    TBIN_DTYPE bins of shape (len(flag_sets), B))."""
+    TBIN_DTYPE bins of shape (len(flag_sets), B)).
+    jobdist=(bounds, edges): also compute every replica's job statistics by job size on the device (gs_set_jobdist)
+    and append (JCLASS_DTYPE records (len(flag_sets), C), CDF counts (len(flag_sets), C, 3, E + 1)) to the result."""
     if timeline is not None:
         W, B = check_timeline(timeline)
         bins = np.zeros((len(flag_sets), B), dtype=capi.TBIN_DTYPE)
+    if jobdist is not None:
+        jd_bounds, jd_edges = check_jobdist(jobdist)
+        nc = len(jd_bounds) + 1
+        jd_cls = np.zeros((len(flag_sets), nc), dtype=capi.JCLASS_DTYPE)
+        jd_hist = np.zeros((len(flag_sets), nc, 3, len(jd_edges) + 1), dtype=np.uint32)
     out = np.zeros(len(flag_sets), dtype=capi.SUMMARY_DTYPE)
     aware = [i for i, fl in enumerate(flag_sets) if _is_utilisation_aware(fl)]
     plain = [i for i in range(len(flag_sets)) if i not in set(aware)]
@@ -194,19 +222,28 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
             _horus_run(eng, sims, rows_cap)
             if timeline is not None:
                 eng.set_timeline(W, B)
+            if jobdist is not None:
+                eng.set_jobdist(jd_bounds, jd_edges)
             out[aware] = eng.summarize()
             if timeline is not None:
                 bins[aware] = eng.timeline()
+            if jobdist is not None:
+                jd_cls[aware], jd_hist[aware] = eng.jobdist()
     if plain:
         sims = _plain_setup([flag_sets[i] for i in plain])
         with capi.Engine(device=device, nsims=len(sims)) as eng:
             _plain_load(eng, sims)
             if timeline is not None:
                 eng.set_timeline(W, B)
+            if jobdist is not None:
+                eng.set_jobdist(jd_bounds, jd_edges)
             out[plain] = eng.run_summarized()
             if timeline is not None:
                 bins[plain] = eng.timeline()
-    return out if timeline is None else (out, bins)
+            if jobdist is not None:
+                jd_cls[plain], jd_hist[plain] = eng.jobdist()
+    res = (out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
+    return res[0] if len(res) == 1 else res
 
 
 def load_gap_scale(load):
@@ -229,7 +266,7 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n):
         raise ValueError(f"bootstrap: the utilisation-aware engine ({', '.join(sorted(set(aware)))}) has no generated traces")
 
 
-def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None):
+def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -241,14 +278,21 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     replica's own trace never reaches the host).  Utilisation-aware configurations are an argument error, as are
     replicas < 1 and non-positive loads; every argument is checked before a trace is read or an engine created.
     timeline=(W, B): also bin every replica's rows on the device and return (summaries, TBIN_DTYPE bins of shape
-    (len(flag_sets), len(loads), replicas, B))."""
+    (len(flag_sets), len(loads), replicas, B)).  jobdist=(bounds, edges): also append (JCLASS_DTYPE records
+    (len(flag_sets), len(loads), replicas, C), CDF counts (len(flag_sets), len(loads), replicas, C, 3, E + 1))."""
     _check_bootstrap_args(flag_sets, replicas, loads, n)
     if timeline is not None:
         W, B = check_timeline(timeline)
+    if jobdist is not None:
+        jd_bounds, jd_edges = check_jobdist(jobdist)
+        nc, nb = len(jd_bounds) + 1, len(jd_edges) + 1
     R, loads = int(replicas), [float(L) for L in loads]
     out = np.zeros((len(flag_sets), len(loads), R), dtype=capi.SUMMARY_DTYPE)
     if timeline is not None:
         bins = np.zeros((len(flag_sets), len(loads), R, B), dtype=capi.TBIN_DTYPE)
+    if jobdist is not None:
+        jd_cls = np.zeros((len(flag_sets), len(loads), R, nc), dtype=capi.JCLASS_DTYPE)
+        jd_hist = np.zeros((len(flag_sets), len(loads), R, nc, 3, nb), dtype=np.uint32)
     by_trace = {}
     for c, fl in enumerate(flag_sets):
         by_trace.setdefault(fl.trace_file, []).append(c)
@@ -270,13 +314,21 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
             eng.boot_traces(params)
             if timeline is not None:
                 eng.set_timeline(W, B)
+            if jobdist is not None:
+                eng.set_jobdist(jd_bounds, jd_edges)
             recs = eng.run_summarized()
             tl = eng.timeline() if timeline is not None else None
+            jd = eng.jobdist() if jobdist is not None else None
         for k, c in enumerate(configs):
-            out[c] = recs[k * len(loads) * R:(k + 1) * len(loads) * R].reshape(len(loads), R)
+            part = slice(k * len(loads) * R, (k + 1) * len(loads) * R)
+            out[c] = recs[part].reshape(len(loads), R)
             if tl is not None:
-                bins[c] = tl[k * len(loads) * R:(k + 1) * len(loads) * R].reshape(len(loads), R, B)
-    return out if timeline is None else (out, bins)
+                bins[c] = tl[part].reshape(len(loads), R, B)
+            if jd is not None:
+                jd_cls[c] = jd[0][part].reshape(len(loads), R, nc)
+                jd_hist[c] = jd[1][part].reshape(len(loads), R, nc, 3, nb)
+    res = (out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
+    return res[0] if len(res) == 1 else res
 
 
 def write_bootstrap_csv(path, flag_sets, loads, records):
@@ -346,6 +398,74 @@ def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95):
                                + _bin_bounds(b, width, tb.shape[1]) + [int(sp["replicas"][b]), level] + summary.timeline_spread_flat(sp, b))
 
 
+def _class_range(c, bounds):
+    """smallest and largest num_gpu of class c ("inf" for the open-ended last class)"""
+    return [bounds[c - 1] if c > 0 else 0, bounds[c] - 1 if c < len(bounds) else "inf"]
+
+
+def write_jobdist_csv(path, flag_sets, classes, hist, bounds, edges):
+    """one line per (configuration, class): the flags, the class, its num_gpu range and summary.jobdist_derived's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["class", "gpus_min", "gpus_max"] + summary.jobdist_columns())
+        for fl, cl, hs in zip(flag_sets, classes, hist):
+            d = summary.jobdist_derived(cl, hs, edges)
+            for c in range(len(cl)):
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, c] + _class_range(c, bounds)
+                           + summary.jobdist_flat(d, c))
+
+
+def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95):
+    """one line per (configuration, load, class): the flags, the load, the class, its num_gpu range, the number of
+    replicas with jobs in it and summary.jobdist_spread's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["load", "class", "gpus_min", "gpus_max", "replicas", "level"] + summary.jobdist_spread_columns())
+        for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
+            for L, cl, hs in zip(loads, per_cl, per_hs):
+                sp = summary.jobdist_spread(cl, hs, edges, level=level)
+                for c in range(cl.shape[1]):
+                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, c] + _class_range(c, bounds)
+                               + [int(sp["replicas"][c]), level] + summary.jobdist_spread_flat(sp, c))
+
+
+def write_jobdist_cdf_csv(path, flag_sets, classes, hist, bounds, edges):
+    """one line per (configuration, class, quantity, edge): the flags, the class, its num_gpu range, the quantity,
+    the edge, the class's jobs and the fraction of them with a value <= the edge"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["class", "gpus_min", "gpus_max", "quantity", "edge", "jobs", "cdf"])
+        for fl, cl, hs in zip(flag_sets, classes, hist):
+            d = summary.jobdist_derived(cl, hs, edges)
+            for c in range(len(cl)):
+                for m in summary.JOBDIST_QUANTITIES:
+                    for e, edge in enumerate(edges):
+                        w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, c] + _class_range(c, bounds)
+                                   + [m, edge, int(d["jobs"][c]), float(d[m + "_cdf"][c, e])])
+
+
+def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95):
+    """one line per (configuration, load, class, quantity, edge): the flags, the load, the class, its num_gpu range,
+    the quantity, the edge, the number of replicas with jobs in the class and the spread of the CDF value"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["load", "class", "gpus_min", "gpus_max", "quantity", "edge", "replicas", "level"]
+                   + [f"cdf_{s}" for s in summary.SPREAD_STATS])
+        for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
+            for L, cl, hs in zip(loads, per_cl, per_hs):
+                sp = summary.jobdist_spread(cl, hs, edges, level=level)
+                for c in range(cl.shape[1]):
+                    for m in summary.JOBDIST_QUANTITIES:
+                        for e, edge in enumerate(edges):
+                            w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, c]
+                                       + _class_range(c, bounds) + [m, edge, int(sp["replicas"][c]), level]
+                                       + [float(sp[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS])
+
+
 def write_summary_csv(path, flag_sets, records):
     """one line per configuration: its flags (SUMMARY_KEYS), the summary fields and the derived numbers (summary.py)"""
     import csv
@@ -385,7 +505,28 @@ def main(argv=None):
     ap.add_argument("--bin-width", type=int, default=None, metavar="W", help="with --timeline: ticks of delta per bin")
     ap.add_argument("--bins", type=int, default=None, metavar="B",
                     help=f"with --timeline: bins (1..{capi.TIMELINE_MAX_BINS}, default 128); the last one is open-ended")
+    ap.add_argument("--jobdist", default=None, metavar="FILE",
+                    help="with --summary: also compute job statistics by job size (num_gpu classes) on the GPU and write one CSV "
+                         "line per (configuration, class) to FILE; with --bootstrap one line per (configuration, load, class) "
+                         "with the spread across replicas")
+    ap.add_argument("--gpu-classes", type=int, nargs="+", default=None, metavar="B",
+                    help="with --jobdist: class bounds B1 < ... < Bk (a job's class is the number of bounds <= its num_gpu; "
+                         f"at most {capi.JOBDIST_MAX_CLASSES - 1}); default: one class")
+    ap.add_argument("--cdf-edges", type=int, nargs="+", default=None, metavar="E",
+                    help=f"with --jobdist: CDF edges in ticks (strictly increasing, at most {capi.JOBDIST_MAX_EDGES}; default 1 2 4 ... 2^30)")
+    ap.add_argument("--jobdist-cdf", default=None, metavar="FILE",
+                    help="with --jobdist: one CSV line per (configuration[, load], class, quantity, edge) with the CDF value or its spread")
     a = ap.parse_args(argv)
+    jobdist = None
+    if a.jobdist is not None:
+        if not a.summary:
+            ap.error("--jobdist needs --summary FILE")
+        try:
+            jobdist = check_jobdist((a.gpu_classes or (), DEFAULT_CDF_EDGES if a.cdf_edges is None else a.cdf_edges))
+        except ValueError as e:
+            ap.error(str(e))
+    elif a.gpu_classes is not None or a.cdf_edges is not None or a.jobdist_cdf is not None:
+        ap.error("--gpu-classes, --cdf-edges and --jobdist-cdf need --jobdist FILE")
     timeline = None
     if a.timeline is not None:
         if not a.summary:
@@ -421,20 +562,30 @@ def main(argv=None):
             _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs)
         except ValueError as e:
             ap.error(str(e))
-        recs = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline)
+        res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist)
+        recs, rest = (res, ()) if timeline is None and jobdist is None else (res[0], res[1:])
         if timeline is not None:
-            recs, bins = recs
-            write_timeline_ci_csv(a.timeline, sets, loads, bins, timeline[0])
+            write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0])
+        if jobdist is not None:
+            cls, hist = rest[-1]
+            write_jobdist_ci_csv(a.jobdist, sets, loads, cls, hist, *jobdist)
+            if a.jobdist_cdf:
+                write_jobdist_cdf_ci_csv(a.jobdist_cdf, sets, loads, cls, hist, *jobdist)
         write_bootstrap_csv(a.summary, sets, loads, recs)
         if a.summary_ci:
             write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs)
         print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads x {a.bootstrap} replicas")
         return
     if a.summary:
-        recs = summarize_batched(sets, timeline=timeline)
+        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist)
+        recs, rest = (res, ()) if timeline is None and jobdist is None else (res[0], res[1:])
         if timeline is not None:
-            recs, bins = recs
-            write_timeline_csv(a.timeline, sets, bins, timeline[0])
+            write_timeline_csv(a.timeline, sets, rest[0], timeline[0])
+        if jobdist is not None:
+            cls, hist = rest[-1]
+            write_jobdist_csv(a.jobdist, sets, cls, hist, *jobdist)
+            if a.jobdist_cdf:
+                write_jobdist_cdf_csv(a.jobdist_cdf, sets, cls, hist, *jobdist)
         write_summary_csv(a.summary, sets, recs)
         print(f"{a.summary}: {len(sets)} configurations")
         return

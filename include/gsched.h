@@ -418,6 +418,41 @@ typedef struct gs_tbin {
 int gs_set_timeline(gs_handle h, int64_t bin_width, int32_t nbins);
 int gs_fetch_timeline(gs_handle h, int first, int count, gs_tbin *out);
 
+/* ---- job statistics by job size (jobdist) ---------------------------------------------------------------
+ * The jobs are the finished jobs of gs_summary's job part, with the same wait = start - arrive, turnaround =
+ * end - arrive, jct, preempt and gpus (num_gpu).  C classes (1 <= C <= GS_JOBDIST_MAX_CLASSES) are given by C - 1
+ * strictly increasing bounds b_1 < ... < b_{C-1}, each >= 1: a job's class is the number of bounds <= gpus (bounds
+ * {5, 17, 65}: classes 1-4, 5-16, 17-64, 65+; C = 1: all jobs).  Per class, one gs_jclass: the class's part of
+ * gs_summary's job fields, exact 128-bit sums of squares, and the order statistics under gs_summary's rank rule
+ * (0 for an empty class).  With C = 1 the record equals the summary's job part field for field.
+ * CDF histogram: E strictly increasing edges e_0 < ... < e_{E-1} (0 <= E <= GS_JOBDIST_MAX_EDGES), one list for
+ * wait, turnaround and jct.  Per (class, quantity) E + 1 uint32 counts: value v goes to bin #{i : e_i < v}, so the
+ * count through bin b is #(v <= e_b), the right-continuous CDF at e_b.  Layout per replica [class][wait, turnaround,
+ * jct][bin].  Every field is an integer; a repeated call gives the same bytes.                                 */
+#define GS_JOBDIST_MAX_CLASSES 8
+#define GS_JOBDIST_MAX_EDGES 255
+typedef struct gs_jclass {
+  int64_t jobs;                                            /* finished jobs in the class                         */
+  int64_t wait_sum, turnaround_sum, jct_sum, preempt_sum, gpu_ticks_sum;   /* as in gs_summary                  */
+  uint64_t wait_sq_lo, wait_sq_hi;                         /* sums of squares, 128-bit                           */
+  uint64_t turnaround_sq_lo, turnaround_sq_hi;
+  uint64_t jct_sq_lo, jct_sq_hi;
+  int32_t wait_q[5], turnaround_q[5], jct_q[5];            /* 50 / 90 / 95 / 99 / 100 %, gs_summary's rank rule   */
+  int32_t reserved;
+} gs_jclass;
+/* gs_set_jobdist: while nclasses > 0, every gs_summarize also computes the class records and CDF histograms of the
+ * replicas it summarises (the job part is recomputed in full on every call, so this may be called at any time);
+ * nclasses = 0 (the default) turns it off, and the arrays are then ignored.  Every replica is marked as not
+ * summarised with this setting.  GS_ERR_ARG for nclasses outside 0..8, nedges outside 0..255, bounds that are not
+ * strictly increasing or below 1, edges that are not strictly increasing, or a NULL array with a positive count;
+ * nothing changes on an error.
+ * gs_fetch_jobdist copies count * C records and count * C * 3 * (E + 1) counts (replica-major; either output may be
+ * NULL) as of the last gs_summarize (synchronous).  GS_ERR_ARG for a bad range, GS_ERR_STATE when the feature is off
+ * or a replica has not been summarised since it was prepared (first gs_run, gs_reset, a new trace, gs_boot_traces)
+ * or since the last gs_set_jobdist.                                                                          */
+int gs_set_jobdist(gs_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges);
+int gs_fetch_jobdist(gs_handle h, int first, int count, gs_jclass *classes_out, uint32_t *hist_out);
+
 /* ---- bootstrap replicas generated on the device ---------------------------------------------------------
  * gs_boot_population gives the handle one base trace P of k >= 1 records (admission order, the gs_load_trace rules;
  * validated once, copied to the device); D holds its k - 1 inter-arrival gaps D[i] = P[i+1].arrive_tick - P[i].arrive_tick.

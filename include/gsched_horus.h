@@ -104,6 +104,10 @@ int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t count, gs_summa
  * it marks every replica as not summarised.  Errors as gs_set_timeline / gs_fetch_timeline.                 */
 int gs_horus_set_timeline(gs_horus_handle h, int64_t bin_width, int32_t nbins);
 int gs_horus_fetch_timeline(gs_horus_handle h, int32_t first, int32_t count, gs_tbin *out);
+/* Job statistics by job size (gs_jclass and CDF histograms, gsched.h) filled by gs_horus_summarize from the same
+ * finished jobs as its job part.  Same meaning and errors as gs_set_jobdist / gs_fetch_jobdist.                 */
+int gs_horus_set_jobdist(gs_horus_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges);
+int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t count, gs_jclass *classes_out, uint32_t *hist_out);
 /* Kernel mapping (no reference counterpart): simulations per warp, 1 (default: lane 0 of each warp) or 32; 0 = one
  * simulation per warp with all 32 lanes scoring a candidate job's devices together (gs_horus_coop_kernel). */
 int gs_horus_set_lanes(gs_horus_handle h, int lanes_per_warp);
