@@ -262,13 +262,14 @@ def load_library():
     lib.gs_summarize.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, f64p]
     lib.gs_boot_population.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
     lib.gs_boot_traces.argtypes = [C.c_void_p, C.c_void_p, f64p]
+    lib.gs_boot_traces_blocked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, f64p]
     lib.gs_fetch_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.gs_set_timeline.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
     lib.gs_fetch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     lib.gs_set_jobdist.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.gs_fetch_jobdist.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
-                 "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
+                 "gs_boot_traces_blocked", "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
         getattr(lib, name).restype = C.c_int
     lib.gs_switch_yarn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, f64p, C.c_int64,
                                    C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_int64]
@@ -662,14 +663,24 @@ class Engine:
         packed = np.ascontiguousarray(packed, dtype=JOBIN_DTYPE)
         self._check(self.lib.gs_boot_population(self.h, packed.ctypes.data_as(C.c_void_p), len(packed)), "gs_boot_population")
 
-    def boot_traces(self, params, with_time=False):
+    def boot_traces(self, params, with_time=False, block_len=None):
         """draw every replica's trace from the population: `params` holds one BOOT_PARAMS_DTYPE record per replica.
-        with_time: returns the generator's kernel milliseconds"""
+        block_len: the mean block length L of a block bootstrap (gs_boot_traces_blocked), one integer for every
+        replica or one per replica; None draws iid replicas (gs_boot_traces).  with_time: returns the generator's
+        kernel milliseconds"""
         params = np.ascontiguousarray(params, dtype=BOOT_PARAMS_DTYPE)
         if params.shape != (self.nsims,):
             raise ValueError(f"boot_traces: one parameter record per replica ({self.nsims}), got shape {params.shape}")
         ms = C.c_double(0.0)
-        self._check(self.lib.gs_boot_traces(self.h, params.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces")
+        if block_len is None:
+            self._check(self.lib.gs_boot_traces(self.h, params.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces")
+        else:
+            L = np.asarray(block_len)
+            if L.dtype.kind not in "iu" or L.shape not in ((), (self.nsims,)) or (L < 0).any() or (L > 2 ** 32 - 1).any():
+                raise ValueError(f"boot_traces: block_len must be one uint32 or one per replica ({self.nsims})")
+            L = np.ascontiguousarray(np.broadcast_to(L, (self.nsims,)), dtype=np.uint32)
+            self._check(self.lib.gs_boot_traces_blocked(self.h, params.ctypes.data_as(C.c_void_p), L.ctypes.data_as(C.c_void_p), C.byref(ms)),
+                        "gs_boot_traces_blocked")
         self._n = [int(k) for k in params["n"].tolist()]
         return ms.value if with_time else None
 

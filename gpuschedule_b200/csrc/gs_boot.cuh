@@ -9,13 +9,25 @@
 //   gap         g_0 = 0, g_j = D[floor(w1 * (K - 1) / 2^64)] (0 when K = 1)
 //   arrival     arrive_j = floor((g_0 + ... + g_j) * gap_num / gap_den), exact integers
 //   record      {arrive_j, P[r_j].gpus, P[r_j].gpu_per_task, 0, P[r_j].mem_bytes, P[r_j].duration}
-// w2 and w3 are unused.  The generator, the pick and the arithmetic are __host__ __device__: tests/emu/boot_emu.cpp
-// runs them with g++, and tracegen.bootstrap_packed is their numpy mirror.
+// w3 is unused, and so is w2 unless the replica is blocked.
+//
+// Blocked replicas (gs_boot_traces_blocked, the stationary bootstrap of Politis & Romano) resample runs of consecutive
+// jobs of geometric length with mean L, so that a trace's bursts survive.  Job 0 starts a block; job j > 0 starts one
+// iff floor(w2 * L / 2^64) == 0.  With b_j the last block start <= j and s_b = floor(w0_b * K / 2^64), job j copies
+//   row  r_j = (s_{b_j} + (j - b_j)) mod K
+//   gap  g_j = D[r_j - 1], the gap that preceded the row in the base trace, for a job that continues a block without
+//        wrapping (r_j > 0); the iid gap above for a block start or a wrapped row
+// With L = 1 every job starts a block, which is the iid bootstrap.  The generator, the picks and the arithmetic are
+// __host__ __device__: tests/emu/boot_emu.cpp and tests/emu/boot_block_emu.cpp run them with g++, and
+// tracegen.bootstrap_packed is their numpy mirror.
 //
 // gs_boot_kernel: one block per replica walks its jobs in chunks of the block size -- a Philox block per job, a gather
 // of the population row, a block-wide inclusive int64 scan of the gaps with a carry between chunks -- and writes the
 // chunk's 32-byte records through shared memory into the replica's slot of the trace arena with contiguous 16-byte
-// stores.  The same pass reduces the replica's span-pool bound (sum of min(tasks, M)) and last arrival tick.
+// stores.  The same pass reduces the replica's span-pool bound (sum of min(tasks, M)) and last arrival tick.  The
+// blocked instantiation first runs a block-wide inclusive max-scan of the key (j << 32) | s_j of every block start
+// (0 for other jobs), carried between chunks like the gap sum, so each job reads b_j and s_{b_j} from its scanned key
+// however many chunks and wraps of the population its block spans.
 #pragma once
 
 #include <stdint.h>
@@ -72,6 +84,28 @@ GS_BOOT_HD void gs_boot_pick(uint64_t seed, uint64_t stream, long long j, long l
   gap = (j > 0 && K > 1) ? (long long)gs_boot_mulhi(b.w[1], (uint64_t)(K - 1)) : -1;
 }
 
+// gs_boot_pick for a replica with mean block length L >= 1: row is s_j (the row a block starting at j begins with),
+// gap the iid gap index; returns whether job j starts a block.
+GS_BOOT_HD bool gs_boot_pick_blocked(uint64_t seed, uint64_t stream, long long j, long long K, uint64_t L, long long &row, long long &gap) {
+  const GsPhilox b = gs_boot_philox(seed, stream, (uint64_t)j + 1u, 0, 0, 0);
+  row = (long long)gs_boot_mulhi(b.w[0], (uint64_t)K);
+  gap = (j > 0 && K > 1) ? (long long)gs_boot_mulhi(b.w[1], (uint64_t)(K - 1)) : -1;
+  return j == 0 || gs_boot_mulhi(b.w[2], L) == 0;
+}
+
+// Scan key of job j: (j << 32) | s_j for a block start, 0 otherwise.  j and s_j are below 2^31, so the maximum over
+// jobs 0..j is the key of b_j (job 0's key is 0 when s_0 = 0, which decodes to the same b_j = 0, s = 0).
+GS_BOOT_HD long long gs_boot_block_key(bool start, long long j, long long s) { return start ? (j << 32) | s : 0; }
+
+// Row of job j from the scanned key of its block start: (s_b + (j - b)) mod K.  The sum stays below 2^32.
+GS_BOOT_HD long long gs_boot_block_row(long long key, long long j, long long K) {
+  const long long b = key >> 32, s = key & 0xffffffffll;
+  return (long long)((uint32_t)(s + (j - b)) % (uint32_t)K);
+}
+
+// Gap index of job j (-1: g_j = 0): the iid pick for a block start or a wrapped row, else the row's own preceding gap.
+GS_BOOT_HD long long gs_boot_block_gap(bool start, long long row, long long iid_gap) { return (start || row == 0) ? iid_gap : row - 1; }
+
 // arrive = floor(S * gap_num / gap_den) for a gap sum S >= 0.  The caller bounds S * gap_num below 2^62
 // (gs_boot_arrive_bound), so the product fits in 64 bits.
 GS_BOOT_HD int gs_boot_arrive(long long S, int gap_num, int gap_den) { return (int)(S * (long long)gap_num / gap_den); }
@@ -89,25 +123,51 @@ namespace {
 struct GsBootRep {        // one replica's parameters as the kernel reads them
   uint64_t seed, stream;
   long long n;
-  int gap_num, gap_den, M, pad;
+  int gap_num, gap_den, M;
+  uint32_t block_len;     // mean block length L (read by the blocked instantiation only)
 };
 
-// out[2 b] = sum over the jobs of min(tasks, M), out[2 b + 1] = last arrival tick (0 without jobs)
+// out[2 b] = sum over the jobs of min(tasks, M), out[2 b + 1] = last arrival tick (0 without jobs).
+// BLOCKED = false is the iid bootstrap; BLOCKED = true draws blocks of mean length R.block_len (1 gives the iid trace).
+template <bool BLOCKED>
 __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRep *reps, const JobIn *pop, const int *gaps, long long K,
                                                                  JobIn *arena, long long stride_recs, long long *out) {
   __shared__ int4 stage[2 * GS_BOOT_THREADS];
   __shared__ long long warp_tot[GS_BOOT_THREADS / 32];
+  __shared__ long long warp_key[BLOCKED ? GS_BOOT_THREADS / 32 : 1];
   __shared__ long long red[2][GS_BOOT_THREADS / 32];
   const GsBootRep R = reps[blockIdx.x];
   int4 *dst = reinterpret_cast<int4 *>(arena + stride_recs * (long long)blockIdx.x);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  long long carry = 0, spans = 0, last = 0;
+  long long carry = 0, spans = 0, last = 0, key_carry = 0;
   for (long long j0 = 0; j0 < R.n; j0 += blockDim.x) {
     const long long j = j0 + threadIdx.x;
     const bool in = j < R.n;
     long long g = 0;
     int4 lo = make_int4(0, 0, 0, 0), hi = make_int4(0, 0, 0, 0);
-    if (in) {
+    if constexpr (BLOCKED) {
+      long long s = 0, gi = -1;
+      bool start = false;
+      if (in) start = gs_boot_pick_blocked(R.seed, R.stream, j, K, R.block_len, s, gi);
+      long long key = gs_boot_block_key(start, j, s);   // inclusive max-scan: lanes, then warps, then the carry
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const long long y = __shfl_up_sync(0xffffffffu, key, o);
+        if (lane >= o) key = max(key, y);
+      }
+      if (lane == 31) warp_key[warp] = key;
+      __syncthreads();
+      long long before = key_carry;
+      for (int w = 0; w < nwarps; ++w) { const long long t = warp_key[w]; before = w < warp ? max(before, t) : before; key_carry = max(key_carry, t); }
+      key = max(key, before);
+      if (in) {                                        // warp_key is next written after the gap scan's barrier
+        const long long row = gs_boot_block_row(key, j, K);
+        const long long gj = gs_boot_block_gap(start, row, gi);
+        const int4 *src = reinterpret_cast<const int4 *>(pop + row);
+        lo = __ldg(src); hi = __ldg(src + 1);
+        if (gj >= 0) g = __ldg(gaps + gj);
+      }
+    } else if (in) {
       long long row, gi;
       gs_boot_pick(R.seed, R.stream, j, K, row, gi);
       const int4 *src = reinterpret_cast<const int4 *>(pop + row);

@@ -1306,12 +1306,17 @@ extern "C" int gs_boot_population(gs_handle h, const gs_jobin *trace, int64_t k)
 }
 
 extern "C" int gs_boot_traces(gs_handle h, const gs_boot_params *params, double *kernel_ms) {
+  return gs_boot_traces_blocked(h, params, nullptr, kernel_ms);
+}
+
+extern "C" int gs_boot_traces_blocked(gs_handle h, const gs_boot_params *params, const uint32_t *block_len, double *kernel_ms) {
   if (!h) return GS_ERR_ARG;
   if (!params) return fail(h, GS_ERR_ARG, "gs_boot_traces: params is NULL");
   if (!h->d_pop) return fail(h, GS_ERR_STATE, "gs_boot_traces: call gs_boot_population first");
   // every check before anything changes: a refused call leaves the replicas' traces as they were
   std::vector<GsBootRep> reps((size_t)h->nsims);
   int64_t nmax = 1;
+  bool blocked = false;                                 // some replica has L > 1: the blocked instantiation
   for (int i = 0; i < h->nsims; ++i) {
     const SimHost &s = h->sims[(size_t)i];
     const gs_boot_params &p = params[i];
@@ -1321,9 +1326,11 @@ extern "C" int gs_boot_traces(gs_handle h, const gs_boot_params *params, double 
     if (p.gap_num < 0 || p.gap_den < 1) return fail(h, GS_ERR_ARG, "gs_boot_traces: the gap scale needs gap_num >= 0 and gap_den >= 1");
     if (gs_boot_arrive_bound(p.n, h->pop_max_gap, p.gap_num, p.gap_den) >= 0x7fffffffll)
       return fail(h, GS_ERR_ARG, "gs_boot_traces: the last arrival tick can reach 2^31 - 1 (fewer jobs or a smaller gap scale)");
+    if (block_len && block_len[i] == 0) return fail(h, GS_ERR_ARG, "gs_boot_traces_blocked: block_len must be >= 1");
     GsBootRep &r = reps[(size_t)i];
     r.seed = p.seed; r.stream = p.stream; r.n = p.n; r.gap_num = p.gap_num; r.gap_den = p.gap_den;
-    r.M = s.cl.num_switch * s.cl.num_node_p_switch; r.pad = 0;
+    r.M = s.cl.num_switch * s.cl.num_node_p_switch; r.block_len = block_len ? block_len[i] : 1u;
+    blocked = blocked || r.block_len > 1;
     nmax = std::max(nmax, p.n);
   }
   CU(cudaSetDevice(h->device));
@@ -1338,8 +1345,9 @@ extern "C" int gs_boot_traces(gs_handle h, const gs_boot_params *params, double 
   const int *gaps = (const int *)((unsigned char *)h->d_pop + align_up(sizeof(JobIn) * (size_t)h->pop_k));
   CU(cudaMemcpyAsync(d, reps.data(), sizeof(GsBootRep) * reps.size(), cudaMemcpyHostToDevice, h->stream));
   CU(cudaEventRecord(h->e0, h->stream));
-  gs_boot_kernel<<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>((const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena,
-                                                                       (long long)(h->tarena_stride / sizeof(JobIn)), (long long *)(d + off_out));
+  (blocked ? gs_boot_kernel<true> : gs_boot_kernel<false>)<<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>(
+      (const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena, (long long)(h->tarena_stride / sizeof(JobIn)),
+      (long long *)(d + off_out));
   CU(cudaGetLastError());
   h->launches += 1;
   CU(cudaEventRecord(h->e1, h->stream));

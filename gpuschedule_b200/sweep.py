@@ -13,7 +13,7 @@ from fractions import Fraction
 
 import numpy as np
 
-from . import capi, rngcol, summary
+from . import capi, rngcol, summary, tracegen
 from .infrastructure import Infrastructure
 from .jobs import JobQueueManager, JobsManager
 from .log_manager import LogManager
@@ -252,7 +252,7 @@ def load_gap_scale(load):
     return f.numerator, f.denominator
 
 
-def _check_bootstrap_args(flag_sets, replicas, loads, n):
+def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1):
     if int(replicas) < 1:
         raise ValueError("bootstrap: replicas must be >= 1")
     if not len(loads) or not all(math.isfinite(float(L)) and float(L) > 0 for L in loads):
@@ -261,12 +261,16 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n):
         raise ValueError("bootstrap: a load is too small to be expressed as a gap scale")
     if n is not None and not 0 <= int(n) < 2 ** 31 - 64:
         raise ValueError("bootstrap: n out of range")
+    try:
+        tracegen.check_block_len(block_len)
+    except ValueError as e:
+        raise ValueError(f"bootstrap: {e}") from None
     aware = [fl.schedule for fl in flag_sets if _is_utilisation_aware(fl)]
     if aware:
         raise ValueError(f"bootstrap: the utilisation-aware engine ({', '.join(sorted(set(aware)))}) has no generated traces")
 
 
-def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None):
+def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -279,8 +283,12 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     replicas < 1 and non-positive loads; every argument is checked before a trace is read or an engine created.
     timeline=(W, B): also bin every replica's rows on the device and return (summaries, TBIN_DTYPE bins of shape
     (len(flag_sets), len(loads), replicas, B)).  jobdist=(bounds, edges): also append (JCLASS_DTYPE records
-    (len(flag_sets), len(loads), replicas, C), CDF counts (len(flag_sets), len(loads), replicas, C, 3, E + 1))."""
-    _check_bootstrap_args(flag_sets, replicas, loads, n)
+    (len(flag_sets), len(loads), replicas, C), CDF counts (len(flag_sets), len(loads), replicas, C, 3, E + 1)).
+    block_len=L > 1 draws every replica as a stationary block bootstrap with mean block length L
+    (gs_boot_traces_blocked): runs of consecutive jobs keep their order and the gaps between them, so a trace's bursts
+    survive resampling; the same replica index is coupled across values of L."""
+    _check_bootstrap_args(flag_sets, replicas, loads, n, block_len)
+    block_len = tracegen.check_block_len(block_len)
     if timeline is not None:
         W, B = check_timeline(timeline)
     if jobdist is not None:
@@ -311,7 +319,7 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
                         params[i] = (seed, r, jobs, num, den)
                         i += 1
             eng.boot_population(base)
-            eng.boot_traces(params)
+            eng.boot_traces(params, block_len=None if block_len == 1 else block_len)
             if timeline is not None:
                 eng.set_timeline(W, B)
             if jobdist is not None:
@@ -331,31 +339,42 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     return res[0] if len(res) == 1 else res
 
 
-def write_bootstrap_csv(path, flag_sets, loads, records):
-    """one line per (configuration, load, replica): replica, load, the configuration's flags, the summary columns"""
+def _block_col(block_len):
+    """the block_len column of the bootstrap files: none for iid replicas (block_len None)"""
+    return [] if block_len is None else ["block_len"]
+
+
+def _block_val(block_len):
+    return [] if block_len is None else [block_len]
+
+
+def write_bootstrap_csv(path, flag_sets, loads, records, block_len=None):
+    """one line per (configuration, load, replica): replica, load, block_len (with a block length), the
+    configuration's flags, the summary columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(["replica", "load"] + SUMMARY_KEYS + summary.columns())
+        w.writerow(["replica", "load"] + _block_col(block_len) + SUMMARY_KEYS + summary.columns())
         for fl, per_load in zip(flag_sets, records):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
             for L, recs in zip(loads, per_load):
                 for r, rec in enumerate(recs):
-                    w.writerow([r, L, fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + summary.flat(rec, *shape))
+                    w.writerow([r, L] + _block_val(block_len) + [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + summary.flat(rec, *shape))
 
 
-def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95):
-    """one line per (configuration, load): the flags, the load, the replica count and summary.spread's columns"""
+def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95, block_len=None):
+    """one line per (configuration, load): the flags, the load, block_len (with a block length), the replica count
+    and summary.spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load", "replicas", "level"] + summary.spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["replicas", "level"] + summary.spread_columns())
         for fl, per_load in zip(flag_sets, records):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
             for L, recs in zip(loads, per_load):
-                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, len(recs), level]
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L] + _block_val(block_len) + [len(recs), level]
                            + summary.spread_flat(summary.spread(recs, *shape, level=level)))
 
 
@@ -381,20 +400,20 @@ def write_timeline_csv(path, flag_sets, bins, width):
                            + _bin_bounds(b, width, len(tb)) + summary.timeline_flat(d, b))
 
 
-def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95):
-    """one line per (configuration, load, bin): the flags, the load, the bin, its tick range, the number of replicas
-    with rows in it and summary.timeline_spread's columns"""
+def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95, block_len=None):
+    """one line per (configuration, load, bin): the flags, the load, block_len (with a block length), the bin, its
+    tick range, the number of replicas with rows in it and summary.timeline_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load", "bin", "bin_start", "bin_end", "replicas", "level"] + summary.timeline_spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["bin", "bin_start", "bin_end", "replicas", "level"] + summary.timeline_spread_columns())
         for fl, per_load in zip(flag_sets, bins):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
             for L, tb in zip(loads, per_load):
                 sp = summary.timeline_spread(tb, *shape, level=level)
                 for b in range(tb.shape[1]):
-                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, b]
+                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L] + _block_val(block_len) + [b]
                                + _bin_bounds(b, width, tb.shape[1]) + [int(sp["replicas"][b]), level] + summary.timeline_spread_flat(sp, b))
 
 
@@ -416,19 +435,19 @@ def write_jobdist_csv(path, flag_sets, classes, hist, bounds, edges):
                            + summary.jobdist_flat(d, c))
 
 
-def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95):
-    """one line per (configuration, load, class): the flags, the load, the class, its num_gpu range, the number of
-    replicas with jobs in it and summary.jobdist_spread's columns"""
+def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None):
+    """one line per (configuration, load, class): the flags, the load, block_len (with a block length), the class, its
+    num_gpu range, the number of replicas with jobs in it and summary.jobdist_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load", "class", "gpus_min", "gpus_max", "replicas", "level"] + summary.jobdist_spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["class", "gpus_min", "gpus_max", "replicas", "level"] + summary.jobdist_spread_columns())
         for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
             for L, cl, hs in zip(loads, per_cl, per_hs):
                 sp = summary.jobdist_spread(cl, hs, edges, level=level)
                 for c in range(cl.shape[1]):
-                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, c] + _class_range(c, bounds)
-                               + [int(sp["replicas"][c]), level] + summary.jobdist_spread_flat(sp, c))
+                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L] + _block_val(block_len) + [c]
+                               + _class_range(c, bounds) + [int(sp["replicas"][c]), level] + summary.jobdist_spread_flat(sp, c))
 
 
 def write_jobdist_cdf_csv(path, flag_sets, classes, hist, bounds, edges):
@@ -447,13 +466,14 @@ def write_jobdist_cdf_csv(path, flag_sets, classes, hist, bounds, edges):
                                    + [m, edge, int(d["jobs"][c]), float(d[m + "_cdf"][c, e])])
 
 
-def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95):
-    """one line per (configuration, load, class, quantity, edge): the flags, the load, the class, its num_gpu range,
-    the quantity, the edge, the number of replicas with jobs in the class and the spread of the CDF value"""
+def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None):
+    """one line per (configuration, load, class, quantity, edge): the flags, the load, block_len (with a block
+    length), the class, its num_gpu range, the quantity, the edge, the number of replicas with jobs in the class and
+    the spread of the CDF value"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load", "class", "gpus_min", "gpus_max", "quantity", "edge", "replicas", "level"]
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["class", "gpus_min", "gpus_max", "quantity", "edge", "replicas", "level"]
                    + [f"cdf_{s}" for s in summary.SPREAD_STATS])
         for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
             for L, cl, hs in zip(loads, per_cl, per_hs):
@@ -461,8 +481,8 @@ def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edge
                 for c in range(cl.shape[1]):
                     for m in summary.JOBDIST_QUANTITIES:
                         for e, edge in enumerate(edges):
-                            w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L, c]
-                                       + _class_range(c, bounds) + [m, edge, int(sp["replicas"][c]), level]
+                            w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L]
+                                       + _block_val(block_len) + [c] + _class_range(c, bounds) + [m, edge, int(sp["replicas"][c]), level]
                                        + [float(sp[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS])
 
 
@@ -497,6 +517,9 @@ def main(argv=None):
     ap.add_argument("--load", type=float, nargs="+", default=None, metavar="L",
                     help="with --bootstrap: offered loads, the trace's inter-arrival gaps scaled by 1/L (default 1)")
     ap.add_argument("--jobs", type=int, default=None, metavar="N", help="with --bootstrap: jobs per replica (default: the trace's)")
+    ap.add_argument("--block-len", type=int, default=None, metavar="L",
+                    help="with --bootstrap: draw block bootstrap replicas with mean block length L (1..2^32 - 1), which keep runs "
+                         "of consecutive jobs and their gaps together; every output file gets a block_len column after load")
     ap.add_argument("--summary-ci", default=None, metavar="FILE",
                     help="with --bootstrap: one CSV line per (configuration, load) with the mean, std and 95%% interval across replicas")
     ap.add_argument("--timeline", default=None, metavar="FILE",
@@ -539,8 +562,8 @@ def main(argv=None):
             ap.error(str(e))
     elif a.bin_width is not None or a.bins is not None:
         ap.error("--bin-width and --bins need --timeline FILE")
-    if a.bootstrap is None and (a.load is not None or a.jobs is not None or a.summary_ci is not None):
-        ap.error("--load, --jobs and --summary-ci need --bootstrap")
+    if a.bootstrap is None and (a.load is not None or a.jobs is not None or a.summary_ci is not None or a.block_len is not None):
+        ap.error("--load, --jobs, --block-len and --summary-ci need --bootstrap")
     if a.bootstrap is not None:
         if not a.summary:
             ap.error("--bootstrap needs --summary FILE")
@@ -559,21 +582,23 @@ def main(argv=None):
     if a.bootstrap is not None:
         loads = a.load or [1.0]
         try:
-            _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs)
+            _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs, 1 if a.block_len is None else a.block_len)
         except ValueError as e:
             ap.error(str(e))
-        res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist)
+        bl = a.block_len
+        res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist,
+                                  block_len=1 if bl is None else bl)
         recs, rest = (res, ()) if timeline is None and jobdist is None else (res[0], res[1:])
         if timeline is not None:
-            write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0])
+            write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0], block_len=bl)
         if jobdist is not None:
             cls, hist = rest[-1]
-            write_jobdist_ci_csv(a.jobdist, sets, loads, cls, hist, *jobdist)
+            write_jobdist_ci_csv(a.jobdist, sets, loads, cls, hist, *jobdist, block_len=bl)
             if a.jobdist_cdf:
-                write_jobdist_cdf_ci_csv(a.jobdist_cdf, sets, loads, cls, hist, *jobdist)
-        write_bootstrap_csv(a.summary, sets, loads, recs)
+                write_jobdist_cdf_ci_csv(a.jobdist_cdf, sets, loads, cls, hist, *jobdist, block_len=bl)
+        write_bootstrap_csv(a.summary, sets, loads, recs, block_len=bl)
         if a.summary_ci:
-            write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs)
+            write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs, block_len=bl)
         print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads x {a.bootstrap} replicas")
         return
     if a.summary:

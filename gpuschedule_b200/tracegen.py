@@ -22,6 +22,8 @@ Distributions follow SURVEY.md section 8(d):
 """
 from __future__ import annotations
 
+import operator
+
 import numpy as np
 
 # Iteration-count sample of the reference's distribution-driven generator
@@ -110,16 +112,31 @@ def philox4x64(seed, stream, counters):
     return np.stack([c0, c1, c2, c3], axis=-1)
 
 
-def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1):
+def check_block_len(block_len):
+    """the mean block length L of a blocked bootstrap as an int in 1..2^32 - 1, or ValueError"""
+    if isinstance(block_len, (bool, np.bool_)):
+        raise ValueError("block_len must be an integer in 1..2^32 - 1")
+    try:
+        L = operator.index(block_len)
+    except TypeError:
+        raise ValueError("block_len must be an integer in 1..2^32 - 1") from None
+    if not 1 <= L <= 2 ** 32 - 1:
+        raise ValueError("block_len must be an integer in 1..2^32 - 1")
+    return L
+
+
+def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_len=1):
     """Replica (seed, stream) of `n` jobs drawn from `population` (JOBIN_DTYPE records of one trace in admission order):
     job j resamples a row and an inter-arrival gap of the population with the Philox4x64-10 block at counter
     (j + 1, 0, 0, 0), and its arrival is floor(gap sum * gap_num / gap_den) (include/gsched.h, gs_boot_traces).
-    Returns (JOBIN_DTYPE records, source rows)."""
+    block_len=L > 1 resamples blocks of consecutive rows of mean length L instead, each row with the gap that preceded
+    it in the population (gs_boot_traces_blocked); L = 1 is the iid bootstrap.  Returns (JOBIN_DTYPE records, source rows)."""
     from .capi import JOBIN_DTYPE
     pop = np.ascontiguousarray(population, dtype=JOBIN_DTYPE)
     k, n, gap_num, gap_den = len(pop), int(n), int(gap_num), int(gap_den)
     if k < 1 or not 0 <= n < 2 ** 31 - 64 or gap_num < 0 or gap_den < 1:
         raise ValueError("bootstrap_packed: needs a population of at least one record, 0 <= n < 2^31 - 64, gap_num >= 0, gap_den >= 1")
+    L = check_block_len(block_len)
     gaps = np.diff(pop["arrive_tick"].astype(np.int64))
     max_gap = int(gaps.max()) if len(gaps) else 0
     if n > 1 and (n - 1) * max_gap * gap_num // gap_den >= 2 ** 31 - 1:
@@ -128,9 +145,15 @@ def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1):
     ctr[:, 0] = np.arange(1, n + 1, dtype=np.uint64)
     w = philox4x64(seed, stream, ctr)
     rows = mulhi64(w[:, 0], np.uint64(k)).astype(np.int64)
+    j = np.arange(n, dtype=np.int64)
+    start = mulhi64(w[:, 2], np.uint64(L)) == 0                   # block starts; always for L = 1
+    start[:1] = True
+    b = np.maximum.accumulate(np.where(start, j, 0)) if n else j  # last block start <= j
+    rows = (rows[b] + (j - b)) % k
     g = np.zeros(n, dtype=np.int64)
     if k > 1 and n > 1:
-        g[1:] = gaps[mulhi64(w[1:, 1], np.uint64(k - 1)).astype(np.int64)]
+        gi = mulhi64(w[1:, 1], np.uint64(k - 1)).astype(np.int64)
+        g[1:] = gaps[np.where(start[1:] | (rows[1:] == 0), gi, rows[1:] - 1)]
     out = np.zeros(n, dtype=JOBIN_DTYPE)
     out["arrive_tick"] = np.cumsum(g) * gap_num // gap_den       # below 2^62 by the bound checked above
     src = pop[rows]
@@ -139,12 +162,12 @@ def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1):
     return out, rows
 
 
-def bootstrap_table(base_table, seed, stream, n, gap_num=1, gap_den=1):
+def bootstrap_table(base_table, seed, stream, n, gap_num=1, gap_den=1, block_len=1):
     """bootstrap_packed of a JobTable as a JobTable of its own (labels 0..n-1, the source rows' num_gpu_text and
     utilisation columns, submit = arrive), so that a generated replica can go through the ordinary upload path and
     the ordinary log writers."""
     from .ingest import JobTable
-    recs, rows = bootstrap_packed(base_table.packed(), seed, stream, n, gap_num, gap_den)
+    recs, rows = bootstrap_packed(base_table.packed(), seed, stream, n, gap_num, gap_den, block_len)
     pick = lambda a: None if a is None else np.ascontiguousarray(np.asarray(a)[rows])
     t = JobTable(
         n=len(recs), label=[str(i) for i in range(len(recs))],

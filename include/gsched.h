@@ -462,13 +462,20 @@ int gs_fetch_jobdist(gs_handle h, int first, int count, gs_jclass *classes_out, 
  *   {floor(S_j * gap_num / gap_den), P[r].gpus, P[r].gpu_per_task, 0, P[r].mem_bytes, P[r].duration}
  * with r = floor(w0 * k / 2^64), S_j = g_0 + ... + g_j, g_0 = 0, g_j = D[floor(w1 * (k - 1) / 2^64)] (0 when k = 1).
  * gap_num / gap_den = 1 / 1 keeps the base trace's arrival rate in expectation, 1 / 2 doubles the offered load; the same
- * (seed, stream) draws the same rows and gaps at every load (common random numbers).  Afterwards every replica is in the
- * state gs_load_traces_packed leaves (loaded, not prepared, span budget applied); kernel_ms (may be NULL) receives the
- * generator's device time.  gs_fetch_trace copies the n records of any resident trace of one replica (synchronous).
+ * (seed, stream) draws the same rows and gaps at every load (common random numbers).  w3 is unused, and w2 is used
+ * only by gs_boot_traces_blocked, which draws replica sim as a stationary block bootstrap with mean block length
+ * L = block_len[sim] (block_len NULL: L = 1 for all, exactly gs_boot_traces): job 0 starts a block, job j > 0 starts one
+ * iff floor(w2 * L / 2^64) == 0; with b the last block start <= j and s_b = floor(w0_b * k / 2^64), job j copies row
+ * r = (s_b + j - b) mod k, and its gap is D[r - 1] when j continues a block with r > 0, the iid gap above otherwise.
+ * L = 1 is the iid bootstrap, byte for byte; the same (seed, stream) is coupled across loads and values of L.
+ * Afterwards every replica is in the state gs_load_traces_packed leaves (loaded, not prepared, span budget applied);
+ * kernel_ms (may be NULL) receives the generator's device time.  gs_fetch_trace copies the n records of any resident
+ * trace of one replica (synchronous).
  * Errors (nothing changes): GS_ERR_ARG for a NULL argument, k < 1 or a record that breaks the load rules, n outside
- * gs_load_traces_packed's range, gap_num < 0 or gap_den < 1, a replica whose cluster has network costs, or a worst-case
- * last arrival floor((n - 1) * max(D) * gap_num / gap_den) of 2^31 - 1 or more; GS_ERR_STATE without a population, for
- * a replica not configured with gs_config_sim, or (gs_fetch_trace) for a replica that holds no trace.          */
+ * gs_load_traces_packed's range, gap_num < 0 or gap_den < 1, block_len[sim] == 0, a replica whose cluster has network
+ * costs, or a worst-case last arrival floor((n - 1) * max(D) * gap_num / gap_den) of 2^31 - 1 or more; GS_ERR_STATE
+ * without a population, for a replica not configured with gs_config_sim, or (gs_fetch_trace) for a replica that holds
+ * no trace.                                                                                                  */
 typedef struct gs_boot_params {
   uint64_t seed, stream;    /* Philox key                                                                     */
   int64_t n;                /* jobs                                                                           */
@@ -476,6 +483,8 @@ typedef struct gs_boot_params {
 } gs_boot_params;           /* 32 bytes */
 int gs_boot_population(gs_handle h, const gs_jobin *trace, int64_t k);
 int gs_boot_traces(gs_handle h, const gs_boot_params *params /* nsims */, double *kernel_ms);
+int gs_boot_traces_blocked(gs_handle h, const gs_boot_params *params /* nsims */, const uint32_t *block_len /* nsims; NULL = all 1 */,
+                           double *kernel_ms);
 int gs_fetch_trace(gs_handle h, int sim, gs_jobin *out /* n records */);
 
 /* Stateless candidate scoring: evaluate b jobs against ONE cluster state.

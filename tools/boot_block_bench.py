@@ -1,0 +1,104 @@
+"""Cost of block bootstrap replicas (gs_boot_traces_blocked) against iid replicas (gs_boot_traces).
+
+Workload: bench.py's fifo step -- replicas x 100k jobs on 4x32x8, span budget 1.5 -- on one handle, the population one
+fast_table trace of 100k jobs (bench.py's generator), replica r drawn with Philox key (seed, r) at the base trace's
+arrival rate.  Three loops, each gs_boot_traces[_blocked] -> gs_run -> gs_summarize, alternated step by step after
+warm-up (the order rotates every step):
+  iid     gs_boot_traces
+  L16     gs_boot_traces_blocked, mean block length 16 for every replica
+  L1024   gs_boot_traces_blocked, mean block length 1024
+Reports per loop the medians (and min / max) of the generator's, the engine's and the summary's kernel times, the
+wall-clock time per step, the engine's events and the mean wait over all replicas: blocked traces change the workload
+the engine sees, not only the generator.  A seeded sample of replicas of every loop is compared with
+tracegen.bootstrap_packed record for record.  The GPU's name and power limit are read in the same run.  Prints one
+JSON line."""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
+sys.path.insert(0, os.path.join(REPO, "tools"))
+
+from bench import BASE_SEED, fast_table  # noqa: E402  (the benchmark's own trace generator)
+from summary_bench import gpu_info  # noqa: E402
+
+LOOPS = (("iid", None), ("L16", 16), ("L1024", 1024))
+
+
+def step(eng, R, params, block_len):
+    """generate -> gs_run -> gs_summarize; (wall s, generator ms, engine ms, summary ms, events, wait sum, finished)"""
+    k0 = eng.stats(0).kernel_ms
+    t0 = time.perf_counter()
+    gen_ms = eng.boot_traces(params, with_time=True, block_len=block_len)
+    eng.run(0, 0)
+    out, sum_ms = eng.summarize(with_time=True)
+    wall = time.perf_counter() - t0
+    assert out["done"].all()
+    eng_ms = eng.stats(0).kernel_ms - k0
+    events = sum(int(eng.stats(i).events) for i in range(R))
+    return wall, gen_ms, eng_ms, sum_ms, events, int(out["wait_sum"].sum()), int(out["finished"].sum())
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--replicas", type=int, default=3696, help="as bench.py: the H100's 132 SMs x 28 resident warps")
+    ap.add_argument("--jobs", type=int, default=100000)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps of each loop")
+    ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--seed", type=int, default=1, help="Philox seed of the generated replicas")
+    ap.add_argument("--sample", type=int, default=4, help="replicas of each loop compared with the numpy mirror")
+    args = ap.parse_args()
+    from gpuschedule_b200 import capi, tracegen
+    R, n = args.replicas, args.jobs
+    gpu = gpu_info()
+    cluster = capi.make_cluster(4, 32, 8)
+    population = fast_table(n, BASE_SEED).packed()
+    params = np.zeros(R, dtype=capi.BOOT_PARAMS_DTYPE)
+    params["seed"], params["stream"], params["n"], params["gap_num"], params["gap_den"] = args.seed, np.arange(R), n, 1, 1
+
+    res = {name: [] for name, _ in LOOPS}
+    checked = 0
+    rng = np.random.default_rng(7)
+    with capi.Engine(device=0, nsims=R) as eng:
+        eng.set_async(True)
+        for i in range(R):
+            eng.config(i, cluster)
+        eng.set_span_budget(1.5)
+        eng.boot_population(population)
+        for s in range(args.warmup + args.steps):
+            for k in range(len(LOOPS)):
+                name, L = LOOPS[(s + k) % len(LOOPS)]
+                r = step(eng, R, params, L)
+                if s >= args.warmup:
+                    res[name].append(r)
+        for name, L in LOOPS:
+            eng.boot_traces(params, block_len=L)
+            for i in sorted(rng.choice(R, size=min(args.sample, R), replace=False).tolist()):
+                want = tracegen.bootstrap_packed(population, args.seed, i, n, block_len=1 if L is None else L)[0]
+                assert eng.fetch_trace(i).tobytes() == want.tobytes(), f"{name}: replica {i} differs from tracegen.bootstrap_packed"
+                checked += 1
+
+    def stat(name, k):
+        v = [r[k] for r in res[name]]
+        return {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))}
+    out = {"gpu": gpu, "workload": f"{n}-job traces x {R} replicas, 4x32x8, fifo+yarn (bench.py's step), span budget 1.5",
+           "steps": args.steps, "warmup": args.warmup}
+    for name, L in LOOPS:
+        last = res[name][-1]
+        out[name] = {"block_len": L, "generator_kernel_ms": stat(name, 1), "engine_kernel_ms": stat(name, 2),
+                     "summary_kernel_ms": stat(name, 3), "wall_ms_per_step": float(np.median([r[0] for r in res[name]]) * 1e3),
+                     "events_per_step": last[4], "mean_wait_ticks": last[5] / max(last[6], 1)}
+    out["checked_replicas"] = checked
+    out["gpu_after"] = gpu_info()
+    print(json.dumps(out), flush=True)
+
+
+if __name__ == "__main__":
+    main()
