@@ -267,6 +267,15 @@ __device__ __forceinline__ int warp_incl_scan(int v, int lane) {
   return v;
 }
 
+// exact int64 sum of one int per lane: 32 pending times can add up past 2^31 - 1 (the thread kernel and the oracle sum
+// into int64), so the warp sums the arithmetic high 16 bits and the low 16 bits apart; each partial sum stays below 2^21
+// in magnitude, so the 32-bit reductions cannot wrap
+__device__ __forceinline__ long long warp_sum_i64(int v) {
+  const int hi = __reduce_add_sync(FULL, v >> 16);
+  const unsigned lo = __reduce_add_sync(FULL, (unsigned)v & 0xffffu);
+  return (long long)hi * 65536 + (long long)lo;
+}
+
 __global__ void __launch_bounds__(32, GS_POLICY_MINBLOCKS) gs_dlas_warp_kernel(SimDev *sims, int nsims, long long max_ticks) {
   const int sim = blockIdx.x;
   const int lane = threadIdx.x;
@@ -452,6 +461,7 @@ __global__ void __launch_bounds__(32, GS_POLICY_MINBLOCKS) gs_dlas_warp_kernel(S
         if (flip_run) { r.status = PST_RUNNING; r.resume += 1; if (r.start < 0) r.start = event_time; pj[j] = r; }
         if (flip_pre) { r.status = PST_PENDING; pj[j] = r; }
         events += __popc(__ballot_sync(FULL, flip_run)) + __popc(__ballot_sync(FULL, flip_pre));
+        // the admitted GPUs of a chunk come out of free_gpu <= M * G <= 2^26 (check_cluster), so this int sum cannot wrap
         busy += __reduce_add_sync(FULL, admitted ? g : 0);
         {
           long long mc = admitted ? (long long)g * (jr.memb < cap_bytes ? jr.memb : cap_bytes) : 0;
@@ -505,7 +515,7 @@ __global__ void __launch_bounds__(32, GS_POLICY_MINBLOCKS) gs_dlas_warp_kernel(S
       running += __popc(__ballot_sync(FULL, valid && isrun));
       queued += __popc(__ballot_sync(FULL, valid && !isrun));
       pmax = max(pmax, __reduce_max_sync(FULL, pend));
-      psum += (long long)__reduce_add_sync(FULL, pend);
+      psum += warp_sum_i64(pend);
     }
     __syncwarp();
     if (lane == 0) {
@@ -768,7 +778,7 @@ __global__ void __launch_bounds__(32, GS_POLICY_MINBLOCKS) gs_sortpol_warp_kerne
       running += __popc(__ballot_sync(FULL, isrun_));                                                 \
       queued += __popc(__ballot_sync(FULL, (valid_) && !isrun_));                                     \
       pmax = max(pmax, __reduce_max_sync(FULL, pend_));                                               \
-      psum += (long long)__reduce_add_sync(FULL, pend_);                                              \
+      psum += warp_sum_i64(pend_);                                                                    \
     } while (0)
     if (sjf) {
       for (int nd = lane; nd < M; nd += 32) { nidle[nd] = G; nkfree[nd] = K; }
@@ -835,7 +845,7 @@ __global__ void __launch_bounds__(32, GS_POLICY_MINBLOCKS) gs_sortpol_warp_kerne
               for (int nb = 0; nb < M && cap < want; nb += 32) {
                 const int nd = nb + lane;
                 const int c = nd < M ? max(min(nidle[nd] / rhc, nkfree[nd]), 0) : 0;
-                cap += __reduce_add_sync(FULL, c);
+                cap += __reduce_add_sync(FULL, c);        // c <= G <= 64 per lane: the int sum cannot wrap
               }
               placed = (int)min((long long)rcount, cap / rtasks);
               long long todo = (long long)placed * rtasks;
@@ -860,6 +870,7 @@ __global__ void __launch_bounds__(32, GS_POLICY_MINBLOCKS) gs_sortpol_warp_kerne
         else if (valid && ok && r.start < 0) { r.start = event_time; pj[j] = r; }
         if (flip_pre) { r.status = PST_PENDING; pj[j] = r; }
         events += __popc(__ballot_sync(FULL, flip_run)) + __popc(__ballot_sync(FULL, flip_pre));
+        // placed jobs hold distinct devices, at most M * G <= 2^26 (check_cluster): this int sum cannot wrap
         busy += __reduce_add_sync(FULL, ok ? hg : 0);
         long long mc = ok ? (long long)hg * (memb < cap_bytes ? memb : cap_bytes) : 0;
         #pragma unroll
@@ -896,6 +907,7 @@ __global__ void __launch_bounds__(32, GS_POLICY_MINBLOCKS) gs_sortpol_warp_kerne
         if (flip_run) { r.status = PST_RUNNING; r.resume += 1; if (r.start < 0) r.start = event_time; pj[j] = r; }
         if (flip_pre) { r.status = PST_PENDING; pj[j] = r; }
         events += __popc(__ballot_sync(FULL, flip_run)) + __popc(__ballot_sync(FULL, flip_pre));
+        // the admitted GPUs of a chunk come out of free_gpu <= M * G <= 2^26 (check_cluster), so this int sum cannot wrap
         busy += __reduce_add_sync(FULL, admitted ? g : 0);
         long long mc = admitted ? (long long)g * (jr.memb < cap_bytes ? jr.memb : cap_bytes) : 0;
         #pragma unroll

@@ -3,9 +3,11 @@
 
     python tests/golden/fuzz_policy_reference.py [n_cases] [first_seed]
 
-Every case draws a random cluster, trace and policy parameters (sjf / dlas / dlas-gpu with 1..8 queues
-and random limits / gittins with a random service quantum), executes the reference's
-smallest_first_sim_jobs / dlas_sim_jobs / gittins_sim_jobs VERBATIM through make_policy_golden.py's stub
+Every case is policy_case(seed) of tests/test_policy_fuzz_cpu.py -- the generator of the GPU fuzz: 1 .. 64 GPUs
+per node, up to 140 nodes, slot-bound nodes, leaks, jobs wider than the cluster, bursts of arrivals, whole-tick and
+sub-tick durations, 1 .. 8 dlas queues with limits up to 2^31 + 6 * 10^9, gittins quanta -- at its full range of up to
+600 jobs (the reference runs such a case in well under a second, so no cap is needed) and with the gittins table the
+reference itself derives from the trace.  It executes the reference's smallest_first_sim_jobs / dlas_sim_jobs / gittins_sim_jobs VERBATIM through make_policy_golden.py's stub
 harness and compares every completion and every checkpoint with the C restatement.  A reference run
 that raises (its own list.remove / assertion failures on inputs outside its domain) is reported as
 "reference raised" and skipped.  Needs /root/reference, so it is NOT part of the suite; its last run is
@@ -13,9 +15,6 @@ recorded in DESIGN.md section 5.
 """
 import os
 import sys
-import tempfile
-
-import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
@@ -24,72 +23,45 @@ sys.path.insert(0, os.path.join(REPO, "tests"))
 sys.path.insert(0, HERE)
 
 import make_policy_golden as mpg  # noqa: E402
-from gpuschedule_b200 import capi, ingest, policies, tracegen  # noqa: E402
+from gpuschedule_b200 import capi, policies  # noqa: E402
 import oracle  # noqa: E402
+from test_policy_fuzz_cpu import policy_case  # noqa: E402
 from test_policy_golden import check_against_expected  # noqa: E402
 
 
-def random_case(seed):
-    rng = np.random.default_rng(seed)
-    policy = str(rng.choice(["sjf", "dlas", "dlas-gpu", "gittins"]))
-    G = int(rng.choice([2, 4, 8, 8]))
-    ckw = dict(num_switch=int(rng.integers(1, 3)), num_node_p_switch=int(rng.integers(1, 9)), num_gpu_p_node=G)
-    if policy == "sjf" and rng.random() < 0.5:
-        ckw.update(num_cpu_p_node=int(rng.choice([24, 60, 128])), mem_p_node=int(rng.choice([120, 300, 512])))
-    gpc = int(rng.choice([1, 1, 2])) if policy == "sjf" else 1
-    total = ckw["num_switch"] * ckw["num_node_p_switch"] * G
-    base = [1, 1, 2, 2, 3, 4, 6, 8, 12, 16]
-    choices = sorted(set(int(x) * gpc for x in rng.choice(base, size=4)))
-    if policy != "sjf":
-        choices = [c for c in choices if c <= total] or [1]      # GPU counting: a job wider than the cluster never runs
-    probs = rng.dirichlet(np.ones(len(choices)))
-    n = int(rng.integers(20, 200))
-    df = tracegen.synth_frame(n, seed=5000 + seed, rate=float(rng.choice([0.3, 0.8, 1.5, 3.0])), gpu_per_container=gpc,
-                              gpu_choices=choices, gpu_probs=probs,
-                              max_mem_mib=int(rng.choice([16384, 33000]))).drop(columns=["model"])
-    pkw = {}
-    if policy in ("dlas", "dlas-gpu"):
-        nq = int(rng.integers(1, 9))
-        lim = np.cumsum(rng.integers(2, 60 if policy == "dlas" else 300, size=nq - 1)).tolist()
-        pkw = dict(num_queue=nq, queue_limit=[int(x) for x in lim])
-    elif policy == "gittins":
-        pkw = dict(gittins_delta=int(rng.choice([5, 20, 60, 200, 3250])))
-    return policy, ckw, df, pkw
-
-
-def run_case(seed, workdir):
-    policy, ckw, df, pkw = random_case(seed)
-    trace = os.path.join(workdir, f"t{seed}.csv")
-    df.to_csv(trace, index=False)
-    table = ingest.JobTraceReader(trace).prepare_jobs().table(0.5)
+def run_case(seed):
+    """policy_case(seed) of tests/test_policy_fuzz_cpu.py (the cases the GPU fuzz runs), its gittins table rebuilt
+    from the trace: the reference derives that table from the trace itself (parse_job_dist)"""
+    case = policy_case(seed)
+    table = case.table
     try:
-        comp, chk, gtab, unfinished = mpg.run_reference_policy(table, ckw, policy, **pkw)
+        comp, chk, gtab, unfinished = mpg.run_reference_policy(table, case.ckw, case.name, **case.pkw)
     except Exception as e:                                           # noqa: BLE001 - the reference's own failures
-        return f"reference raised {type(e).__name__}: {e}"
-    kw = dict(pkw)
-    if policy == "gittins":
+        return case, f"reference raised {type(e).__name__}: {e}"
+    kw = dict(case.pkw)
+    if case.name == "gittins":
         kw["gittins_table"] = policies.build_gittins_table(policies.gittins_samples(table), kw.get("gittins_delta", 3250.0))
-    res = oracle.run_policy(capi.make_cluster(**ckw), capi.make_policy(policy, **kw), table)
+    res = oracle.run_policy(capi.make_cluster(**case.ckw), capi.make_policy(case.name, **kw), table)
     check_against_expected(table, res, {"completions": comp, "checkpoints": chk, "unfinished": unfinished})
-    return None
+    return case, None
 
 
 def main():
     n_cases = int(sys.argv[1]) if len(sys.argv) > 1 else 100
     first = int(sys.argv[2]) if len(sys.argv) > 2 else 0
     ok = raised = 0
-    with tempfile.TemporaryDirectory(prefix="gspolfuzz_") as wd:
-        for seed in range(first, first + n_cases):
-            try:
-                msg = run_case(seed, wd)
-            except AssertionError:
-                print(f"MISMATCH seed {seed}: {random_case(seed)[0]} {random_case(seed)[1]} {random_case(seed)[3]}")
-                raise
-            if msg:
-                raised += 1
-                print(f"seed {seed}: {msg}")
-            else:
-                ok += 1
+    for seed in range(first, first + n_cases):
+        try:
+            case, msg = run_case(seed)
+        except AssertionError:
+            case = policy_case(seed)
+            print(f"MISMATCH seed {seed}: {case.name} {case.ckw} {case.pkw} n={case.table.n}")
+            raise
+        if msg:
+            raised += 1
+            print(f"seed {seed} ({case.name} {case.ckw} {case.pkw}): {msg}")
+        else:
+            ok += 1
     print(f"{ok} cases identical, {raised} outside the reference's domain (it raised)")
 
 
