@@ -95,6 +95,12 @@ JCLASS_DTYPE = np.dtype([("jobs", "<i8"), ("wait_sum", "<i8"), ("turnaround_sum"
 assert JCLASS_DTYPE.itemsize == 160
 JOBDIST_MAX_CLASSES = 8
 JOBDIST_MAX_EDGES = 255
+# gs_jpair (include/gsched.h): one job-size class of a pair of replicas on the same trace -- per quantity (wait,
+# turnaround, jct) the per-job differences d = x_b - x_a over the jobs finished in both runs: counts by sign, exact
+# sums, 128-bit sums of squares, and the nearest-rank points of d ascending (q_hi) and descending (q_lo)
+JPAIR_DTYPE = np.dtype([("jobs", "<i8"), ("only_a", "<i8"), ("only_b", "<i8"), ("lt", "<i8", (3,)), ("eq", "<i8", (3,)), ("gt", "<i8", (3,)),
+                        ("d_sum", "<i8", (3,)), ("d_sq_lo", "<u8", (3,)), ("d_sq_hi", "<u8", (3,)), ("q_hi", "<i4", (3, 5)), ("q_lo", "<i4", (3, 5))])
+assert JPAIR_DTYPE.itemsize == 288
 
 JOBIN_DTYPE = np.dtype([("arrive_tick", "<i4"), ("gpus", "<i4"), ("gpu_per_task", "<i4"), ("ps_count", "<i4"),
                         ("mem_bytes", "<i8"), ("duration", "<f8")])
@@ -202,6 +208,9 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_fetch_timeline.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.gs_horus_set_jobdist.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.gs_horus_fetch_jobdist.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.gs_horus_compare.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, f64p]
+    lib.gs_horus_compare.restype = C.c_int
     for name in ("gs_horus_summarize", "gs_horus_set_timeline", "gs_horus_fetch_timeline", "gs_horus_set_jobdist", "gs_horus_fetch_jobdist", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
                  "gs_horus_run", "gs_horus_stats", "gs_horus_fetch"):
         getattr(lib, name).restype = C.c_int
@@ -268,6 +277,9 @@ def load_library():
     lib.gs_fetch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     lib.gs_set_jobdist.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.gs_fetch_jobdist.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.gs_compare.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                               C.c_void_p, C.c_void_p, f64p]
+    lib.gs_compare.restype = C.c_int
     for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
                  "gs_boot_traces_blocked", "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
         getattr(lib, name).restype = C.c_int
@@ -510,6 +522,12 @@ class HorusEngine:
         """(JCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3, E + 1)) as of the last summarize()"""
         return _fetch_jobdist(self, self.lib.gs_horus_fetch_jobdist, "gs_horus_fetch_jobdist", first, count)
 
+    def compare(self, a, b, bounds=(), edges=(), with_time=False):
+        """paired per-job comparison of replicas b[i] against a[i] on the same trace (include/gsched_horus.h:
+        gs_horus_compare): (JPAIR_DTYPE records (P, C), uint32 CDF counts of d (P, C, 3, E + 1)); with_time: and the
+        kernel milliseconds"""
+        return _compare(self, self.lib.gs_horus_compare, "gs_horus_compare", a, b, bounds, edges, with_time)
+
 
 def _fetch_timeline(eng, fn, what, first, count):
     count = eng.nsims - first if count is None else int(count)
@@ -532,6 +550,27 @@ def _set_jobdist(eng, fn, what, bounds, edges):
     eng._check(fn(eng.h, len(b) + 1, b.ctypes.data_as(C.c_void_p) if len(b) else None, len(e),
                   e.ctypes.data_as(C.c_void_p) if len(e) else None), what)
     eng._jd_shape = (len(b) + 1, len(e))
+
+
+def _compare(eng, fn, what, a, b, bounds, edges, with_time):
+    a = np.ascontiguousarray(np.asarray(a, dtype=np.int64).reshape(-1))
+    b = np.ascontiguousarray(np.asarray(b, dtype=np.int64).reshape(-1))
+    if a.shape != b.shape:
+        raise GsError(f"{what}: a and b must have the same length", GS_ERR_ARG)
+    bd = np.asarray(bounds, dtype=np.int64).reshape(-1)
+    ed = np.asarray(edges, dtype=np.int64).reshape(-1)
+    for arr in (a, b, bd, ed):
+        if arr.size and (arr.min() < -2 ** 31 or arr.max() >= 2 ** 31):
+            raise GsError(f"{what}: indices, bounds and edges must be int32", GS_ERR_ARG)
+    a, b, bd, ed = (np.ascontiguousarray(x, dtype=np.int32) for x in (a, b, bd, ed))
+    P, nc, ne = len(a), len(bd) + 1, len(ed)
+    recs = np.zeros((max(P, 1), nc), dtype=JPAIR_DTYPE)
+    hist = np.zeros((max(P, 1), nc, 3, ne + 1), dtype=np.uint32)
+    vp = lambda x: x.ctypes.data_as(C.c_void_p) if len(x) else None
+    ms = C.c_double(0.0)
+    eng._check(fn(eng.h, P, vp(a), vp(b), nc, vp(bd), ne, vp(ed), recs.ctypes.data_as(C.c_void_p), hist.ctypes.data_as(C.c_void_p),
+                  C.byref(ms)), what)
+    return (recs[:P], hist[:P], ms.value) if with_time else (recs[:P], hist[:P])
 
 
 def _fetch_jobdist(eng, fn, what, first, count):
@@ -850,6 +889,13 @@ class Engine:
         """(JCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3, E + 1)) of replicas [first, first+count)
         as of the last summarize(); count[..., m, b] = #(value m <= edges[b]) - #(value m <= edges[b - 1])"""
         return _fetch_jobdist(self, self.lib.gs_fetch_jobdist, "gs_fetch_jobdist", first, count)
+
+    def compare(self, a, b, bounds=(), edges=(), with_time=False):
+        """paired per-job comparison of replicas b[i] against a[i], which hold the same trace, over the jobs finished so
+        far (include/gsched.h: gs_compare): len(bounds) + 1 classes by num_gpu, per quantity d = x_b - x_a of wait /
+        turnaround / jct.  Returns (JPAIR_DTYPE records (P, C), uint32 CDF counts of d at `edges` (P, C, 3, E + 1));
+        with_time: and the kernel milliseconds"""
+        return _compare(self, self.lib.gs_compare, "gs_compare", a, b, bounds, edges, with_time)
 
     def run_summarized(self, rows_cap=0):
         """Run every replica to its exit condition, summarising after every launch and fetching no rows; returns

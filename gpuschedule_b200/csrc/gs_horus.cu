@@ -1,6 +1,7 @@
 // gs_horus.cu -- C ABI (include/gsched_horus.h) and kernel of the utilisation-aware placement engine.
 // One simulation per thread (see gs_horus_core.cuh for the semantics and the reference citations).
 #include <cuda_runtime.h>
+#include <string.h>
 
 #include <algorithm>
 #include <string>
@@ -71,12 +72,27 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_htl_rows_kernel(const HSim 
   gs_tl_fold_rows(bins + (size_t)r * (size_t)B, B, W, S.rows, S.util, 0, 0, S.ticks);
 }
 
+#endif  // __CUDACC__
+
+// The trace fields gs_horus_load_trace takes of job j are equal in both jobs (doubles compared bit for bit).
+static __host__ __device__ inline long long gs_hjob_bits(double v) { long long u; memcpy(&u, &v, 8); return u; }
+static __host__ __device__ inline bool gs_hjob_same(const HJob &x, const HJob &y) {
+  return x.arrive == y.arrive && x.gpus == y.gpus && x.gpc == y.gpc && x.mem_b == y.mem_b &&
+         gs_hjob_bits(x.duration) == gs_hjob_bits(y.duration) && gs_hjob_bits(x.util_avg) == gs_hjob_bits(y.util_avg) &&
+         gs_hjob_bits(x.util_max) == gs_hjob_bits(y.util_max) && gs_hjob_bits(x.mem_avg_mib) == gs_hjob_bits(y.mem_avg_mib);
+}
+
+#ifdef __CUDACC__
+// job(r, i) is the i-th job of the finish order, job_at(r, j) job j of the trace (meaningful once it has finished).
 struct GsSumHorusJobs {
   const HSim *sims;
   __device__ long long finished(int r) const { return sims[r].nfin; }
-  __device__ GsSumJob job(int r, long long i) const {
+  __device__ long long n(int r) const { return sims[r].n; }
+  __device__ int order(int r, long long i) const { return sims[r].fin[i]; }
+  __device__ GsSumJob job(int r, long long i) const { return job_at(r, sims[r].fin[i]); }
+  __device__ bool same_job(int ra, int rb, int j) const { return gs_hjob_same(sims[ra].jobs[j], sims[rb].jobs[j]); }
+  __device__ GsSumJob job_at(int r, int j) const {
     const HSim &S = sims[r];
-    const int j = S.fin[i];
     const gs_horus_job_rec rec = S.recs[j];
     return gs_sum_job(S.jobs[j].arrive, rec.start, rec.end, rec.jct, rec.preempt, S.jobs[j].gpus);
   }
@@ -617,5 +633,87 @@ extern "C" int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t 
   if (hist_out)
     HCU(cudaMemcpyAsync(hist_out, h->d_jd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   HCU(cudaStreamSynchronize(h->stream));
+  return GS_OK;
+}
+
+extern "C" int gs_horus_compare(gs_horus_handle h, int32_t npairs, const int32_t *a, const int32_t *b, int32_t nclasses, const int32_t *bounds,
+                                int32_t nedges, const int32_t *edges, gs_jpair *out, uint32_t *hist_out, double *kernel_ms) {
+  if (!h) return GS_ERR_ARG;
+  if (npairs < 0 || (npairs > 0 && (!a || !b || !out))) return hfail(h, GS_ERR_ARG, "gs_horus_compare: bad arguments");
+  GsJdCfg cfg;
+  const char *why = nullptr;
+  if (!gs_jd_make_cfg(nclasses, bounds, nedges, edges, cfg, &why)) return hfail(h, GS_ERR_ARG, std::string("gs_horus_compare: ") + why);
+  if (nclasses == 0) return hfail(h, GS_ERR_ARG, "gs_horus_compare: nclasses must be in 1..8");
+  const int nsims = (int)h->sims.size();
+  for (int i = 0; i < npairs; ++i)
+    if (a[i] < 0 || a[i] >= nsims || b[i] < 0 || b[i] >= nsims) return hfail(h, GS_ERR_ARG, "gs_horus_compare: a replica index is out of range");
+  long long nmax = 1;
+  for (int i = 0; i < npairs; ++i) {
+    const HorusSimHost &sa = h->sims[(size_t)a[i]], &sb = h->sims[(size_t)b[i]];
+    if (!sa.prepared || !sb.prepared) return hfail(h, GS_ERR_STATE, "gs_horus_compare: a replica has not run yet");
+    if (sa.dev.n != sb.dev.n) return hfail(h, GS_ERR_ARG, "gs_horus_compare: pair " + std::to_string(i) + " holds traces of different lengths");
+    nmax = std::max(nmax, (long long)sa.dev.n);
+  }
+  if (kernel_ms) *kernel_ms = 0.0;
+  if (npairs == 0) return GS_OK;
+  HCU(cudaSetDevice(h->device));
+  const size_t P = (size_t)npairs, C = (size_t)cfg.nclasses, nb = (size_t)cfg.nedges + 1;
+  std::vector<int> flags(P, 0);
+  std::vector<gs_jpair> recs(P * C);
+  std::vector<uint32_t> hist(P * C * 3 * nb);
+#ifdef __CUDACC__
+  int per_sm = 1, sms = 132;
+  HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_cmp_pairs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+  const int grid = std::min(npairs, std::max(1, per_sm) * sms);
+  const size_t pitch = (size_t)(nmax + 63) / 64 * 64;
+  // scratch: pair indices, trace-differ flags, records, CDF counts, per-block work
+  const size_t o_a = 0, o_b = up(4 * P), o_flag = up(o_b + 4 * P), o_rec = up(o_flag + 4 * P);
+  const size_t o_hist = up(o_rec + sizeof(gs_jpair) * P * C), o_work = up(o_hist + 4 * P * C * 3 * nb);
+  const size_t need = o_work + 4 * sizeof(int) * pitch * (size_t)grid;
+  if (h->sum_scratch_bytes < need) {
+    if (h->d_sum_scratch) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_sum_scratch); }
+    h->d_sum_scratch = nullptr; h->sum_scratch_bytes = 0;
+    HCU(cudaMalloc(&h->d_sum_scratch, need));
+    h->sum_scratch_bytes = need;
+  }
+  unsigned char *d = (unsigned char *)h->d_sum_scratch;
+  HCU(cudaMemcpyAsync(d + o_a, a, 4 * P, cudaMemcpyHostToDevice, h->stream));
+  HCU(cudaMemcpyAsync(d + o_b, b, 4 * P, cudaMemcpyHostToDevice, h->stream));
+  HCU(cudaEventRecord(h->ev0, h->stream));
+  gs_cmp_pairs_kernel<GsSumHorusJobs><<<(unsigned)grid, GS_SUM_THREADS, 0, h->stream>>>(
+      GsSumHorusJobs{h->d_sims}, npairs, (const int *)(d + o_a), (const int *)(d + o_b), cfg, (gs_jpair *)(d + o_rec),
+      (unsigned *)(d + o_hist), (int *)(d + o_flag), (int *)(d + o_work), (long long)pitch);
+  HCU(cudaGetLastError());
+  HCU(cudaEventRecord(h->ev1, h->stream));
+  HCU(cudaMemcpyAsync(flags.data(), d + o_flag, 4 * P, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaMemcpyAsync(recs.data(), d + o_rec, sizeof(gs_jpair) * P * C, cudaMemcpyDeviceToHost, h->stream));
+  if (hist_out) HCU(cudaMemcpyAsync(hist.data(), d + o_hist, 4 * hist.size(), cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
+#else   // host build for tests/emu: the same steps, one pair after the other
+  for (size_t p = 0; p < P; ++p) {
+    const HSim &A = h->d_sims[a[p]], &B = h->d_sims[b[p]];
+    for (int j = 0; j < A.n && !flags[p]; ++j) flags[p] = !gs_hjob_same(A.jobs[j], B.jobs[j]);
+    if (flags[p]) continue;
+    std::vector<GsSumJob> ja((size_t)A.n), jb((size_t)B.n);
+    for (int j = 0; j < A.n; ++j) {
+      ja[(size_t)j] = gs_sum_job(A.jobs[j].arrive, A.recs[j].start, A.recs[j].end, A.recs[j].jct, A.recs[j].preempt, A.jobs[j].gpus);
+      jb[(size_t)j] = gs_sum_job(B.jobs[j].arrive, B.recs[j].start, B.recs[j].end, B.recs[j].jct, B.recs[j].preempt, B.jobs[j].gpus);
+    }
+    gs_cmp_pair_serial(ja.data(), jb.data(), A.n, A.fin, A.nfin, B.fin, B.nfin, cfg, recs.data() + p * C, hist.data() + p * C * 3 * nb);
+  }
+  (void)nmax;
+#endif
+  h->launches += 1;
+  for (size_t i = 0; i < P; ++i)
+    if (flags[i]) return hfail(h, GS_ERR_ARG, "gs_horus_compare: pair " + std::to_string(i) + " (replicas " + std::to_string(a[i]) + ", " +
+                                              std::to_string(b[i]) + ") holds different traces");
+  memcpy(out, recs.data(), sizeof(gs_jpair) * recs.size());
+  if (hist_out) memcpy(hist_out, hist.data(), 4 * hist.size());
+#ifdef __CUDACC__
+  float ms = 0.f;
+  HCU(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+  if (kernel_ms) *kernel_ms = ms;
+#endif
   return GS_OK;
 }

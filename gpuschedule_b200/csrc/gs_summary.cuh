@@ -286,7 +286,10 @@ static inline bool gs_jd_make_cfg(int32_t nclasses, const int32_t *bounds, int32
 // v * v (< 2^62 for any int32 v) added to a 128-bit sum of squares.
 GS_SUM_HD void gs_jd_add_sq(uint64_t &lo, uint64_t &hi, int v) { gs_sum_add128(lo, hi, (gs_i128)((long long)v * v)); }
 
+static_assert(sizeof(gs_jpair) == 288, "gs_jpair is 288 bytes");
+
 #ifndef __CUDACC__
+#include <vector>
 // Host forms of the job part (the host-emulation build of gs_horus.cu, CPU tests): the same sums, and the same radix
 // select run serially, one target at a time.
 static inline void gs_sum_select_serial(const int *v, long long k, int out[5]) {
@@ -369,6 +372,61 @@ static inline void gs_jd_jobs_serial(const GsSumJob *jobs, long long k, const Gs
     gs_sum_select_serial(seg + 2 * pitch, kc, J.jct_q);
   }
   delete[] vals;
+}
+
+// Paired comparison of one pair (gs_jpair): ja / jb the job values of runs a and b by trace index j < n (read only for
+// jobs finished in that run, except `gpus`, which both share), fin_a / fin_b their finish orders.  out[0 .. C) and
+// hist[C][3][E + 1] are overwritten.  The kernel's steps, serially: membership words, per-class counts, differences
+// scattered into per-class segments, then per class the fold and the two selects (ascending, then negated).  The
+// traces' equality is the caller's to check.
+static inline void gs_cmp_pair_serial(const GsSumJob *ja, const GsSumJob *jb, long long n, const int *fin_a, long long ka,
+                                      const int *fin_b, long long kb, const GsJdCfg &cfg, gs_jpair *out, uint32_t *hist) {
+  const int C = cfg.nclasses, nb = cfg.nedges + 1;
+  const long long pitch = n > 0 ? n : 1;
+  std::vector<int> mem((size_t)pitch, 0), vals((size_t)(3 * pitch));
+  for (long long i = 0; i < ka; ++i) mem[(size_t)fin_a[i]] = 1;
+  for (long long i = 0; i < kb; ++i) mem[(size_t)fin_b[i]] |= 2;
+  long long cnt[3][GS_JOBDIST_MAX_CLASSES] = {};          // jobs, only_a, only_b
+  for (long long j = 0; j < n; ++j) {
+    const int w = mem[(size_t)j];
+    if (w == 0) continue;
+    const int c = gs_jd_class(cfg.bounds, C - 1, ja[j].gpus);
+    cnt[w == 3 ? 0 : w == 1 ? 1 : 2][c] += 1;
+  }
+  long long cur[GS_JOBDIST_MAX_CLASSES], off = 0;
+  for (int c = 0; c < C; ++c) { cur[c] = off; off += cnt[0][c]; }
+  for (long long j = 0; j < n; ++j) {
+    if (mem[(size_t)j] != 3) continue;
+    const long long pos = cur[gs_jd_class(cfg.bounds, C - 1, ja[j].gpus)]++;
+    vals[(size_t)pos] = jb[j].wait - ja[j].wait;
+    vals[(size_t)(pitch + pos)] = jb[j].turn - ja[j].turn;
+    vals[(size_t)(2 * pitch + pos)] = jb[j].jct - ja[j].jct;
+  }
+  for (long long i = 0; i < (long long)C * 3 * nb; ++i) hist[i] = 0;
+  off = 0;
+  for (int c = 0; c < C; ++c) {
+    gs_jpair &P = out[c];
+    P = gs_jpair{};
+    const long long kc = cnt[0][c];
+    P.jobs = kc; P.only_a = cnt[1][c]; P.only_b = cnt[2][c];
+    uint32_t *hc = hist + (size_t)c * 3 * nb;
+    for (int m = 0; m < 3; ++m) {
+      int *seg = vals.data() + m * pitch + off;
+      for (long long i = 0; i < kc; ++i) {
+        const int d = seg[i];
+        P.lt[m] += d < 0; P.eq[m] += d == 0; P.gt[m] += d > 0;
+        P.d_sum[m] += d;
+        gs_jd_add_sq(P.d_sq_lo[m], P.d_sq_hi[m], d);
+        hc[m * nb + gs_jd_bin(cfg.edges, cfg.nedges, d)] += 1;
+      }
+      gs_sum_select_serial(seg, kc, P.q_hi[m]);
+      for (long long i = 0; i < kc; ++i) seg[i] = -seg[i];
+      int q[5];
+      gs_sum_select_serial(seg, kc, q);
+      for (int t = 0; t < 5; ++t) P.q_lo[m][t] = -q[t];
+    }
+    off += kc;
+  }
 }
 #endif
 
@@ -799,6 +857,146 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_jd_jobs_kernel(Src src, int
           J.jct_q[t] = kc > 0 ? (int)(s[11] + (long long)prefix[10 + t]) : 0;
         }
         classes[(size_t)r * C + c] = J;
+      }
+      __syncthreads();
+      off += kc;
+    }
+  }
+}
+
+// Paired comparison (gs_jpair) of pairs (pa[p], pb[p]), p < npairs, one block per pair in turn (grid-stride).  Src
+// supplies n(r), finished(r), order(r, i) (the i-th job of the finish order), job_at(r, j) (job j of the trace) and
+// same_job(ra, rb, j) (the trace records of job j are equal); the host has checked that both replicas hold n jobs.
+// scratch: 4 * pitch ints per block, membership words then three columns of differences.  Per pair:
+// (1) membership words: zeroed, bit 1 from a's finish order, bit 2 from b's (each job is at most once in an order, so
+// plain stores); (2) one pass in trace order: trace equality (a pair that differs sets flags[p] and stops here) and
+// the per-class counts jobs / only_a / only_b, block-reduced; (3) class offsets, and d = x_b - x_a of every job
+// finished in both runs scattered into its class's segment through warp-aggregated cursors (jd's step 3); (4) per
+// class: counts by sign, sums, 128-bit sums of squares (as sums of 32-bit halves), min / max block-reduced, CDF counts
+// into shared counters, gs_sum_select over the segment for q_hi, then the segment negated in place and selected again
+// for q_lo = -result.  Outputs recs[p * C + c], hists[((p * C + c) * 3 + m) * (E + 1) + bin].
+template <class Src>
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_cmp_pairs_kernel(Src src, int npairs, const int *pa, const int *pb, GsJdCfg cfg,
+                                                                     gs_jpair *recs, unsigned *hists, int *flags, int *scratch,
+                                                                     long long pitch) {
+  __shared__ unsigned hist[GS_SUM_TARGETS * GS_SUM_BINS];
+  __shared__ unsigned long long prefix[GS_SUM_TARGETS];
+  __shared__ unsigned cdf[3 * (GS_JOBDIST_MAX_EDGES + 1)];
+  __shared__ int edges[GS_JOBDIST_MAX_EDGES];
+  __shared__ long long cls_cnt[3][GS_JOBDIST_MAX_CLASSES];    // jobs, only_a, only_b per class
+  __shared__ long long cursor[GS_JOBDIST_MAX_CLASSES];
+  __shared__ gs_jpair rec;
+  const int C = cfg.nclasses, E = cfg.nedges, nb = E + 1;
+  const int lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < E; i += blockDim.x) edges[i] = cfg.edges[i];
+  int *mem = scratch + (size_t)blockIdx.x * 4 * (size_t)pitch;
+  int *vals = mem + pitch;
+  for (int p = blockIdx.x; p < npairs; p += gridDim.x) {
+    const int ra = pa[p], rb = pb[p];
+    const long long n = src.n(ra), ka = src.finished(ra), kb = src.finished(rb);
+    for (long long j = threadIdx.x; j < n; j += blockDim.x) mem[j] = 0;
+    __syncthreads();
+    for (long long i = threadIdx.x; i < ka; i += blockDim.x) mem[src.order(ra, i)] = 1;
+    __syncthreads();
+    for (long long i = threadIdx.x; i < kb; i += blockDim.x) mem[src.order(rb, i)] |= 2;
+    __syncthreads();
+    long long red[3 * GS_JOBDIST_MAX_CLASSES];
+#pragma unroll
+    for (int e = 0; e < 3 * GS_JOBDIST_MAX_CLASSES; ++e) red[e] = 0;
+    int diff = 0;
+    for (long long j = threadIdx.x; j < n; j += blockDim.x) {
+      diff |= !src.same_job(ra, rb, (int)j);
+      const int w = mem[j];
+      if (w == 0) continue;
+      const int c = gs_jd_class(cfg.bounds, C - 1, src.job_at(ra, (int)j).gpus);
+      const int s = w == 3 ? 0 : w == 1 ? GS_JOBDIST_MAX_CLASSES : 2 * GS_JOBDIST_MAX_CLASSES;
+#pragma unroll
+      for (int u = 0; u < GS_JOBDIST_MAX_CLASSES; ++u) {
+        if (c == u) { red[u] += s == 0; red[GS_JOBDIST_MAX_CLASSES + u] += s == GS_JOBDIST_MAX_CLASSES; red[2 * GS_JOBDIST_MAX_CLASSES + u] += s == 2 * GS_JOBDIST_MAX_CLASSES; }
+      }
+    }
+    diff = __syncthreads_or(diff);
+    if (threadIdx.x == 0) flags[p] = diff;
+    if (diff) continue;                                       // (block-uniform; the host refuses the call)
+    gs_sum_block_vec<3 * GS_JOBDIST_MAX_CLASSES, 3 * GS_JOBDIST_MAX_CLASSES, 0>(red);
+    if (threadIdx.x < GS_JOBDIST_MAX_CLASSES) {
+      const int c = threadIdx.x;
+      long long off = 0;
+#pragma unroll
+      for (int u = 0; u < GS_JOBDIST_MAX_CLASSES; ++u) off += u < c ? red[u] : 0;
+#pragma unroll
+      for (int u = 0; u < GS_JOBDIST_MAX_CLASSES; ++u) {
+        if (u == c) { cls_cnt[0][c] = red[u]; cls_cnt[1][c] = red[GS_JOBDIST_MAX_CLASSES + u]; cls_cnt[2][c] = red[2 * GS_JOBDIST_MAX_CLASSES + u]; }
+      }
+      cursor[c] = off;
+    }
+    __syncthreads();
+    for (long long j0 = 0; j0 < n; j0 += blockDim.x) {      // (warp-uniform trip count: the shuffles see full warps)
+      const long long j = j0 + threadIdx.x;
+      const bool in = j < n && mem[j] == 3;
+      GsSumJob va, vb;
+      int c = -1;
+      if (in) { va = src.job_at(ra, (int)j); vb = src.job_at(rb, (int)j); c = gs_jd_class(cfg.bounds, C - 1, va.gpus); }
+      const unsigned peers = __match_any_sync(0xffffffffu, c);
+      const int head = __ffs(peers) - 1;
+      long long base = 0;
+      if (in && lane == head) base = atomicAdd((unsigned long long *)&cursor[c], (unsigned long long)__popc(peers));
+      base = __shfl_sync(0xffffffffu, base, head);
+      if (in) {
+        const long long pos = base + __popc(peers & ((1u << lane) - 1u));
+        vals[pos] = vb.wait - va.wait; vals[pitch + pos] = vb.turn - va.turn; vals[2 * pitch + pos] = vb.jct - va.jct;
+      }
+    }
+    __syncthreads();
+    long long off = 0;
+    for (int c = 0; c < C; ++c) {
+      const long long kc = cls_cnt[0][c];
+      int *seg = vals + off;
+      for (int i = threadIdx.x; i < 3 * nb; i += blockDim.x) cdf[i] = 0;
+      if (threadIdx.x == 0) { rec = gs_jpair{}; rec.jobs = kc; rec.only_a = cls_cnt[1][c]; rec.only_b = cls_cnt[2][c]; }
+      __syncthreads();
+      long long mn[3], mx[3];
+#pragma unroll
+      for (int m = 0; m < 3; ++m) {                         // one quantity at a time (7 values per reduction: no spills)
+        // #(d < 0), #(d > 0), sum, squares as the sums of their high and low 32-bit halves, min, max
+        long long s[7] = {0, 0, 0, 0, 0, 0x7fffffff, -0x80000000ll};
+        for (long long i = threadIdx.x; i < kc; i += blockDim.x) {
+          const int d = seg[m * pitch + i];
+          const unsigned long long sq = (unsigned long long)((long long)d * d);
+          s[0] += d < 0; s[1] += d > 0; s[2] += d;
+          s[3] += (long long)(sq >> 32); s[4] += (long long)(sq & 0xffffffffull);
+          s[5] = min(s[5], (long long)d); s[6] = max(s[6], (long long)d);
+          atomicAdd(&cdf[m * nb + gs_jd_bin(edges, E, d)], 1u);
+        }
+        gs_sum_block_vec<7, 5, 1>(s);                       // (its barriers also publish the CDF counts)
+        mn[m] = s[5]; mx[m] = s[6];
+        if (threadIdx.x == 0) {
+          rec.lt[m] = s[0]; rec.gt[m] = s[1]; rec.eq[m] = kc - s[0] - s[1]; rec.d_sum[m] = s[2];
+          gs_sum_add128(rec.d_sq_lo[m], rec.d_sq_hi[m], ((gs_i128)s[3] << 32) + s[4]);
+        }
+      }
+      unsigned *hout = hists + ((size_t)p * C + c) * 3 * (size_t)nb;
+      for (int i = threadIdx.x; i < 3 * nb; i += blockDim.x) hout[i] = cdf[i];
+      long long span = 0;
+#pragma unroll
+      for (int m = 0; m < 3; ++m) span = max(span, mx[m] - mn[m]);
+      gs_sum_select(hist, prefix, seg, pitch, kc, mn, span);
+      if (threadIdx.x == 0)
+        for (int m = 0; m < 3; ++m)
+          for (int t = 0; t < 5; ++t) rec.q_hi[m][t] = kc > 0 ? (int)(mn[m] + (long long)prefix[m * 5 + t]) : 0;
+      for (long long i = threadIdx.x; i < kc; i += blockDim.x) {
+#pragma unroll
+        for (int m = 0; m < 3; ++m) seg[m * pitch + i] = -seg[m * pitch + i];
+      }
+      long long nmin[3];
+#pragma unroll
+      for (int m = 0; m < 3; ++m) nmin[m] = -mx[m];
+      __syncthreads();                                      // thread 0 has read prefix; the negated segment is published
+      gs_sum_select(hist, prefix, seg, pitch, kc, nmin, span);
+      if (threadIdx.x == 0) {
+        for (int m = 0; m < 3; ++m)
+          for (int t = 0; t < 5; ++t) rec.q_lo[m][t] = kc > 0 ? (int)-(nmin[m] + (long long)prefix[m * 5 + t]) : 0;
+        recs[(size_t)p * C + c] = rec;
       }
       __syncthreads();
       off += kc;

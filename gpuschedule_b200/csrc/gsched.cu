@@ -1104,13 +1104,23 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_tl_rows_kernel(const SimDev
   gs_tl_util_nan(T, B);
 }
 
-// The finished jobs as job.csv prints them (gs_expand_jobs_kernel for fifo, the job records otherwise).
+// The finished jobs as job.csv prints them (gs_expand_jobs_kernel for fifo, the job records otherwise).  job(r, i) is
+// the i-th job of the finish order, job_at(r, j) job j of the trace (meaningful once it has finished).
 struct GsSumEngineJobs {
   const SimDev *sims;
   __device__ long long finished(int r) const { return sims[r].finished; }
-  __device__ GsSumJob job(int r, long long i) const {
+  __device__ long long n(int r) const { return sims[r].n; }
+  __device__ int order(int r, long long i) const { return sims[r].fin[i]; }
+  __device__ GsSumJob job(int r, long long i) const { return job_at(r, sims[r].fin[i]); }
+  // the gs_jobin records of job j in the traces of replicas ra and rb are byte-equal
+  __device__ bool same_job(int ra, int rb, int j) const {
+    const unsigned long long *x = reinterpret_cast<const unsigned long long *>(sims[ra].jobs + j);
+    const unsigned long long *y = reinterpret_cast<const unsigned long long *>(sims[rb].jobs + j);
+    static_assert(sizeof(JobIn) == 32, "JobIn is four 64-bit words");
+    return x[0] == y[0] && x[1] == y[1] && x[2] == y[2] && x[3] == y[3];
+  }
+  __device__ GsSumJob job_at(int r, int j) const {
     const SimDev &S = sims[r];
-    const int j = S.fin[i];
     const JobIn jb = S.jobs[j];
     if (S.policy == GS_SCHED_FIFO) {
       const int st = S.jstart[j];
@@ -1271,6 +1281,63 @@ extern "C" int gs_fetch_jobdist(gs_handle h, int first, int count, gs_jclass *cl
   if (hist_out)
     CU(cudaMemcpyAsync(hist_out, h->d_jd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(wait_stream(h));
+  return GS_OK;
+}
+
+extern "C" int gs_compare(gs_handle h, int32_t npairs, const int32_t *a, const int32_t *b, int32_t nclasses, const int32_t *bounds,
+                          int32_t nedges, const int32_t *edges, gs_jpair *out, uint32_t *hist_out, double *kernel_ms) {
+  if (!h) return GS_ERR_ARG;
+  if (npairs < 0 || (npairs > 0 && (!a || !b || !out))) return fail(h, GS_ERR_ARG, "gs_compare: bad arguments");
+  GsJdCfg cfg;
+  const char *why = nullptr;
+  if (!gs_jd_make_cfg(nclasses, bounds, nedges, edges, cfg, &why)) return fail(h, GS_ERR_ARG, std::string("gs_compare: ") + why);
+  if (nclasses == 0) return fail(h, GS_ERR_ARG, "gs_compare: nclasses must be in 1..8");
+  int64_t nmax = 1;
+  for (int i = 0; i < npairs; ++i)
+    if (a[i] < 0 || a[i] >= h->nsims || b[i] < 0 || b[i] >= h->nsims) return fail(h, GS_ERR_ARG, "gs_compare: a replica index is out of range");
+  for (int i = 0; i < npairs; ++i) {
+    const SimHost &sa = h->sims[(size_t)a[i]], &sb = h->sims[(size_t)b[i]];
+    if (!sa.prepared || !sb.prepared) return fail(h, GS_ERR_STATE, "gs_compare: a replica has not run yet");
+    if (sa.dev.n != sb.dev.n) return fail(h, GS_ERR_ARG, "gs_compare: pair " + std::to_string(i) + " holds traces of different lengths");
+    nmax = std::max(nmax, (int64_t)sa.dev.n);
+  }
+  if (kernel_ms) *kernel_ms = 0.0;
+  if (npairs == 0) return GS_OK;
+  CU(cudaSetDevice(h->device));
+  int per_sm = 1, sms = 132;
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_cmp_pairs_kernel<GsSumEngineJobs>, GS_SUM_THREADS, 0));
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+  const int grid = std::min(npairs, std::max(1, per_sm) * sms);
+  const size_t pitch = align_up((size_t)nmax, 64), P = (size_t)npairs, C = (size_t)cfg.nclasses, nb = (size_t)cfg.nedges + 1;
+  // scratch: pair indices, trace-differ flags, records, CDF counts, per-block work
+  const size_t o_a = 0, o_b = align_up(4 * P), o_flag = align_up(o_b + 4 * P), o_rec = align_up(o_flag + 4 * P);
+  const size_t o_hist = align_up(o_rec + sizeof(gs_jpair) * P * C), o_work = align_up(o_hist + 4 * P * C * 3 * nb);
+  int rc = ensure_scratch(h, o_work + 4 * sizeof(int) * pitch * (size_t)grid);
+  if (rc) return rc;
+  unsigned char *d = (unsigned char *)h->d_scratch;
+  CU(cudaMemcpyAsync(d + o_a, a, 4 * P, cudaMemcpyHostToDevice, h->stream));
+  CU(cudaMemcpyAsync(d + o_b, b, 4 * P, cudaMemcpyHostToDevice, h->stream));
+  CU(cudaEventRecord(h->e0, h->stream));
+  gs_cmp_pairs_kernel<GsSumEngineJobs><<<(unsigned)grid, GS_SUM_THREADS, 0, h->stream>>>(
+      GsSumEngineJobs{h->d_sims}, npairs, (const int *)(d + o_a), (const int *)(d + o_b), cfg, (gs_jpair *)(d + o_rec),
+      (unsigned *)(d + o_hist), (int *)(d + o_flag), (int *)(d + o_work), (long long)pitch);
+  CU(cudaGetLastError());
+  h->launches += 1;
+  CU(cudaEventRecord(h->e1, h->stream));
+  std::vector<int> flags(P);
+  std::vector<gs_jpair> recs(P * C);
+  std::vector<uint32_t> hist(hist_out ? P * C * 3 * nb : 0);
+  CU(cudaMemcpyAsync(flags.data(), d + o_flag, 4 * P, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaMemcpyAsync(recs.data(), d + o_rec, sizeof(gs_jpair) * P * C, cudaMemcpyDeviceToHost, h->stream));
+  if (hist_out) CU(cudaMemcpyAsync(hist.data(), d + o_hist, 4 * hist.size(), cudaMemcpyDeviceToHost, h->stream));
+  CU(wait_stream(h));
+  for (size_t i = 0; i < P; ++i)
+    if (flags[i]) return fail(h, GS_ERR_ARG, "gs_compare: pair " + std::to_string(i) + " (replicas " + std::to_string(a[i]) + ", " +
+                                             std::to_string(b[i]) + ") holds different traces");
+  memcpy(out, recs.data(), sizeof(gs_jpair) * recs.size());
+  if (hist_out) memcpy(hist_out, hist.data(), 4 * hist.size());
+  float ms = 0; cudaEventElapsedTime(&ms, h->e0, h->e1);
+  if (kernel_ms) *kernel_ms = ms;
   return GS_OK;
 }
 

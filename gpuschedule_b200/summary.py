@@ -20,6 +20,11 @@ Job statistics by job size (capi.JCLASS_DTYPE records and CDF counts from Engine
 turnaround and jct, and their CDF at every edge -- job_analysis.ipynb's breakdown by used_gpus and
 scheduler_analysis.ipynb's mean / median / std -- and `jobdist_spread` their spread per class over the replicas that
 have jobs in that class.
+
+Paired comparisons (capi.JPAIR_DTYPE records and CDF counts from Engine.compare / HorusEngine.compare): `pair_derived`
+gives per class and quantity the per-job differences d = x_b - x_a of two configurations on the same trace -- their
+mean, sample std, shares below / at / above zero, ten order statistics and CDF --, `pair_spread` their spread over
+replicas, and `paired_spread` the replica-level differences b - a of the makespan and every derived number.
 """
 from __future__ import annotations
 
@@ -313,3 +318,134 @@ def jobdist_spread_columns():
 
 def jobdist_spread_flat(sp, c):
     return [float(sp[name][s][c]) for name in JOBDIST_METRICS for s in SPREAD_STATS]
+
+
+# ---------------------------------------------------------------- paired comparisons of two configurations
+PAIR_POINTS = ("p0", "p1", "p5", "p10", "p50_lo", "p50", "p90", "p95", "p99", "p100")
+PAIR_STATS = ("d_mean", "d_std", "lt_share", "eq_share", "gt_share") + tuple(f"d_{p}" for p in PAIR_POINTS)
+PAIR_METRICS = tuple(f"{m}_{s}" for m in JOBDIST_QUANTITIES for s in PAIR_STATS)
+PAIR_COUNTS = ("jobs", "only_a", "only_b")
+
+
+def _jpair_numbers(rec):
+    """the PAIR_METRICS of one JPAIR_DTYPE record as a dict of floats (NaN without jobs; std NaN below two jobs).  The
+    mean is the exact sum over the job count rounded once, the sample variance (n * sumsq - sum^2) / (n * (n - 1))
+    exact in Python ints and rounded once.  Points: d_p100 .. d_p50 from q_hi, d_p50_lo .. d_p0 from q_lo."""
+    n = int(rec["jobs"])
+    out = {}
+    for i, m in enumerate(JOBDIST_QUANTITIES):
+        s, sq = int(rec["d_sum"][i]), u128(rec["d_sq_lo"][i], rec["d_sq_hi"][i])
+        out[m + "_d_mean"] = s / n if n else math.nan
+        out[m + "_d_std"] = math.sqrt(float(Fraction(n * sq - s * s, n * (n - 1)))) if n > 1 else math.nan
+        for k in ("lt", "eq", "gt"):
+            out[f"{m}_{k}_share"] = int(rec[k][i]) / n if n else math.nan
+        hi, lo = rec["q_hi"][i].tolist(), rec["q_lo"][i].tolist()
+        for p, v in zip(("p50", "p90", "p95", "p99", "p100"), hi):
+            out[f"{m}_d_{p}"] = float(v) if n else math.nan
+        for p, v in zip(("p50_lo", "p10", "p5", "p1", "p0"), lo):
+            out[f"{m}_d_{p}"] = float(v) if n else math.nan
+    return out
+
+
+def pair_derived(recs, hist, edges):
+    """Per class of one pair: `recs` JPAIR_DTYPE (C,), `hist` CDF counts of d (C, 3, E + 1), `edges` the E signed edges.
+    Returns {"jobs", "only_a", "only_b": int arrays (C,), metric: float array (C,) for every PAIR_METRICS entry,
+    "<quantity>_cdf": float array (C, E) = #(d <= edge) / jobs}; NaN for a class without jobs in both runs."""
+    recs, hist = np.asarray(recs), np.asarray(hist, dtype=np.int64)
+    if recs.ndim != 1 or hist.shape != (len(recs), 3, len(edges) + 1):
+        raise ValueError("pair_derived: expected recs (C,) and hist (C, 3, len(edges) + 1)")
+    out = {k: recs[k].astype(np.int64) for k in PAIR_COUNTS}
+    nums = [_jpair_numbers(rec) for rec in recs]
+    for name in PAIR_METRICS:
+        out[name] = np.array([d[name] for d in nums], dtype=np.float64)
+    jobs = out["jobs"]
+    cum = np.cumsum(hist, axis=2)[:, :, :len(edges)]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        for i, m in enumerate(JOBDIST_QUANTITIES):
+            out[m + "_cdf"] = np.where(jobs[:, None] > 0, cum[:, i, :] / np.where(jobs > 0, jobs, 1)[:, None], np.nan)
+    return out
+
+
+def pair_spread(recs, hist, edges, level=0.95):
+    """Spread per class across replicas of one pair of configurations: `recs` (replicas, C), `hist` (replicas, C, 3,
+    E + 1).  For every class, over the replicas with jobs finished in both runs in it: {"replicas": int array (C,),
+    name: {mean, std, lo, hi: float arrays (C,)} for the counts (PAIR_COUNTS) and every PAIR_METRICS entry,
+    "<quantity>_cdf": {mean, std, lo, hi: float arrays (C, E)}}, with spread's rules."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    recs, hist = np.asarray(recs), np.asarray(hist)
+    if recs.ndim != 2 or hist.shape != recs.shape + (3, len(edges) + 1):
+        raise ValueError("pair_spread: expected recs (replicas, C) and hist (replicas, C, 3, len(edges) + 1)")
+    per = [pair_derived(recs[r], hist[r], edges) for r in range(recs.shape[0])]
+    nc, ne = recs.shape[1], len(edges)
+    reach = recs["jobs"] > 0
+    out = {"replicas": reach.sum(axis=0).astype(np.int64)}
+    for name in PAIR_COUNTS + PAIR_METRICS:
+        cols = [_spread_of(np.array([d[name][c] for r, d in enumerate(per) if reach[r, c]], dtype=np.float64), level) for c in range(nc)]
+        out[name] = {s: np.array([col[s] for col in cols], dtype=np.float64) for s in SPREAD_STATS}
+    for m in JOBDIST_QUANTITIES:
+        st = {s: np.full((nc, ne), math.nan) for s in SPREAD_STATS}
+        cdf = np.stack([d[m + "_cdf"] for d in per]) if per else np.zeros((0, nc, ne))
+        for c in range(nc):
+            for e in range(ne):
+                sp = _spread_of(cdf[reach[:, c], c, e], level)
+                for s in SPREAD_STATS:
+                    st[s][c, e] = sp[s]
+        out[m + "_cdf"] = st
+    return out
+
+
+def pair_columns():
+    """names of the flat per-(class, quantity) columns `pair_flat` returns, in order"""
+    return list(PAIR_COUNTS) + list(PAIR_STATS)
+
+
+def pair_flat(d, c, m):
+    """class c, quantity m of a pair_derived dict as a list of Python values"""
+    return [int(d[k][c]) for k in PAIR_COUNTS] + [float(d[f"{m}_{s}"][c]) for s in PAIR_STATS]
+
+
+def pair_spread_columns():
+    return [f"{name}_{s}" for name in PAIR_COUNTS + PAIR_STATS for s in SPREAD_STATS]
+
+
+def pair_spread_flat(sp, c, m):
+    return [float(sp[name if name in PAIR_COUNTS else f"{m}_{name}"][s][c]) for name in PAIR_COUNTS + PAIR_STATS for s in SPREAD_STATS]
+
+
+PAIRED_STATS = SPREAD_STATS + ("b_lt_a", "b_eq_a", "b_gt_a")
+
+
+def paired_spread(records_a, records_b, cluster_a, cluster_b, level=0.95):
+    """Replica-level differences of two configurations run on the same replicas (common random numbers): for every
+    replica r, b - a of the makespan and of every derived number, each side derived with its own cluster
+    ((n_nodes, gpus_per_node, gpu_mem_cap_mib)).  Returns {metric: {mean, std, lo, hi (spread's rules over the
+    differences), b_lt_a, b_eq_a, b_gt_a (replicas where b < a, b == a, b > a; a NaN difference counts in none)}}
+    for every SPREAD_METRICS entry."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    if len(records_a) != len(records_b):
+        raise ValueError("paired_spread: the two configurations need the same replicas")
+    diff = {m: [] for m in SPREAD_METRICS}
+    for ra, rb in zip(records_a, records_b):
+        da, db = derived(ra, *cluster_a), derived(rb, *cluster_b)
+        diff["makespan"].append(float(int(rb["makespan"]) - int(ra["makespan"])))
+        for m in SPREAD_METRICS[1:]:
+            diff[m].append(db[m] - da[m])
+    out = {}
+    for m, vals in diff.items():
+        v = np.asarray(vals, dtype=np.float64)
+        sp = _spread_of(v, level)
+        sp.update(b_lt_a=int((v < 0).sum()), b_eq_a=int((v == 0).sum()), b_gt_a=int((v > 0).sum()))
+        out[m] = sp
+    return out
+
+
+def paired_columns():
+    return [f"{m}_{s}" for m in SPREAD_METRICS for s in PAIRED_STATS]
+
+
+def paired_flat(sp):
+    return [sp[m][s] for m in SPREAD_METRICS for s in PAIRED_STATS]

@@ -197,14 +197,55 @@ def check_jobdist(jobdist):
     return tuple(bounds), tuple(edges)
 
 
-def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None):
+DEFAULT_DIFF_EDGES = tuple(-2 ** i for i in range(30, -1, -1)) + (0,) + tuple(2 ** i for i in range(31))
+
+
+def check_compare(compare, flag_sets):
+    """(pairs as a tuple of (a, b) configuration indices, class bounds, signed CDF edges) of a compare argument, or
+    ValueError: both configurations of a pair must share a trace file and an engine (both utilisation-aware or
+    neither)"""
+    try:
+        pairs, bounds, edges = compare
+        pairs = tuple((int(a), int(b)) for a, b in pairs)
+    except (TypeError, ValueError):
+        raise ValueError("compare: expected (pairs of configuration indices, class bounds, CDF edges)") from None
+    try:
+        bounds, edges = check_jobdist((bounds, edges))
+    except ValueError as e:
+        raise ValueError(f"compare: {e}") from None
+    for a, b in pairs:
+        if not (0 <= a < len(flag_sets) and 0 <= b < len(flag_sets)):
+            raise ValueError(f"compare: pair ({a}, {b}) names a configuration that does not exist")
+        fa, fb = flag_sets[a], flag_sets[b]
+        if fa.trace_file != fb.trace_file:
+            raise ValueError(f"compare: configurations {a} and {b} run on different trace files")
+        if _is_utilisation_aware(fa) != _is_utilisation_aware(fb):
+            raise ValueError(f"compare: {fa.schedule} and {fb.schedule} run on different engines (utilisation-aware and not); "
+                             "such pairs are not supported")
+    return pairs, bounds, edges
+
+
+def _compare_in(eng, pairs, members, bounds, edges):
+    """gs_compare of the pairs whose configurations are replicas `members` of the handle (in that order)"""
+    pos = {c: i for i, c in enumerate(members)}
+    return eng.compare([pos[a] for a, _ in pairs], [pos[b] for _, b in pairs], bounds, edges)
+
+
+def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None, compare=None):
     """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
     same configurations and random streams as run_batched, but no row or job record is read back and nothing is
     written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus.
     timeline=(W, B): also bin every replica's rows on the device (gs_set_timeline) and return (summaries,
     TBIN_DTYPE bins of shape (len(flag_sets), B)).
     jobdist=(bounds, edges): also compute every replica's job statistics by job size on the device (gs_set_jobdist)
-    and append (JCLASS_DTYPE records (len(flag_sets), C), CDF counts (len(flag_sets), C, 3, E + 1)) to the result."""
+    and append (JCLASS_DTYPE records (len(flag_sets), C), CDF counts (len(flag_sets), C, 3, E + 1)) to the result.
+    compare=(pairs, bounds, edges): also compare every pair (a, b) of configuration indices job by job on the device
+    (gs_compare, after the runs) and append (JPAIR_DTYPE records (len(pairs), C), CDF counts of d (len(pairs), C, 3,
+    E + 1)) as the last element; both configurations of a pair must share a trace file and an engine."""
+    if compare is not None:
+        pairs, cmp_bounds, cmp_edges = check_compare(compare, flag_sets)
+        cmp_recs = np.zeros((len(pairs), len(cmp_bounds) + 1), dtype=capi.JPAIR_DTYPE)
+        cmp_hist = np.zeros((len(pairs), len(cmp_bounds) + 1, 3, len(cmp_edges) + 1), dtype=np.uint32)
     if timeline is not None:
         W, B = check_timeline(timeline)
         bins = np.zeros((len(flag_sets), B), dtype=capi.TBIN_DTYPE)
@@ -229,6 +270,9 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 bins[aware] = eng.timeline()
             if jobdist is not None:
                 jd_cls[aware], jd_hist[aware] = eng.jobdist()
+            sel = [k for k, (a, _) in enumerate(pairs) if a in set(aware)] if compare is not None else []
+            if sel:
+                cmp_recs[sel], cmp_hist[sel] = _compare_in(eng, [pairs[k] for k in sel], aware, cmp_bounds, cmp_edges)
     if plain:
         sims = _plain_setup([flag_sets[i] for i in plain])
         with capi.Engine(device=device, nsims=len(sims)) as eng:
@@ -242,7 +286,11 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 bins[plain] = eng.timeline()
             if jobdist is not None:
                 jd_cls[plain], jd_hist[plain] = eng.jobdist()
-    res = (out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
+            sel = [k for k, (a, _) in enumerate(pairs) if a in set(plain)] if compare is not None else []
+            if sel:
+                cmp_recs[sel], cmp_hist[sel] = _compare_in(eng, [pairs[k] for k in sel], plain, cmp_bounds, cmp_edges)
+    res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
+           + (((cmp_recs, cmp_hist),) if compare is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -270,7 +318,8 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1):
         raise ValueError(f"bootstrap: the utilisation-aware engine ({', '.join(sorted(set(aware)))}) has no generated traces")
 
 
-def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1):
+def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1,
+                        compare=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -286,8 +335,13 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     (len(flag_sets), len(loads), replicas, C), CDF counts (len(flag_sets), len(loads), replicas, C, 3, E + 1)).
     block_len=L > 1 draws every replica as a stationary block bootstrap with mean block length L
     (gs_boot_traces_blocked): runs of consecutive jobs keep their order and the gaps between them, so a trace's bursts
-    survive resampling; the same replica index is coupled across values of L."""
+    survive resampling; the same replica index is coupled across values of L.
+    compare=(pairs, bounds, edges): also compare replica (a, L, r) with (b, L, r) job by job on the device for every pair
+    (a, b) of configuration indices (both on one trace file) and append (JPAIR_DTYPE records (len(pairs), len(loads),
+    replicas, C), CDF counts of d (len(pairs), len(loads), replicas, C, 3, E + 1)) as the last element."""
     _check_bootstrap_args(flag_sets, replicas, loads, n, block_len)
+    if compare is not None:
+        pairs, cmp_bounds, cmp_edges = check_compare(compare, flag_sets)
     block_len = tracegen.check_block_len(block_len)
     if timeline is not None:
         W, B = check_timeline(timeline)
@@ -301,6 +355,10 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     if jobdist is not None:
         jd_cls = np.zeros((len(flag_sets), len(loads), R, nc), dtype=capi.JCLASS_DTYPE)
         jd_hist = np.zeros((len(flag_sets), len(loads), R, nc, 3, nb), dtype=np.uint32)
+    if compare is not None:
+        cmp_nc, cmp_nb = len(cmp_bounds) + 1, len(cmp_edges) + 1
+        cmp_recs = np.zeros((len(pairs), len(loads), R, cmp_nc), dtype=capi.JPAIR_DTYPE)
+        cmp_hist = np.zeros((len(pairs), len(loads), R, cmp_nc, 3, cmp_nb), dtype=np.uint32)
     by_trace = {}
     for c, fl in enumerate(flag_sets):
         by_trace.setdefault(fl.trace_file, []).append(c)
@@ -327,6 +385,15 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
             recs = eng.run_summarized()
             tl = eng.timeline() if timeline is not None else None
             jd = eng.jobdist() if jobdist is not None else None
+            sel = [k for k, (a, _) in enumerate(pairs) if a in set(configs)] if compare is not None else []
+            if sel:
+                pos = {c: k for k, c in enumerate(configs)}
+                span = np.arange(len(loads) * R)                  # replica (config k, load l, r) is k * len(loads) * R + l * R + r
+                ia = np.concatenate([pos[pairs[k][0]] * len(loads) * R + span for k in sel])
+                ib = np.concatenate([pos[pairs[k][1]] * len(loads) * R + span for k in sel])
+                cr, ch = eng.compare(ia, ib, cmp_bounds, cmp_edges)
+                cmp_recs[sel] = cr.reshape(len(sel), len(loads), R, cmp_nc)
+                cmp_hist[sel] = ch.reshape(len(sel), len(loads), R, cmp_nc, 3, cmp_nb)
         for k, c in enumerate(configs):
             part = slice(k * len(loads) * R, (k + 1) * len(loads) * R)
             out[c] = recs[part].reshape(len(loads), R)
@@ -335,7 +402,8 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
             if jd is not None:
                 jd_cls[c] = jd[0][part].reshape(len(loads), R, nc)
                 jd_hist[c] = jd[1][part].reshape(len(loads), R, nc, 3, nb)
-    res = (out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
+    res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
+           + (((cmp_recs, cmp_hist),) if compare is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -486,6 +554,86 @@ def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edge
                                        + [float(sp[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS])
 
 
+def _pair_keys(fl, base):
+    return [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, base.schedule]
+
+
+def write_paired_csv(path, flag_sets, pairs, recs, hist, bounds, edges):
+    """one line per (configuration b of a pair, class, quantity): b's flags, the base configuration's schedule, the
+    class, its num_gpu range, the quantity and summary.pair_derived's columns for d = x_b - x_base"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["base_schedule", "class", "gpus_min", "gpus_max", "quantity"] + summary.pair_columns())
+        for (a, b), rc, hs in zip(pairs, recs, hist):
+            d = summary.pair_derived(rc, hs, edges)
+            for c in range(len(rc)):
+                for m in summary.JOBDIST_QUANTITIES:
+                    w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + [c] + _class_range(c, bounds) + [m] + summary.pair_flat(d, c, m))
+
+
+def write_paired_ci_csv(path, flag_sets, pairs, loads, recs, hist, bounds, edges, level=0.95, block_len=None):
+    """one line per (configuration b of a pair, load, class, quantity): b's flags, the base schedule, the load,
+    block_len (with a block length), the class, its num_gpu range, the quantity, the replicas with jobs finished in
+    both runs in the class and summary.pair_spread's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["base_schedule", "load"] + _block_col(block_len) + ["class", "gpus_min", "gpus_max", "quantity", "replicas", "level"]
+                   + summary.pair_spread_columns())
+        for (a, b), per_rc, per_hs in zip(pairs, recs, hist):
+            for L, rc, hs in zip(loads, per_rc, per_hs):
+                sp = summary.pair_spread(rc, hs, edges, level=level)
+                for c in range(rc.shape[1]):
+                    for m in summary.JOBDIST_QUANTITIES:
+                        w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + [L] + _block_val(block_len) + [c] + _class_range(c, bounds)
+                                   + [m, int(sp["replicas"][c]), level] + summary.pair_spread_flat(sp, c, m))
+
+
+def write_paired_cdf_csv(path, flag_sets, pairs, recs, hist, bounds, edges, loads=None, level=0.95, block_len=None):
+    """one line per (configuration b of a pair[, load], class, quantity, edge): b's flags, the base schedule[, the load,
+    block_len], the class, its num_gpu range, the quantity, the edge and the fraction of the jobs finished in both
+    runs with d <= edge (with loads: the replicas with such jobs and the spread of that fraction)"""
+    import csv
+    boot = loads is not None
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) if boot else []) + ["class", "gpus_min", "gpus_max", "quantity", "edge"]
+                   + (["replicas", "level"] + [f"cdf_{s}" for s in summary.SPREAD_STATS] if boot else ["jobs", "cdf"]))
+        for (a, b), per_rc, per_hs in zip(pairs, recs, hist):
+            keys = _pair_keys(flag_sets[b], flag_sets[a])
+            for L, rc, hs in (zip(loads, per_rc, per_hs) if boot else [(None, per_rc, per_hs)]):
+                d = summary.pair_spread(rc, hs, edges, level=level) if boot else summary.pair_derived(rc, hs, edges)
+                for c in range(rc.shape[-1]):
+                    for m in summary.JOBDIST_QUANTITIES:
+                        for e, edge in enumerate(edges):
+                            tail = ([int(d["replicas"][c]), level] + [float(d[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS] if boot
+                                    else [int(d["jobs"][c]), float(d[m + "_cdf"][c, e])])
+                            w.writerow(keys + ([L] + _block_val(block_len) if boot else []) + [c] + _class_range(c, bounds) + [m, edge] + tail)
+
+
+def write_paired_summary_csv(path, flag_sets, pairs, records, loads=None, level=0.95, block_len=None):
+    """one line per (configuration b of a pair[, load]): b's flags, the base schedule[, the load, block_len], the
+    replicas and summary.paired_spread's columns: the replica-level differences b - base of the makespan and of every
+    derived number (records: (configurations, loads, replicas) with loads, else one record per configuration)"""
+    import csv
+    boot = loads is not None
+
+    def shape(fl):
+        cl = Infrastructure(fl).gs_cluster()
+        return cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) if boot else []) + ["replicas", "level"] + summary.paired_columns())
+        for a, b in pairs:
+            sa, sb = shape(flag_sets[a]), shape(flag_sets[b])
+            per = zip(loads, records[a], records[b]) if boot else [(None, records[a:a + 1], records[b:b + 1])]
+            for L, ra, rb in per:
+                sp = summary.paired_spread(ra, rb, sa, sb, level=level)
+                w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + ([L] + _block_val(block_len) if boot else []) + [len(ra), level]
+                           + summary.paired_flat(sp))
+
+
 def write_summary_csv(path, flag_sets, records):
     """one line per configuration: its flags (SUMMARY_KEYS), the summary fields and the derived numbers (summary.py)"""
     import csv
@@ -539,6 +687,20 @@ def main(argv=None):
                     help=f"with --jobdist: CDF edges in ticks (strictly increasing, at most {capi.JOBDIST_MAX_EDGES}; default 1 2 4 ... 2^30)")
     ap.add_argument("--jobdist-cdf", default=None, metavar="FILE",
                     help="with --jobdist: one CSV line per (configuration[, load], class, quantity, edge) with the CDF value or its spread")
+    ap.add_argument("--compare", default=None, metavar="BASE",
+                    help="with --summary: pair every other --schedule with BASE (one of the --schedule values) on the same trace and "
+                         "repeat (with --bootstrap: the same load and replica) and compare them job by job on the GPU")
+    ap.add_argument("--paired", default=None, metavar="FILE",
+                    help="with --compare: one CSV line per (configuration, class, quantity) with the per-job differences "
+                         "d = x - x_BASE of wait / turnaround / jct; with --bootstrap one line per (configuration, load, class, "
+                         "quantity) with their spread across replicas.  Classes: --gpu-classes")
+    ap.add_argument("--paired-cdf", default=None, metavar="FILE", help="with --paired: the CDF of d at the --diff-edges")
+    ap.add_argument("--diff-edges", type=int, nargs="+", default=None, metavar="E",
+                    help=f"with --compare: signed CDF edges of d in ticks (strictly increasing, at most {capi.JOBDIST_MAX_EDGES}; "
+                         "default -2^30 ... -2 -1 0 1 2 ... 2^30)")
+    ap.add_argument("--paired-summary", default=None, metavar="FILE",
+                    help="with --compare: one CSV line per configuration (with --bootstrap: per configuration and load) with the "
+                         "replica-level differences from BASE of the makespan and of every derived number")
     a = ap.parse_args(argv)
     jobdist = None
     if a.jobdist is not None:
@@ -548,8 +710,18 @@ def main(argv=None):
             jobdist = check_jobdist((a.gpu_classes or (), DEFAULT_CDF_EDGES if a.cdf_edges is None else a.cdf_edges))
         except ValueError as e:
             ap.error(str(e))
-    elif a.gpu_classes is not None or a.cdf_edges is not None or a.jobdist_cdf is not None:
-        ap.error("--gpu-classes, --cdf-edges and --jobdist-cdf need --jobdist FILE")
+    elif a.cdf_edges is not None or a.jobdist_cdf is not None or (a.gpu_classes is not None and a.paired is None):
+        ap.error("--gpu-classes, --cdf-edges and --jobdist-cdf need --jobdist FILE (--gpu-classes: or --paired FILE)")
+    if a.compare is None:
+        if a.paired is not None or a.paired_cdf is not None or a.diff_edges is not None or a.paired_summary is not None:
+            ap.error("--paired, --paired-cdf, --diff-edges and --paired-summary need --compare BASE")
+    else:
+        if not a.summary:
+            ap.error("--compare needs --summary FILE")
+        if a.schedule.count(a.compare) != 1:
+            ap.error(f"--compare: {a.compare} must be exactly one of the --schedule values")
+        if a.paired_cdf is not None and a.paired is None:
+            ap.error("--paired-cdf needs --paired FILE")
     timeline = None
     if a.timeline is not None:
         if not a.summary:
@@ -579,6 +751,21 @@ def main(argv=None):
                                        num_node_p_switch=a.num_node_p_switch, num_queue=a.num_queue, num_buffer=a.num_buffer,
                                        log_path=os.path.join(f"batched_{tag}", f"{scheme}_{sc}"),
                                        seed=a.seed if a.seed < 0 else a.seed + rep))
+    compare = None
+    if a.compare is not None:
+        pairs, S, R = [], len(a.schedule), a.repeats
+        base = a.schedule.index(a.compare)
+        for i, fl in enumerate(sets):                     # sets[(trace * S + schedule) * R + repeat]
+            if fl.schedule == a.compare:
+                continue
+            j = (i // (S * R) * S + base) * R + i % R
+            if _is_utilisation_aware(fl) != _is_utilisation_aware(sets[j]):
+                ap.error(f"--compare: {fl.schedule} and {a.compare} run on different engines; such pairs are not supported")
+            pairs.append((j, i))
+        try:
+            compare = check_compare((pairs, a.gpu_classes or (), DEFAULT_DIFF_EDGES if a.diff_edges is None else a.diff_edges), sets)
+        except ValueError as e:
+            ap.error(str(e))
     if a.bootstrap is not None:
         loads = a.load or [1.0]
         try:
@@ -587,8 +774,18 @@ def main(argv=None):
             ap.error(str(e))
         bl = a.block_len
         res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist,
-                                  block_len=1 if bl is None else bl)
-        recs, rest = (res, ()) if timeline is None and jobdist is None else (res[0], res[1:])
+                                  block_len=1 if bl is None else bl, compare=compare)
+        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None else (res[0], res[1:])
+        if compare is not None:
+            pairs, cmp_bounds, cmp_edges = compare
+            prec, phist = rest[-1]
+            rest = rest[:-1]
+            if a.paired:
+                write_paired_ci_csv(a.paired, sets, pairs, loads, prec, phist, cmp_bounds, cmp_edges, block_len=bl)
+            if a.paired_cdf:
+                write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges, loads=loads, block_len=bl)
+            if a.paired_summary:
+                write_paired_summary_csv(a.paired_summary, sets, pairs, recs, loads=loads, block_len=bl)
         if timeline is not None:
             write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0], block_len=bl)
         if jobdist is not None:
@@ -602,8 +799,18 @@ def main(argv=None):
         print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads x {a.bootstrap} replicas")
         return
     if a.summary:
-        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist)
-        recs, rest = (res, ()) if timeline is None and jobdist is None else (res[0], res[1:])
+        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare)
+        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None else (res[0], res[1:])
+        if compare is not None:
+            pairs, cmp_bounds, cmp_edges = compare
+            prec, phist = rest[-1]
+            rest = rest[:-1]
+            if a.paired:
+                write_paired_csv(a.paired, sets, pairs, prec, phist, cmp_bounds, cmp_edges)
+            if a.paired_cdf:
+                write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges)
+            if a.paired_summary:
+                write_paired_summary_csv(a.paired_summary, sets, pairs, recs)
         if timeline is not None:
             write_timeline_csv(a.timeline, sets, rest[0], timeline[0])
         if jobdist is not None:

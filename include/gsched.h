@@ -453,6 +453,42 @@ typedef struct gs_jclass {
 int gs_set_jobdist(gs_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges);
 int gs_fetch_jobdist(gs_handle h, int first, int count, gs_jclass *classes_out, uint32_t *hist_out);
 
+/* ---- paired per-job comparison of two replicas on the same trace ------------------------------------------
+ * A pair (a, b) is two replicas of one handle that hold the same trace: the same job count n and, for every j < n,
+ * a byte-equal gs_jobin record (gs_horus_compare: equal fields as taken by gs_horus_load_trace).  They may differ in
+ * anything else (policy, cluster, dlas limits, network cost); (a, a) is a pair too.  Per job j the quantities x are
+ * gs_summary's wait, turnaround and jct; job j is finished in a run if it is in that replica's finish order so far,
+ * so a pair may be compared after any gs_run window (gs_summarize is not needed first).  Classes are jobdist's
+ * (C - 1 strictly increasing bounds >= 1, 1 <= C <= 8); both runs share the trace, so they agree on every class.
+ * Every x is a non-negative int32 (start >= arrive, end >= arrive), so d = x_b - x_a has |d| <= 2^31 - 1 and both d
+ * and -d fit in int32.  Per (pair, class) one gs_jpair; its order statistics sort the k = `jobs` differences
+ * ascending, d_(0) <= ... <= d_(k-1), and with rank_t the nearest rank of gs_summary (50 / 90 / 95 / 99 / 100 %) give
+ * q_hi[m][t] = d_(rank_t) and q_lo[m][t] = d_(k-1-rank_t): q_hi[m][4] is the maximum, q_lo[m][4] the minimum, and
+ * swapping a pair gives q_hi(b, a) = -q_lo(a, b).  0 when k = 0.
+ * Optional CDF of d: E strictly increasing signed int32 edges (0 <= E <= 255), per (pair, class, quantity) E + 1
+ * uint32 counts, value d in bin #(edges < d) (jobdist's rule).  Every field is an integer; a repeated call gives the
+ * same bytes.                                                                                                 */
+typedef struct gs_jpair {
+  int64_t jobs;                      /* jobs of the class finished in both runs                                    */
+  int64_t only_a, only_b;            /* finished in run a only / in run b only                                     */
+  int64_t lt[3], eq[3], gt[3];       /* per quantity (wait, turnaround, jct), d = x_b - x_a: #(d < 0), #(d == 0),
+                                        #(d > 0) over the `jobs` jobs                                               */
+  int64_t d_sum[3];
+  uint64_t d_sq_lo[3], d_sq_hi[3];   /* exact 128-bit sum of d^2                                                   */
+  int32_t q_hi[3][5];                /* d ascending, gs_summary's nearest ranks 50 / 90 / 95 / 99 / 100 %          */
+  int32_t q_lo[3][5];                /* d descending, the same ranks: 50 % and 10 / 5 / 1 / 0 % from below         */
+} gs_jpair;
+/* gs_compare: npairs pairs (a[i], b[i]) into out (pair-major, npairs * C records) and, when hist_out is not NULL,
+ * npairs * C * 3 * (E + 1) counts ([pair][class][wait, turnaround, jct][bin]).  Synchronous; one kernel launch when
+ * npairs > 0, none when npairs == 0.  Uses the handle's summary scratch in stream order and touches no summary
+ * accumulator, watermark, timeline or jobdist state.  kernel_ms (may be NULL) receives the kernel's device time.
+ * Errors leave out, hist_out and the handle unchanged: GS_ERR_ARG for npairs < 0, a NULL a, b or out with npairs > 0,
+ * an index outside [0, nsims), classes or edges gs_set_jobdist refuses or C = 0, pairs with different job counts,
+ * and pairs whose traces differ (found on the device; gs_last_error names the first such pair); GS_ERR_STATE for
+ * a replica that has not run.                                                                                 */
+int gs_compare(gs_handle h, int32_t npairs, const int32_t *a, const int32_t *b, int32_t nclasses, const int32_t *bounds,
+               int32_t nedges, const int32_t *edges, gs_jpair *out, uint32_t *hist_out, double *kernel_ms);
+
 /* ---- bootstrap replicas generated on the device ---------------------------------------------------------
  * gs_boot_population gives the handle one base trace P of k >= 1 records (admission order, the gs_load_trace rules;
  * validated once, copied to the device); D holds its k - 1 inter-arrival gaps D[i] = P[i+1].arrive_tick - P[i].arrive_tick.

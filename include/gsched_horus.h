@@ -108,6 +108,11 @@ int gs_horus_fetch_timeline(gs_horus_handle h, int32_t first, int32_t count, gs_
  * finished jobs as its job part.  Same meaning and errors as gs_set_jobdist / gs_fetch_jobdist.                 */
 int gs_horus_set_jobdist(gs_horus_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges);
 int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t count, gs_jclass *classes_out, uint32_t *hist_out);
+/* Paired per-job comparison (gs_jpair, gsched.h: gs_compare) of replicas of this handle that hold the same trace: equal
+ * arrival, gpus, gpu_per_container, duration, memory, utilisation and mean-memory fields for every job.  The same
+ * outputs, launches and errors as gs_compare; a replica has run once gs_horus_run has prepared it.           */
+int gs_horus_compare(gs_horus_handle h, int32_t npairs, const int32_t *a, const int32_t *b, int32_t nclasses, const int32_t *bounds,
+                     int32_t nedges, const int32_t *edges, gs_jpair *out, uint32_t *hist_out, double *kernel_ms);
 /* Kernel mapping (no reference counterpart): simulations per warp, 1 (default: lane 0 of each warp) or 32; 0 = one
  * simulation per warp with all 32 lanes scoring a candidate job's devices together (gs_horus_coop_kernel). */
 int gs_horus_set_lanes(gs_horus_handle h, int lanes_per_warp);
