@@ -272,6 +272,8 @@ def load_library():
     lib.gs_boot_population.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
     lib.gs_boot_traces.argtypes = [C.c_void_p, C.c_void_p, f64p]
     lib.gs_boot_traces_blocked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, f64p]
+    lib.gs_boot_mixes.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+    lib.gs_boot_traces_mixed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, f64p]
     lib.gs_fetch_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.gs_set_timeline.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
     lib.gs_fetch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
@@ -281,7 +283,7 @@ def load_library():
                                C.c_void_p, C.c_void_p, f64p]
     lib.gs_compare.restype = C.c_int
     for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
-                 "gs_boot_traces_blocked", "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
+                 "gs_boot_traces_blocked", "gs_boot_mixes", "gs_boot_traces_mixed", "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
         getattr(lib, name).restype = C.c_int
     lib.gs_switch_yarn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, f64p, C.c_int64,
                                    C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_int64]
@@ -701,23 +703,51 @@ class Engine:
         packed = table_or_packed.packed() if hasattr(table_or_packed, "packed") else table_or_packed
         packed = np.ascontiguousarray(packed, dtype=JOBIN_DTYPE)
         self._check(self.lib.gs_boot_population(self.h, packed.ctypes.data_as(C.c_void_p), len(packed)), "gs_boot_population")
+        self._pop_k = len(packed)
 
-    def boot_traces(self, params, with_time=False, block_len=None):
+    def boot_mixes(self, weights):
+        """the job mixes of the current population (gs_boot_mixes): `weights` holds one row of uint32 weights per mix,
+        one weight per population record (shape (mixes, k)); mix m draws record i with probability w_i / sum(w).
+        An empty array (shape (0, k) or (0,)) clears them"""
+        w = np.asarray(weights)
+        if w.size == 0:
+            self._check(self.lib.gs_boot_mixes(self.h, 0, None), "gs_boot_mixes")
+            return
+        if w.ndim != 2 or w.dtype.kind not in "iu" or (w < 0).any() or (w > 2 ** 32 - 1).any():
+            raise ValueError("boot_mixes: expected a 2-d array of uint32 weights (mixes, population records)")
+        k = getattr(self, "_pop_k", None)
+        if k is not None and w.shape[1] != k:
+            raise ValueError(f"boot_mixes: expected one weight per population record ({k}), got {w.shape[1]}")
+        w = np.ascontiguousarray(w, dtype=np.uint32)
+        self._check(self.lib.gs_boot_mixes(self.h, len(w), w.ctypes.data_as(C.c_void_p)), "gs_boot_mixes")
+
+    def boot_traces(self, params, with_time=False, block_len=None, mix=None):
         """draw every replica's trace from the population: `params` holds one BOOT_PARAMS_DTYPE record per replica.
         block_len: the mean block length L of a block bootstrap (gs_boot_traces_blocked), one integer for every
-        replica or one per replica; None draws iid replicas (gs_boot_traces).  with_time: returns the generator's
-        kernel milliseconds"""
+        replica or one per replica; None draws iid replicas (gs_boot_traces).  mix: the job mix of boot_mixes each
+        replica draws its rows from (gs_boot_traces_mixed), one index for every replica or one per replica, -1 for
+        the unweighted bootstrap; None draws every replica unweighted.  with_time: returns the generator's kernel
+        milliseconds"""
         params = np.ascontiguousarray(params, dtype=BOOT_PARAMS_DTYPE)
         if params.shape != (self.nsims,):
             raise ValueError(f"boot_traces: one parameter record per replica ({self.nsims}), got shape {params.shape}")
         ms = C.c_double(0.0)
-        if block_len is None:
-            self._check(self.lib.gs_boot_traces(self.h, params.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces")
-        else:
+        if block_len is not None:
             L = np.asarray(block_len)
             if L.dtype.kind not in "iu" or L.shape not in ((), (self.nsims,)) or (L < 0).any() or (L > 2 ** 32 - 1).any():
                 raise ValueError(f"boot_traces: block_len must be one uint32 or one per replica ({self.nsims})")
             L = np.ascontiguousarray(np.broadcast_to(L, (self.nsims,)), dtype=np.uint32)
+        if mix is not None:
+            M = np.asarray(mix)
+            if M.dtype.kind not in "iu" or M.shape not in ((), (self.nsims,)) or (M < -2 ** 31).any() or (M > 2 ** 31 - 1).any():
+                raise ValueError(f"boot_traces: mix must be one int32 or one per replica ({self.nsims})")
+            M = np.ascontiguousarray(np.broadcast_to(M, (self.nsims,)), dtype=np.int32)
+            self._check(self.lib.gs_boot_traces_mixed(self.h, params.ctypes.data_as(C.c_void_p),
+                                                      None if block_len is None else L.ctypes.data_as(C.c_void_p),
+                                                      M.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces_mixed")
+        elif block_len is None:
+            self._check(self.lib.gs_boot_traces(self.h, params.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces")
+        else:
             self._check(self.lib.gs_boot_traces_blocked(self.h, params.ctypes.data_as(C.c_void_p), L.ctypes.data_as(C.c_void_p), C.byref(ms)),
                         "gs_boot_traces_blocked")
         self._n = [int(k) for k in params["n"].tolist()]

@@ -9,7 +9,7 @@
 //   gap         g_0 = 0, g_j = D[floor(w1 * (K - 1) / 2^64)] (0 when K = 1)
 //   arrival     arrive_j = floor((g_0 + ... + g_j) * gap_num / gap_den), exact integers
 //   record      {arrive_j, P[r_j].gpus, P[r_j].gpu_per_task, 0, P[r_j].mem_bytes, P[r_j].duration}
-// w3 is unused, and so is w2 unless the replica is blocked.
+// w3 is unused unless the replica is mixed, and w2 unless it is blocked.
 //
 // Blocked replicas (gs_boot_traces_blocked, the stationary bootstrap of Politis & Romano) resample runs of consecutive
 // jobs of geometric length with mean L, so that a trace's bursts survive.  Job 0 starts a block; job j > 0 starts one
@@ -21,16 +21,26 @@
 // __host__ __device__: tests/emu/boot_emu.cpp and tests/emu/boot_block_emu.cpp run them with g++, and
 // tracegen.bootstrap_packed is their numpy mirror.
 //
+// Mixed replicas (gs_boot_mixes / gs_boot_traces_mixed) draw row i with probability w_i / T for integer weights w
+// (T = sum w_i >= 1) through an exact integer alias table {U_i, A_i} (Walker / Vose; gs_boot_alias_build): with
+// c = floor(w0 * K / 2^64), the row the unweighted bootstrap takes, and u = floor(w3 * T / 2^64), job j takes
+//   row  c if u < U_c, else A_c
+// Blocked mixed replicas apply this to s_b at block starts only; a block still continues through the base trace in
+// order.  Equal weights give U_i = T everywhere, so every job keeps c: the unweighted replica byte for byte.
+//
 // gs_boot_kernel: one block per replica walks its jobs in chunks of the block size -- a Philox block per job, a gather
 // of the population row, a block-wide inclusive int64 scan of the gaps with a carry between chunks -- and writes the
 // chunk's 32-byte records through shared memory into the replica's slot of the trace arena with contiguous 16-byte
 // stores.  The same pass reduces the replica's span-pool bound (sum of min(tasks, M)) and last arrival tick.  The
 // blocked instantiation first runs a block-wide inclusive max-scan of the key (j << 32) | s_j of every block start
 // (0 for other jobs), carried between chunks like the gap sum, so each job reads b_j and s_{b_j} from its scanned key
-// however many chunks and wraps of the population its block spans.
+// however many chunks and wraps of the population its block spans.  The mixed instantiations (MIXED = true) read a
+// replica's table offset and T from one extra per-replica record and load one 16-byte table entry per job.
 #pragma once
 
 #include <stdint.h>
+
+#include <vector>
 
 #include "gsched.h"
 
@@ -106,6 +116,59 @@ GS_BOOT_HD long long gs_boot_block_row(long long key, long long j, long long K) 
 // Gap index of job j (-1: g_j = 0): the iid pick for a block start or a wrapped row, else the row's own preceding gap.
 GS_BOOT_HD long long gs_boot_block_gap(bool start, long long row, long long iid_gap) { return (start || row == 0) ? iid_gap : row - 1; }
 
+// One column of an alias table: a job whose column is c keeps row c iff floor(w3 * T / 2^64) < u, else takes row a.
+struct alignas(16) GsBootAlias { uint64_t u, a; };
+
+// The alias table of the K integer weights w (Walker / Vose, exact integers): with T = sum w_i and q_i = w_i * K
+// (both below 2^63 for K < 2^31), take FIFO worklists S = {i : q_i < T} and G = {i : q_i >= T} in ascending row order;
+// while both are non-empty, take s from the front of S, let g be the front of G, set U_s = q_s, A_s = g and
+// q_g -= T - q_s, and move g to the back of S once q_g < T.  Every row still in G gets U_i = T, A_i = i.  Returns T and
+// fills tab[K]; T = 0 (all weights 0) writes nothing.  Row m is then drawn with probability w_m / T: U_m plus the
+// T - U_i of every other column i that aliases m is w_m * K.
+static inline uint64_t gs_boot_alias_build(const uint32_t *w, long long K, GsBootAlias *tab) {
+  uint64_t T = 0;
+  for (long long i = 0; i < K; ++i) T += w[i];
+  if (T == 0) return 0;
+  std::vector<uint64_t> q((size_t)K);
+  std::vector<long long> S, G;
+  S.reserve((size_t)K); G.reserve((size_t)K);
+  for (long long i = 0; i < K; ++i) {
+    q[(size_t)i] = (uint64_t)w[i] * (uint64_t)K;
+    (q[(size_t)i] < T ? S : G).push_back(i);
+  }
+  size_t s0 = 0, g0 = 0;
+  while (s0 < S.size() && g0 < G.size()) {
+    const long long s = S[s0++], g = G[g0];
+    tab[s].u = q[(size_t)s]; tab[s].a = (uint64_t)g;
+    q[(size_t)g] -= T - q[(size_t)s];
+    if (q[(size_t)g] < T) { ++g0; S.push_back(g); }
+  }
+  for (; g0 < G.size(); ++g0) { tab[G[g0]].u = T; tab[G[g0]].a = (uint64_t)G[g0]; }   // S is empty here
+  return T;
+}
+
+// Row of a job whose unweighted row (column) is c under the alias table tab with weight sum T; T = 0 is the
+// unweighted replica of a mixed launch (mix -1) and keeps c.
+GS_BOOT_HD long long gs_boot_alias_pick(const GsBootAlias *tab, uint64_t T, long long c, uint64_t w3) {
+  if (T == 0) return c;
+#ifdef __CUDA_ARCH__
+  const ulonglong2 e = __ldg(reinterpret_cast<const ulonglong2 *>(tab + c));
+  return gs_boot_mulhi(w3, T) < e.x ? c : (long long)e.y;
+#else
+  return gs_boot_mulhi(w3, T) < tab[c].u ? c : (long long)tab[c].a;
+#endif
+}
+
+// gs_boot_pick_blocked of a mixed replica: row is the weighted pick (s_j when blocked), gap the iid gap index; returns
+// whether job j starts a block (always true for L = 1).
+GS_BOOT_HD bool gs_boot_pick_mixed(uint64_t seed, uint64_t stream, long long j, long long K, uint64_t L, const GsBootAlias *tab, uint64_t T,
+                                   long long &row, long long &gap) {
+  const GsPhilox b = gs_boot_philox(seed, stream, (uint64_t)j + 1u, 0, 0, 0);
+  row = gs_boot_alias_pick(tab, T, (long long)gs_boot_mulhi(b.w[0], (uint64_t)K), b.w[3]);
+  gap = (j > 0 && K > 1) ? (long long)gs_boot_mulhi(b.w[1], (uint64_t)(K - 1)) : -1;
+  return j == 0 || gs_boot_mulhi(b.w[2], L) == 0;
+}
+
 // arrive = floor(S * gap_num / gap_den) for a gap sum S >= 0.  The caller bounds S * gap_num below 2^62
 // (gs_boot_arrive_bound), so the product fits in 64 bits.
 GS_BOOT_HD int gs_boot_arrive(long long S, int gap_num, int gap_den) { return (int)(S * (long long)gap_num / gap_den); }
@@ -127,11 +190,27 @@ struct GsBootRep {        // one replica's parameters as the kernel reads them
   uint32_t block_len;     // mean block length L (read by the blocked instantiation only)
 };
 
+struct alignas(16) GsBootMix {   // one replica's alias table as the mixed instantiations read it
+  uint64_t T;                    // weight sum; 0: unweighted (mix -1)
+  long long off;                 // first entry of the replica's table in tabs
+};
+
+// gs_boot_pick_mixed of job j of this block's replica, whose table is {T, off} = mixes[blockIdx.x] (T = 0: mix -1).
+static __device__ __forceinline__ bool gs_boot_pick_in_mix(const GsBootMix *mixes, const GsBootAlias *tabs, uint64_t seed, uint64_t stream,
+                                                           long long j, long long K, uint64_t L, long long &row, long long &gap) {
+  const ulonglong2 m = __ldg(reinterpret_cast<const ulonglong2 *>(mixes + blockIdx.x));
+  return gs_boot_pick_mixed(seed, stream, j, K, L, tabs + m.y, m.x, row, gap);
+}
+
 // out[2 b] = sum over the jobs of min(tasks, M), out[2 b + 1] = last arrival tick (0 without jobs).
 // BLOCKED = false is the iid bootstrap; BLOCKED = true draws blocks of mean length R.block_len (1 gives the iid trace).
-template <bool BLOCKED>
+// MIXED = true picks rows (block starts when blocked) through the alias table {T, off} = mixes[b] at tabs + off, two
+// parameters appended as the pack `mix` = (const GsBootMix *mixes, const GsBootAlias *tabs).  The other
+// instantiations have an empty pack: their parameter list, and so their code, is the one they had before mixes.
+template <bool BLOCKED, bool MIXED, class... Mix>
 __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRep *reps, const JobIn *pop, const int *gaps, long long K,
-                                                                 JobIn *arena, long long stride_recs, long long *out) {
+                                                                 JobIn *arena, long long stride_recs, long long *out, Mix... mix) {
+  static_assert(sizeof...(Mix) == (MIXED ? 2 : 0), "the mixed instantiations take (mixes, tabs)");
   __shared__ int4 stage[2 * GS_BOOT_THREADS];
   __shared__ long long warp_tot[GS_BOOT_THREADS / 32];
   __shared__ long long warp_key[BLOCKED ? GS_BOOT_THREADS / 32 : 1];
@@ -148,7 +227,13 @@ __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRe
     if constexpr (BLOCKED) {
       long long s = 0, gi = -1;
       bool start = false;
-      if (in) start = gs_boot_pick_blocked(R.seed, R.stream, j, K, R.block_len, s, gi);
+      if (in) {
+        if constexpr (MIXED) {
+          start = gs_boot_pick_in_mix(mix..., R.seed, R.stream, j, K, R.block_len, s, gi);
+        } else {
+          start = gs_boot_pick_blocked(R.seed, R.stream, j, K, R.block_len, s, gi);
+        }
+      }
       long long key = gs_boot_block_key(start, j, s);   // inclusive max-scan: lanes, then warps, then the carry
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -169,7 +254,11 @@ __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRe
       }
     } else if (in) {
       long long row, gi;
-      gs_boot_pick(R.seed, R.stream, j, K, row, gi);
+      if constexpr (MIXED) {
+        gs_boot_pick_in_mix(mix..., R.seed, R.stream, j, K, 1u, row, gi);
+      } else {
+        gs_boot_pick(R.seed, R.stream, j, K, row, gi);
+      }
       const int4 *src = reinterpret_cast<const int4 *>(pop + row);
       lo = __ldg(src); hi = __ldg(src + 1);
       if (gi >= 0) g = __ldg(gaps + gi);

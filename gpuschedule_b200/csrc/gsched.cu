@@ -127,6 +127,8 @@ struct gs_engine {
   GsJdCfg jd{};                                          // jd.nclasses = 0: off
   // gs_boot_population: the records of the base trace, then its k - 1 gaps (int32)
   void *d_pop = nullptr; int64_t pop_k = 0; int64_t pop_max_gap = 0; double pop_max_need = 1.0;
+  // gs_boot_mixes: nmix alias tables of pop_k entries each, mix-major, and their weight sums
+  GsBootAlias *d_mix = nullptr; int32_t nmix = 0; std::vector<uint64_t> mix_T;
 };
 
 static std::string g_create_err;
@@ -207,6 +209,7 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->d_jd) cudaFree(h->d_jd);
   if (h->d_jd_hist) cudaFree(h->d_jd_hist);
   if (h->d_pop) cudaFree(h->d_pop);
+  if (h->d_mix) cudaFree(h->d_mix);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
   if (h->comm_buf) cudaFree(h->comm_buf);
   if (h->e0) cudaEventDestroy(h->e0);
@@ -1367,8 +1370,48 @@ extern "C" int gs_boot_population(gs_handle h, const gs_jobin *trace, int64_t k)
   cudaError_t e1 = cudaMemcpy(d, ji, sizeof(JobIn) * (size_t)k, cudaMemcpyHostToDevice);
   cudaError_t e2 = cudaMemcpy((unsigned char *)d + off_gaps, gaps.data(), 4 * gaps.size(), cudaMemcpyHostToDevice);
   if (e1 != cudaSuccess || e2 != cudaSuccess) { cudaFree(d); return fail(h, GS_ERR_CUDA, "gs_boot_population: upload failed"); }
-  if (h->d_pop) { CU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_pop); }
+  if (h->d_pop || h->d_mix) CU(cudaStreamSynchronize(h->stream));
+  if (h->d_pop) cudaFree(h->d_pop);
+  if (h->d_mix) cudaFree(h->d_mix);                     // the tables belong to the previous population
   h->d_pop = d; h->pop_k = k; h->pop_max_gap = max_gap; h->pop_max_need = max_need;
+  h->d_mix = nullptr; h->nmix = 0; h->mix_T.clear();
+  return GS_OK;
+}
+
+extern "C" int gs_boot_mixes(gs_handle h, int32_t nmix, const uint32_t *weights) {
+  if (!h) return GS_ERR_ARG;
+  if (nmix < 0) return fail(h, GS_ERR_ARG, "gs_boot_mixes: nmix must be >= 0");
+  if (nmix > 0 && !weights) return fail(h, GS_ERR_ARG, "gs_boot_mixes: weights is NULL");
+  if (!h->d_pop) return fail(h, GS_ERR_STATE, "gs_boot_mixes: call gs_boot_population first");
+  // every check before anything changes: a refused call leaves the tables as they were
+  const int64_t K = h->pop_k;
+  for (int32_t m = 0; m < nmix; ++m) {
+    const uint32_t *w = weights + (size_t)m * (size_t)K;
+    bool any = false;
+    for (int64_t i = 0; i < K && !any; ++i) any = w[i] != 0;
+    if (!any) return fail(h, GS_ERR_ARG, "gs_boot_mixes: mix " + std::to_string(m) + " has weight sum 0");
+  }
+  CU(cudaSetDevice(h->device));
+  GsBootAlias *d = nullptr;
+  std::vector<uint64_t> T((size_t)nmix);
+  if (nmix > 0) {
+    if ((uint64_t)nmix * (uint64_t)K > (uint64_t)(SIZE_MAX / 2) / sizeof(GsBootAlias))
+      return fail(h, GS_ERR_CUDA, "gs_boot_mixes: the tables do not fit in memory");
+    if (cudaMalloc(&d, sizeof(GsBootAlias) * (size_t)nmix * (size_t)K) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(h, GS_ERR_CUDA, "gs_boot_mixes: allocation of the alias tables failed");
+    }
+    std::vector<GsBootAlias> tab((size_t)K);              // one mix at a time: host memory stays at one table
+    for (int32_t m = 0; m < nmix; ++m) {
+      T[(size_t)m] = gs_boot_alias_build(weights + (size_t)m * (size_t)K, K, tab.data());
+      if (cudaMemcpy(d + (size_t)m * (size_t)K, tab.data(), sizeof(GsBootAlias) * (size_t)K, cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaFree(d);
+        return fail(h, GS_ERR_CUDA, "gs_boot_mixes: upload failed");
+      }
+    }
+  }
+  if (h->d_mix) { CU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_mix); }
+  h->d_mix = d; h->nmix = nmix; h->mix_T.swap(T);
   return GS_OK;
 }
 
@@ -1377,6 +1420,11 @@ extern "C" int gs_boot_traces(gs_handle h, const gs_boot_params *params, double 
 }
 
 extern "C" int gs_boot_traces_blocked(gs_handle h, const gs_boot_params *params, const uint32_t *block_len, double *kernel_ms) {
+  return gs_boot_traces_mixed(h, params, block_len, nullptr, kernel_ms);
+}
+
+extern "C" int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params, const uint32_t *block_len, const int32_t *mix,
+                                    double *kernel_ms) {
   if (!h) return GS_ERR_ARG;
   if (!params) return fail(h, GS_ERR_ARG, "gs_boot_traces: params is NULL");
   if (!h->d_pop) return fail(h, GS_ERR_STATE, "gs_boot_traces: call gs_boot_population first");
@@ -1384,6 +1432,7 @@ extern "C" int gs_boot_traces_blocked(gs_handle h, const gs_boot_params *params,
   std::vector<GsBootRep> reps((size_t)h->nsims);
   int64_t nmax = 1;
   bool blocked = false;                                 // some replica has L > 1: the blocked instantiation
+  bool mixed = false;                                   // some replica has a mix >= 0: the mixed instantiation
   for (int i = 0; i < h->nsims; ++i) {
     const SimHost &s = h->sims[(size_t)i];
     const gs_boot_params &p = params[i];
@@ -1394,27 +1443,41 @@ extern "C" int gs_boot_traces_blocked(gs_handle h, const gs_boot_params *params,
     if (gs_boot_arrive_bound(p.n, h->pop_max_gap, p.gap_num, p.gap_den) >= 0x7fffffffll)
       return fail(h, GS_ERR_ARG, "gs_boot_traces: the last arrival tick can reach 2^31 - 1 (fewer jobs or a smaller gap scale)");
     if (block_len && block_len[i] == 0) return fail(h, GS_ERR_ARG, "gs_boot_traces_blocked: block_len must be >= 1");
+    if (mix && (mix[i] < -1 || mix[i] >= h->nmix))
+      return fail(h, GS_ERR_ARG, "gs_boot_traces_mixed: mix index out of range [-1, nmix) for replica " + std::to_string(i));
     GsBootRep &r = reps[(size_t)i];
     r.seed = p.seed; r.stream = p.stream; r.n = p.n; r.gap_num = p.gap_num; r.gap_den = p.gap_den;
     r.M = s.cl.num_switch * s.cl.num_node_p_switch; r.block_len = block_len ? block_len[i] : 1u;
     blocked = blocked || r.block_len > 1;
+    mixed = mixed || (mix && mix[i] >= 0);
     nmax = std::max(nmax, p.n);
+  }
+  std::vector<GsBootMix> mixes(mixed ? (size_t)h->nsims : 0);
+  for (size_t i = 0; i < mixes.size(); ++i) {
+    mixes[i].T = mix[i] >= 0 ? h->mix_T[(size_t)mix[i]] : 0;
+    mixes[i].off = mix[i] >= 0 ? (long long)mix[i] * (long long)h->pop_k : 0;
   }
   CU(cudaSetDevice(h->device));
   int rc = reserve_trace_arena(h, nmax);
   if (rc) return rc;
-  const size_t off_out = align_up(sizeof(GsBootRep) * reps.size());
-  rc = ensure_scratch(h, off_out + 16 * reps.size());
+  const size_t off_out = align_up(sizeof(GsBootRep) * reps.size()), off_mix = align_up(off_out + 16 * reps.size());
+  rc = ensure_scratch(h, mixed ? off_mix + sizeof(GsBootMix) * mixes.size() : off_out + 16 * reps.size());
   if (rc) return rc;
   unsigned char *d = (unsigned char *)h->d_scratch;
   std::vector<long long> res(2 * reps.size());
   const JobIn *pop = (const JobIn *)h->d_pop;
   const int *gaps = (const int *)((unsigned char *)h->d_pop + align_up(sizeof(JobIn) * (size_t)h->pop_k));
   CU(cudaMemcpyAsync(d, reps.data(), sizeof(GsBootRep) * reps.size(), cudaMemcpyHostToDevice, h->stream));
+  if (mixed) CU(cudaMemcpyAsync(d + off_mix, mixes.data(), sizeof(GsBootMix) * mixes.size(), cudaMemcpyHostToDevice, h->stream));
   CU(cudaEventRecord(h->e0, h->stream));
-  (blocked ? gs_boot_kernel<true> : gs_boot_kernel<false>)<<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>(
-      (const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena, (long long)(h->tarena_stride / sizeof(JobIn)),
-      (long long *)(d + off_out));
+  const long long stride = (long long)(h->tarena_stride / sizeof(JobIn));
+  if (mixed)
+    (blocked ? gs_boot_kernel<true, true, const GsBootMix *, const GsBootAlias *> : gs_boot_kernel<false, true, const GsBootMix *, const GsBootAlias *>)
+        <<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>((const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena, stride,
+                                                               (long long *)(d + off_out), (const GsBootMix *)(d + off_mix), h->d_mix);
+  else
+    (blocked ? gs_boot_kernel<true, false> : gs_boot_kernel<false, false>)<<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>(
+        (const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena, stride, (long long *)(d + off_out));
   CU(cudaGetLastError());
   h->launches += 1;
   CU(cudaEventRecord(h->e1, h->stream));

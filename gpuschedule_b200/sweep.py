@@ -300,7 +300,41 @@ def load_gap_scale(load):
     return f.numerator, f.denominator
 
 
-def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1):
+def check_mix(mix):
+    """(class bounds, [multipliers per mix]) of a mix argument as tuples of ints, or ValueError: bounds >= 1, int32 and
+    strictly increasing; at least one mix, each with one multiplier in 0..2^32 - 1 per class (len(bounds) + 1)"""
+    try:
+        bounds, mults = mix
+        bounds = tuple(int(b) for b in bounds)
+        mults = [tuple(int(x) for x in m) for m in mults]
+    except (TypeError, ValueError):
+        raise ValueError("mix: expected (class bounds, [multipliers, ...]), sequences of ints") from None
+    if any(b < 1 or b >= 2 ** 31 for b in bounds) or any(b <= a for a, b in zip(bounds, bounds[1:])):
+        raise ValueError("mix: the class bounds must be >= 1, int32 and strictly increasing")
+    if not mults:
+        raise ValueError("mix: at least one mix")
+    for m in mults:
+        if len(m) != len(bounds) + 1:
+            raise ValueError(f"mix: every mix needs {len(bounds) + 1} multipliers (one per class), got {len(m)}")
+        if any(not 0 <= x <= 2 ** 32 - 1 for x in m):
+            raise ValueError("mix: every multiplier must be in 0..2^32 - 1")
+    return bounds, mults
+
+
+def parse_mix_spec(spec, nclasses):
+    """the multipliers of a --mix SPEC: nclasses non-negative integers joined by ':', each <= 2^32 - 1, or ValueError"""
+    parts = str(spec).split(":")
+    if not all(p.isascii() and p.isdigit() for p in parts):
+        raise ValueError(f"--mix: {spec!r} is not non-negative integers joined by ':'")
+    if len(parts) != nclasses:
+        raise ValueError(f"--mix: {spec!r} has {len(parts)} weights, the {nclasses} classes of --mix-classes need {nclasses}")
+    m = tuple(int(p) for p in parts)
+    if any(x > 2 ** 32 - 1 for x in m):
+        raise ValueError(f"--mix: {spec!r} has a weight above 2^32 - 1")
+    return m
+
+
+def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1, mix=None):
     if int(replicas) < 1:
         raise ValueError("bootstrap: replicas must be >= 1")
     if not len(loads) or not all(math.isfinite(float(L)) and float(L) > 0 for L in loads):
@@ -313,13 +347,15 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1):
         tracegen.check_block_len(block_len)
     except ValueError as e:
         raise ValueError(f"bootstrap: {e}") from None
+    if mix is not None:
+        check_mix(mix)
     aware = [fl.schedule for fl in flag_sets if _is_utilisation_aware(fl)]
     if aware:
         raise ValueError(f"bootstrap: the utilisation-aware engine ({', '.join(sorted(set(aware)))}) has no generated traces")
 
 
 def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1,
-                        compare=None):
+                        compare=None, mix=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -338,8 +374,17 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     survive resampling; the same replica index is coupled across values of L.
     compare=(pairs, bounds, edges): also compare replica (a, L, r) with (b, L, r) job by job on the device for every pair
     (a, b) of configuration indices (both on one trace file) and append (JPAIR_DTYPE records (len(pairs), len(loads),
-    replicas, C), CDF counts of d (len(pairs), len(loads), replicas, C, 3, E + 1)) as the last element."""
-    _check_bootstrap_args(flag_sets, replicas, loads, n, block_len)
+    replicas, C), CDF counts of d (len(pairs), len(loads), replicas, C, 3, E + 1)) as the last element.
+    mix=(bounds, [multipliers, ...]): draw the replicas from other job mixes (gs_boot_traces_mixed): under mix m, a base
+    trace row of size class c (the number of bounds <= its num_gpu) is drawn with weight multipliers[m][c] instead of
+    uniformly; gaps and arrivals are drawn as without a mix, and the same replica index is coupled across mixes.
+    Every returned array gains a mix axis right after the loads axis, (configurations, loads, mixes, replicas, ...),
+    and compare pairs (a, L, mix, r) with (b, L, mix, r).  A mix whose weights sum to 0 on a base trace is a
+    ValueError, raised before any engine is created.  A gittins replica still takes its index table from the base
+    trace: the policy is not told about the shift.  With L > 1, only block starts are drawn from the mix."""
+    _check_bootstrap_args(flag_sets, replicas, loads, n, block_len, mix)
+    if mix is not None:
+        mix_bounds, mix_mults = check_mix(mix)
     if compare is not None:
         pairs, cmp_bounds, cmp_edges = check_compare(compare, flag_sets)
     block_len = tracegen.check_block_len(block_len)
@@ -349,35 +394,55 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
         jd_bounds, jd_edges = check_jobdist(jobdist)
         nc, nb = len(jd_bounds) + 1, len(jd_edges) + 1
     R, loads = int(replicas), [float(L) for L in loads]
-    out = np.zeros((len(flag_sets), len(loads), R), dtype=capi.SUMMARY_DTYPE)
+    M = 1 if mix is None else len(mix_mults)
+    lead = (len(loads), R) if mix is None else (len(loads), M, R)   # the axes of one configuration's replicas
+    per = len(loads) * M * R
+    out = np.zeros((len(flag_sets),) + lead, dtype=capi.SUMMARY_DTYPE)
     if timeline is not None:
-        bins = np.zeros((len(flag_sets), len(loads), R, B), dtype=capi.TBIN_DTYPE)
+        bins = np.zeros((len(flag_sets),) + lead + (B,), dtype=capi.TBIN_DTYPE)
     if jobdist is not None:
-        jd_cls = np.zeros((len(flag_sets), len(loads), R, nc), dtype=capi.JCLASS_DTYPE)
-        jd_hist = np.zeros((len(flag_sets), len(loads), R, nc, 3, nb), dtype=np.uint32)
+        jd_cls = np.zeros((len(flag_sets),) + lead + (nc,), dtype=capi.JCLASS_DTYPE)
+        jd_hist = np.zeros((len(flag_sets),) + lead + (nc, 3, nb), dtype=np.uint32)
     if compare is not None:
         cmp_nc, cmp_nb = len(cmp_bounds) + 1, len(cmp_edges) + 1
-        cmp_recs = np.zeros((len(pairs), len(loads), R, cmp_nc), dtype=capi.JPAIR_DTYPE)
-        cmp_hist = np.zeros((len(pairs), len(loads), R, cmp_nc, 3, cmp_nb), dtype=np.uint32)
+        cmp_recs = np.zeros((len(pairs),) + lead + (cmp_nc,), dtype=capi.JPAIR_DTYPE)
+        cmp_hist = np.zeros((len(pairs),) + lead + (cmp_nc, 3, cmp_nb), dtype=np.uint32)
     by_trace = {}
     for c, fl in enumerate(flag_sets):
         by_trace.setdefault(fl.trace_file, []).append(c)
+    groups = []                                           # every trace is read and every mix checked before any engine
     for configs in by_trace.values():
         sims = _plain_setup([flag_sets[c] for c in configs])
         base = sims[0][2].table
+        weights = None
+        if mix is not None:
+            weights = np.stack([tracegen.class_weights(base.gpus, mix_bounds, m) for m in mix_mults])
+            for m, w in enumerate(weights):
+                if not w.any():
+                    raise ValueError(f"bootstrap: mix {':'.join(map(str, mix_mults[m]))} gives every job of "
+                                     f"{flag_sets[configs[0]].trace_file} weight 0")
+        groups.append((configs, sims, base, weights))
+    for configs, sims, base, weights in groups:
         jobs = base.n if n is None else int(n)
-        params = np.zeros(len(configs) * len(loads) * R, dtype=capi.BOOT_PARAMS_DTYPE)
+        params = np.zeros(len(configs) * per, dtype=capi.BOOT_PARAMS_DTYPE)
+        mix_of = np.zeros(len(params), dtype=np.int32)    # replica (config k, load l, mix m, r) is k * per + (l * M + m) * R + r
         with capi.Engine(device=device, nsims=len(params)) as eng:
             i = 0
             for fl, infra, jm, pol in sims:
                 for L in loads:
                     num, den = load_gap_scale(L)
-                    for r in range(R):
-                        eng.config(i, infra.gs_cluster(), pol)
-                        params[i] = (seed, r, jobs, num, den)
-                        i += 1
+                    for m in range(M):
+                        for r in range(R):
+                            eng.config(i, infra.gs_cluster(), pol)
+                            params[i] = (seed, r, jobs, num, den)
+                            mix_of[i] = m
+                            i += 1
             eng.boot_population(base)
-            eng.boot_traces(params, block_len=None if block_len == 1 else block_len)
+            if weights is None:
+                eng.boot_traces(params, block_len=None if block_len == 1 else block_len)
+            else:
+                eng.boot_mixes(weights)
+                eng.boot_traces(params, block_len=None if block_len == 1 else block_len, mix=mix_of)
             if timeline is not None:
                 eng.set_timeline(W, B)
             if jobdist is not None:
@@ -388,20 +453,20 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
             sel = [k for k, (a, _) in enumerate(pairs) if a in set(configs)] if compare is not None else []
             if sel:
                 pos = {c: k for k, c in enumerate(configs)}
-                span = np.arange(len(loads) * R)                  # replica (config k, load l, r) is k * len(loads) * R + l * R + r
-                ia = np.concatenate([pos[pairs[k][0]] * len(loads) * R + span for k in sel])
-                ib = np.concatenate([pos[pairs[k][1]] * len(loads) * R + span for k in sel])
+                span = np.arange(per)                             # replica (config k, load l[, mix m], r) is k * per + ...
+                ia = np.concatenate([pos[pairs[k][0]] * per + span for k in sel])
+                ib = np.concatenate([pos[pairs[k][1]] * per + span for k in sel])
                 cr, ch = eng.compare(ia, ib, cmp_bounds, cmp_edges)
-                cmp_recs[sel] = cr.reshape(len(sel), len(loads), R, cmp_nc)
-                cmp_hist[sel] = ch.reshape(len(sel), len(loads), R, cmp_nc, 3, cmp_nb)
+                cmp_recs[sel] = cr.reshape((len(sel),) + lead + (cmp_nc,))
+                cmp_hist[sel] = ch.reshape((len(sel),) + lead + (cmp_nc, 3, cmp_nb))
         for k, c in enumerate(configs):
-            part = slice(k * len(loads) * R, (k + 1) * len(loads) * R)
-            out[c] = recs[part].reshape(len(loads), R)
+            part = slice(k * per, (k + 1) * per)
+            out[c] = recs[part].reshape(lead)
             if tl is not None:
-                bins[c] = tl[part].reshape(len(loads), R, B)
+                bins[c] = tl[part].reshape(lead + (B,))
             if jd is not None:
-                jd_cls[c] = jd[0][part].reshape(len(loads), R, nc)
-                jd_hist[c] = jd[1][part].reshape(len(loads), R, nc, 3, nb)
+                jd_cls[c] = jd[0][part].reshape(lead + (nc,))
+                jd_hist[c] = jd[1][part].reshape(lead + (nc, 3, nb))
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
            + (((cmp_recs, cmp_hist),) if compare is not None else ()))
     return res[0] if len(res) == 1 else res
@@ -416,33 +481,46 @@ def _block_val(block_len):
     return [] if block_len is None else [block_len]
 
 
-def write_bootstrap_csv(path, flag_sets, loads, records, block_len=None):
-    """one line per (configuration, load, replica): replica, load, block_len (with a block length), the
-    configuration's flags, the summary columns"""
+def _mix_col(mix):
+    """the mix column of the bootstrap files: none without job mixes (mix None)"""
+    return [] if mix is None else ["mix"]
+
+
+def _load_lines(loads, block_len, mix, per_load):
+    """[(values of the load, block_len and mix columns, arrays)] of one configuration's (load[, mix]) lines in line
+    order: per_load holds one entry per load, and with mixes (their SPEC texts) one per (load, mix)"""
+    if mix is None:
+        return [([L] + _block_val(block_len), x) for L, x in zip(loads, per_load)]
+    return [([L] + _block_val(block_len) + [m], x) for L, per_mix in zip(loads, per_load) for m, x in zip(mix, per_mix)]
+
+
+def write_bootstrap_csv(path, flag_sets, loads, records, block_len=None, mix=None):
+    """one line per (configuration, load[, mix], replica): replica, load, block_len (with a block length), mix (with
+    job mixes: their SPEC texts), the configuration's flags, the summary columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(["replica", "load"] + _block_col(block_len) + SUMMARY_KEYS + summary.columns())
+        w.writerow(["replica", "load"] + _block_col(block_len) + _mix_col(mix) + SUMMARY_KEYS + summary.columns())
         for fl, per_load in zip(flag_sets, records):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
-            for L, recs in zip(loads, per_load):
+            for keys, recs in _load_lines(loads, block_len, mix, per_load):
                 for r, rec in enumerate(recs):
-                    w.writerow([r, L] + _block_val(block_len) + [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + summary.flat(rec, *shape))
+                    w.writerow([r] + keys + [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + summary.flat(rec, *shape))
 
 
-def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95, block_len=None):
-    """one line per (configuration, load): the flags, the load, block_len (with a block length), the replica count
-    and summary.spread's columns"""
+def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95, block_len=None, mix=None):
+    """one line per (configuration, load[, mix]): the flags, the load, block_len (with a block length), mix (with job
+    mixes), the replica count and summary.spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["replicas", "level"] + summary.spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["replicas", "level"] + summary.spread_columns())
         for fl, per_load in zip(flag_sets, records):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
-            for L, recs in zip(loads, per_load):
-                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L] + _block_val(block_len) + [len(recs), level]
+            for keys, recs in _load_lines(loads, block_len, mix, per_load):
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [len(recs), level]
                            + summary.spread_flat(summary.spread(recs, *shape, level=level)))
 
 
@@ -468,20 +546,20 @@ def write_timeline_csv(path, flag_sets, bins, width):
                            + _bin_bounds(b, width, len(tb)) + summary.timeline_flat(d, b))
 
 
-def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95, block_len=None):
-    """one line per (configuration, load, bin): the flags, the load, block_len (with a block length), the bin, its
-    tick range, the number of replicas with rows in it and summary.timeline_spread's columns"""
+def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95, block_len=None, mix=None):
+    """one line per (configuration, load[, mix], bin): the flags, the load, block_len (with a block length), mix (with
+    job mixes), the bin, its tick range, the number of replicas with rows in it and summary.timeline_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["bin", "bin_start", "bin_end", "replicas", "level"] + summary.timeline_spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["bin", "bin_start", "bin_end", "replicas", "level"] + summary.timeline_spread_columns())
         for fl, per_load in zip(flag_sets, bins):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
-            for L, tb in zip(loads, per_load):
+            for keys, tb in _load_lines(loads, block_len, mix, per_load):
                 sp = summary.timeline_spread(tb, *shape, level=level)
                 for b in range(tb.shape[1]):
-                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L] + _block_val(block_len) + [b]
+                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [b]
                                + _bin_bounds(b, width, tb.shape[1]) + [int(sp["replicas"][b]), level] + summary.timeline_spread_flat(sp, b))
 
 
@@ -503,18 +581,20 @@ def write_jobdist_csv(path, flag_sets, classes, hist, bounds, edges):
                            + summary.jobdist_flat(d, c))
 
 
-def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None):
-    """one line per (configuration, load, class): the flags, the load, block_len (with a block length), the class, its
-    num_gpu range, the number of replicas with jobs in it and summary.jobdist_spread's columns"""
+def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None, mix=None):
+    """one line per (configuration, load[, mix], class): the flags, the load, block_len (with a block length), mix
+    (with job mixes), the class, its num_gpu range, the number of replicas with jobs in it and
+    summary.jobdist_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["class", "gpus_min", "gpus_max", "replicas", "level"] + summary.jobdist_spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["class", "gpus_min", "gpus_max", "replicas", "level"]
+                   + summary.jobdist_spread_columns())
         for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
-            for L, cl, hs in zip(loads, per_cl, per_hs):
+            for (keys, cl), (_, hs) in zip(_load_lines(loads, block_len, mix, per_cl), _load_lines(loads, block_len, mix, per_hs)):
                 sp = summary.jobdist_spread(cl, hs, edges, level=level)
                 for c in range(cl.shape[1]):
-                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L] + _block_val(block_len) + [c]
+                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [c]
                                + _class_range(c, bounds) + [int(sp["replicas"][c]), level] + summary.jobdist_spread_flat(sp, c))
 
 
@@ -534,23 +614,23 @@ def write_jobdist_cdf_csv(path, flag_sets, classes, hist, bounds, edges):
                                    + [m, edge, int(d["jobs"][c]), float(d[m + "_cdf"][c, e])])
 
 
-def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None):
-    """one line per (configuration, load, class, quantity, edge): the flags, the load, block_len (with a block
-    length), the class, its num_gpu range, the quantity, the edge, the number of replicas with jobs in the class and
+def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None, mix=None):
+    """one line per (configuration, load[, mix], class, quantity, edge): the flags, the load, block_len (with a block
+    length), mix (with job mixes), the class, its num_gpu range, the quantity, the edge, the number of replicas with jobs in the class and
     the spread of the CDF value"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + ["class", "gpus_min", "gpus_max", "quantity", "edge", "replicas", "level"]
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["class", "gpus_min", "gpus_max", "quantity", "edge", "replicas", "level"]
                    + [f"cdf_{s}" for s in summary.SPREAD_STATS])
         for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
-            for L, cl, hs in zip(loads, per_cl, per_hs):
+            for (keys, cl), (_, hs) in zip(_load_lines(loads, block_len, mix, per_cl), _load_lines(loads, block_len, mix, per_hs)):
                 sp = summary.jobdist_spread(cl, hs, edges, level=level)
                 for c in range(cl.shape[1]):
                     for m in summary.JOBDIST_QUANTITIES:
                         for e, edge in enumerate(edges):
-                            w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, L]
-                                       + _block_val(block_len) + [c] + _class_range(c, bounds) + [m, edge, int(sp["replicas"][c]), level]
+                            w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed]
+                                       + keys + [c] + _class_range(c, bounds) + [m, edge, int(sp["replicas"][c]), level]
                                        + [float(sp[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS])
 
 
@@ -572,50 +652,53 @@ def write_paired_csv(path, flag_sets, pairs, recs, hist, bounds, edges):
                     w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + [c] + _class_range(c, bounds) + [m] + summary.pair_flat(d, c, m))
 
 
-def write_paired_ci_csv(path, flag_sets, pairs, loads, recs, hist, bounds, edges, level=0.95, block_len=None):
-    """one line per (configuration b of a pair, load, class, quantity): b's flags, the base schedule, the load,
-    block_len (with a block length), the class, its num_gpu range, the quantity, the replicas with jobs finished in
+def write_paired_ci_csv(path, flag_sets, pairs, loads, recs, hist, bounds, edges, level=0.95, block_len=None, mix=None):
+    """one line per (configuration b of a pair, load[, mix], class, quantity): b's flags, the base schedule, the load,
+    block_len (with a block length), mix (with job mixes), the class, its num_gpu range, the quantity, the replicas with jobs finished in
     both runs in the class and summary.pair_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["base_schedule", "load"] + _block_col(block_len) + ["class", "gpus_min", "gpus_max", "quantity", "replicas", "level"]
+        w.writerow(SUMMARY_KEYS + ["base_schedule", "load"] + _block_col(block_len) + _mix_col(mix) + ["class", "gpus_min", "gpus_max", "quantity", "replicas", "level"]
                    + summary.pair_spread_columns())
         for (a, b), per_rc, per_hs in zip(pairs, recs, hist):
-            for L, rc, hs in zip(loads, per_rc, per_hs):
+            for (keys, rc), (_, hs) in zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)):
                 sp = summary.pair_spread(rc, hs, edges, level=level)
                 for c in range(rc.shape[1]):
                     for m in summary.JOBDIST_QUANTITIES:
-                        w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + [L] + _block_val(block_len) + [c] + _class_range(c, bounds)
+                        w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + keys + [c] + _class_range(c, bounds)
                                    + [m, int(sp["replicas"][c]), level] + summary.pair_spread_flat(sp, c, m))
 
 
-def write_paired_cdf_csv(path, flag_sets, pairs, recs, hist, bounds, edges, loads=None, level=0.95, block_len=None):
-    """one line per (configuration b of a pair[, load], class, quantity, edge): b's flags, the base schedule[, the load,
-    block_len], the class, its num_gpu range, the quantity, the edge and the fraction of the jobs finished in both
+def write_paired_cdf_csv(path, flag_sets, pairs, recs, hist, bounds, edges, loads=None, level=0.95, block_len=None, mix=None):
+    """one line per (configuration b of a pair[, load[, mix]], class, quantity, edge): b's flags, the base schedule[, the
+    load, block_len, mix], the class, its num_gpu range, the quantity, the edge and the fraction of the jobs finished in both
     runs with d <= edge (with loads: the replicas with such jobs and the spread of that fraction)"""
     import csv
     boot = loads is not None
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) if boot else []) + ["class", "gpus_min", "gpus_max", "quantity", "edge"]
+        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["class", "gpus_min", "gpus_max", "quantity", "edge"]
                    + (["replicas", "level"] + [f"cdf_{s}" for s in summary.SPREAD_STATS] if boot else ["jobs", "cdf"]))
         for (a, b), per_rc, per_hs in zip(pairs, recs, hist):
             keys = _pair_keys(flag_sets[b], flag_sets[a])
-            for L, rc, hs in (zip(loads, per_rc, per_hs) if boot else [(None, per_rc, per_hs)]):
+            lines = (zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)) if boot
+                     else [(([], per_rc), ([], per_hs))])
+            for (lk, rc), (_, hs) in lines:
                 d = summary.pair_spread(rc, hs, edges, level=level) if boot else summary.pair_derived(rc, hs, edges)
                 for c in range(rc.shape[-1]):
                     for m in summary.JOBDIST_QUANTITIES:
                         for e, edge in enumerate(edges):
                             tail = ([int(d["replicas"][c]), level] + [float(d[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS] if boot
                                     else [int(d["jobs"][c]), float(d[m + "_cdf"][c, e])])
-                            w.writerow(keys + ([L] + _block_val(block_len) if boot else []) + [c] + _class_range(c, bounds) + [m, edge] + tail)
+                            w.writerow(keys + lk + [c] + _class_range(c, bounds) + [m, edge] + tail)
 
 
-def write_paired_summary_csv(path, flag_sets, pairs, records, loads=None, level=0.95, block_len=None):
-    """one line per (configuration b of a pair[, load]): b's flags, the base schedule[, the load, block_len], the
-    replicas and summary.paired_spread's columns: the replica-level differences b - base of the makespan and of every
-    derived number (records: (configurations, loads, replicas) with loads, else one record per configuration)"""
+def write_paired_summary_csv(path, flag_sets, pairs, records, loads=None, level=0.95, block_len=None, mix=None):
+    """one line per (configuration b of a pair[, load[, mix]]): b's flags, the base schedule[, the load, block_len, mix],
+    the replicas and summary.paired_spread's columns: the replica-level differences b - base of the makespan and of
+    every derived number (records: (configurations, loads[, mixes], replicas) with loads, else one record per
+    configuration)"""
     import csv
     boot = loads is not None
 
@@ -624,13 +707,15 @@ def write_paired_summary_csv(path, flag_sets, pairs, records, loads=None, level=
         return cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) if boot else []) + ["replicas", "level"] + summary.paired_columns())
+        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["replicas", "level"]
+                   + summary.paired_columns())
         for a, b in pairs:
             sa, sb = shape(flag_sets[a]), shape(flag_sets[b])
-            per = zip(loads, records[a], records[b]) if boot else [(None, records[a:a + 1], records[b:b + 1])]
-            for L, ra, rb in per:
+            per = (zip(_load_lines(loads, block_len, mix, records[a]), _load_lines(loads, block_len, mix, records[b])) if boot
+                   else [(([], records[a:a + 1]), ([], records[b:b + 1]))])
+            for (lk, ra), (_, rb) in per:
                 sp = summary.paired_spread(ra, rb, sa, sb, level=level)
-                w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + ([L] + _block_val(block_len) if boot else []) + [len(ra), level]
+                w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + lk + [len(ra), level]
                            + summary.paired_flat(sp))
 
 
@@ -668,6 +753,13 @@ def main(argv=None):
     ap.add_argument("--block-len", type=int, default=None, metavar="L",
                     help="with --bootstrap: draw block bootstrap replicas with mean block length L (1..2^32 - 1), which keep runs "
                          "of consecutive jobs and their gaps together; every output file gets a block_len column after load")
+    ap.add_argument("--mix", nargs="+", default=None, metavar="SPEC",
+                    help="with --bootstrap and --mix-classes: draw the replicas from each job mix SPEC, k + 1 non-negative integer "
+                         "weights joined by ':' (one per class of --mix-classes, each <= 2^32 - 1): a job of class c is drawn "
+                         "with weight SPEC[c] instead of uniformly; every output file gets a mix column after load (after "
+                         "block_len with --block-len)")
+    ap.add_argument("--mix-classes", type=int, nargs="+", default=None, metavar="B",
+                    help="with --mix: class bounds B1 < ... < Bk of the mixes (a job's class is the number of bounds <= its num_gpu)")
     ap.add_argument("--summary-ci", default=None, metavar="FILE",
                     help="with --bootstrap: one CSV line per (configuration, load) with the mean, std and 95%% interval across replicas")
     ap.add_argument("--timeline", default=None, metavar="FILE",
@@ -736,6 +828,17 @@ def main(argv=None):
         ap.error("--bin-width and --bins need --timeline FILE")
     if a.bootstrap is None and (a.load is not None or a.jobs is not None or a.summary_ci is not None or a.block_len is not None):
         ap.error("--load, --jobs, --block-len and --summary-ci need --bootstrap")
+    mix = mix_text = None
+    if a.mix is not None or a.mix_classes is not None:
+        if a.bootstrap is None:
+            ap.error("--mix and --mix-classes need --bootstrap")
+        if a.mix is None or a.mix_classes is None:
+            ap.error("--mix and --mix-classes go together")
+        try:
+            mix = check_mix((a.mix_classes, [parse_mix_spec(m, len(a.mix_classes) + 1) for m in a.mix]))
+        except ValueError as e:
+            ap.error(str(e))
+        mix_text = list(a.mix)
     if a.bootstrap is not None:
         if not a.summary:
             ap.error("--bootstrap needs --summary FILE")
@@ -769,34 +872,35 @@ def main(argv=None):
     if a.bootstrap is not None:
         loads = a.load or [1.0]
         try:
-            _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs, 1 if a.block_len is None else a.block_len)
+            _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs, 1 if a.block_len is None else a.block_len, mix)
         except ValueError as e:
             ap.error(str(e))
         bl = a.block_len
         res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist,
-                                  block_len=1 if bl is None else bl, compare=compare)
+                                  block_len=1 if bl is None else bl, compare=compare, mix=mix)
         recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None else (res[0], res[1:])
         if compare is not None:
             pairs, cmp_bounds, cmp_edges = compare
             prec, phist = rest[-1]
             rest = rest[:-1]
             if a.paired:
-                write_paired_ci_csv(a.paired, sets, pairs, loads, prec, phist, cmp_bounds, cmp_edges, block_len=bl)
+                write_paired_ci_csv(a.paired, sets, pairs, loads, prec, phist, cmp_bounds, cmp_edges, block_len=bl, mix=mix_text)
             if a.paired_cdf:
-                write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges, loads=loads, block_len=bl)
+                write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges, loads=loads, block_len=bl, mix=mix_text)
             if a.paired_summary:
-                write_paired_summary_csv(a.paired_summary, sets, pairs, recs, loads=loads, block_len=bl)
+                write_paired_summary_csv(a.paired_summary, sets, pairs, recs, loads=loads, block_len=bl, mix=mix_text)
         if timeline is not None:
-            write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0], block_len=bl)
+            write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0], block_len=bl, mix=mix_text)
         if jobdist is not None:
             cls, hist = rest[-1]
-            write_jobdist_ci_csv(a.jobdist, sets, loads, cls, hist, *jobdist, block_len=bl)
+            write_jobdist_ci_csv(a.jobdist, sets, loads, cls, hist, *jobdist, block_len=bl, mix=mix_text)
             if a.jobdist_cdf:
-                write_jobdist_cdf_ci_csv(a.jobdist_cdf, sets, loads, cls, hist, *jobdist, block_len=bl)
-        write_bootstrap_csv(a.summary, sets, loads, recs, block_len=bl)
+                write_jobdist_cdf_ci_csv(a.jobdist_cdf, sets, loads, cls, hist, *jobdist, block_len=bl, mix=mix_text)
+        write_bootstrap_csv(a.summary, sets, loads, recs, block_len=bl, mix=mix_text)
         if a.summary_ci:
-            write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs, block_len=bl)
-        print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads x {a.bootstrap} replicas")
+            write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs, block_len=bl, mix=mix_text)
+        print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads"
+              + (f" x {len(mix_text)} mixes" if mix_text else "") + f" x {a.bootstrap} replicas")
         return
     if a.summary:
         res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare)

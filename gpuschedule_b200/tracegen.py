@@ -22,6 +22,7 @@ Distributions follow SURVEY.md section 8(d):
 """
 from __future__ import annotations
 
+import collections
 import operator
 
 import numpy as np
@@ -125,18 +126,77 @@ def check_block_len(block_len):
     return L
 
 
-def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_len=1):
+def alias_table(weights):
+    """The exact integer alias table (Walker / Vose) of per-row weights w (uint32, at least one non-zero), as
+    gs_boot_mixes builds it on the host (include/gsched.h): with T = sum w_i and q_i = w_i * K, FIFO worklists
+    S = {i : q_i < T} and G = {i : q_i >= T} in ascending row order; while both are non-empty, the front s of S gets
+    U_s = q_s, A_s = g (the front of G), q_g -= T - q_s, and g moves to the back of S once q_g < T; every row left in G
+    gets U_i = T, A_i = i.  A job with unweighted row c and u = floor(w3 * T / 2^64) takes row c if u < U_c, else A_c.
+    Returns (U, A) as uint64 / int64 arrays of K entries."""
+    w = check_weights(weights)
+    K, T = len(w), sum(w)
+    q = [x * K for x in w]
+    U, A = [0] * K, [0] * K
+    S = collections.deque(i for i in range(K) if q[i] < T)
+    G = collections.deque(i for i in range(K) if q[i] >= T)
+    while S and G:
+        s, g = S.popleft(), G[0]
+        U[s], A[s] = q[s], g
+        q[g] -= T - q[s]
+        if q[g] < T:
+            S.append(G.popleft())
+    for i in G:
+        U[i], A[i] = T, i
+    return np.array(U, dtype=np.uint64), np.array(A, dtype=np.int64)
+
+
+def check_weights(weights, k=None):
+    """per-row weights as a list of Python ints in 0..2^32 - 1 with a non-zero sum (and k entries), or ValueError"""
+    w = np.asarray(weights)
+    if w.ndim != 1 or not len(w) or (w.dtype.kind not in "iu" and not (w.dtype == object and all(isinstance(x, int) for x in w.tolist()))):
+        raise ValueError("weights: expected a non-empty 1-d sequence of integers")
+    w = [int(x) for x in w.tolist()]
+    if any(not 0 <= x <= 2 ** 32 - 1 for x in w):
+        raise ValueError("weights: every weight must be in 0..2^32 - 1")
+    if k is not None and len(w) != k:
+        raise ValueError(f"weights: expected one weight per population row ({k}), got {len(w)}")
+    if sum(w) < 1:
+        raise ValueError("weights: the weights sum to 0")
+    return w
+
+
+def class_weights(gpus, bounds, multipliers):
+    """per-row weights of a job mix given by size class: row i gets multipliers[c], where c, its class, is the number of
+    `bounds` <= gpus[i] (the rule of gs_set_jobdist).  Returns uint32 weights, one per row."""
+    b = [int(x) for x in bounds]
+    if any(x <= y for y, x in zip(b, b[1:])):
+        raise ValueError("class_weights: the class bounds must be strictly increasing")
+    m = [int(x) for x in multipliers]
+    if len(m) != len(b) + 1:
+        raise ValueError(f"class_weights: expected {len(b) + 1} multipliers (one per class), got {len(m)}")
+    if any(not 0 <= x <= 2 ** 32 - 1 for x in m):
+        raise ValueError("class_weights: every multiplier must be in 0..2^32 - 1")
+    cls = np.searchsorted(np.asarray(b, dtype=np.int64), np.asarray(gpus, dtype=np.int64), side="right")
+    return np.asarray(m, dtype=np.uint32)[cls]
+
+
+def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_len=1, weights=None):
     """Replica (seed, stream) of `n` jobs drawn from `population` (JOBIN_DTYPE records of one trace in admission order):
     job j resamples a row and an inter-arrival gap of the population with the Philox4x64-10 block at counter
     (j + 1, 0, 0, 0), and its arrival is floor(gap sum * gap_num / gap_den) (include/gsched.h, gs_boot_traces).
     block_len=L > 1 resamples blocks of consecutive rows of mean length L instead, each row with the gap that preceded
-    it in the population (gs_boot_traces_blocked); L = 1 is the iid bootstrap.  Returns (JOBIN_DTYPE records, source rows)."""
+    it in the population (gs_boot_traces_blocked); L = 1 is the iid bootstrap.  weights (one uint32 per population
+    row) draws row i with probability w_i / sum(w) through alias_table, at block starts only when blocked
+    (gs_boot_traces_mixed); None is the unweighted bootstrap.  Returns (JOBIN_DTYPE records, source rows)."""
     from .capi import JOBIN_DTYPE
     pop = np.ascontiguousarray(population, dtype=JOBIN_DTYPE)
     k, n, gap_num, gap_den = len(pop), int(n), int(gap_num), int(gap_den)
     if k < 1 or not 0 <= n < 2 ** 31 - 64 or gap_num < 0 or gap_den < 1:
         raise ValueError("bootstrap_packed: needs a population of at least one record, 0 <= n < 2^31 - 64, gap_num >= 0, gap_den >= 1")
     L = check_block_len(block_len)
+    if weights is not None:
+        weights = check_weights(weights, k)
+        U, A = alias_table(weights)
     gaps = np.diff(pop["arrive_tick"].astype(np.int64))
     max_gap = int(gaps.max()) if len(gaps) else 0
     if n > 1 and (n - 1) * max_gap * gap_num // gap_den >= 2 ** 31 - 1:
@@ -145,6 +205,9 @@ def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_le
     ctr[:, 0] = np.arange(1, n + 1, dtype=np.uint64)
     w = philox4x64(seed, stream, ctr)
     rows = mulhi64(w[:, 0], np.uint64(k)).astype(np.int64)
+    if weights is not None:                                        # the alias pick: keep column c iff u < U_c
+        u = mulhi64(w[:, 3], np.uint64(sum(weights)))
+        rows = np.where(u < U[rows], rows, A[rows])
     j = np.arange(n, dtype=np.int64)
     start = mulhi64(w[:, 2], np.uint64(L)) == 0                   # block starts; always for L = 1
     start[:1] = True
@@ -162,12 +225,12 @@ def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_le
     return out, rows
 
 
-def bootstrap_table(base_table, seed, stream, n, gap_num=1, gap_den=1, block_len=1):
+def bootstrap_table(base_table, seed, stream, n, gap_num=1, gap_den=1, block_len=1, weights=None):
     """bootstrap_packed of a JobTable as a JobTable of its own (labels 0..n-1, the source rows' num_gpu_text and
     utilisation columns, submit = arrive), so that a generated replica can go through the ordinary upload path and
     the ordinary log writers."""
     from .ingest import JobTable
-    recs, rows = bootstrap_packed(base_table.packed(), seed, stream, n, gap_num, gap_den, block_len)
+    recs, rows = bootstrap_packed(base_table.packed(), seed, stream, n, gap_num, gap_den, block_len, weights)
     pick = lambda a: None if a is None else np.ascontiguousarray(np.asarray(a)[rows])
     t = JobTable(
         n=len(recs), label=[str(i) for i in range(len(recs))],

@@ -498,8 +498,8 @@ int gs_compare(gs_handle h, int32_t npairs, const int32_t *a, const int32_t *b, 
  *   {floor(S_j * gap_num / gap_den), P[r].gpus, P[r].gpu_per_task, 0, P[r].mem_bytes, P[r].duration}
  * with r = floor(w0 * k / 2^64), S_j = g_0 + ... + g_j, g_0 = 0, g_j = D[floor(w1 * (k - 1) / 2^64)] (0 when k = 1).
  * gap_num / gap_den = 1 / 1 keeps the base trace's arrival rate in expectation, 1 / 2 doubles the offered load; the same
- * (seed, stream) draws the same rows and gaps at every load (common random numbers).  w3 is unused, and w2 is used
- * only by gs_boot_traces_blocked, which draws replica sim as a stationary block bootstrap with mean block length
+ * (seed, stream) draws the same rows and gaps at every load (common random numbers).  w3 is used only by gs_boot_traces_mixed (below),
+ * and w2 only by gs_boot_traces_blocked, which draws replica sim as a stationary block bootstrap with mean block length
  * L = block_len[sim] (block_len NULL: L = 1 for all, exactly gs_boot_traces): job 0 starts a block, job j > 0 starts one
  * iff floor(w2 * L / 2^64) == 0; with b the last block start <= j and s_b = floor(w0_b * k / 2^64), job j copies row
  * r = (s_b + j - b) mod k, and its gap is D[r - 1] when j continues a block with r > 0, the iid gap above otherwise.
@@ -522,6 +522,29 @@ int gs_boot_traces(gs_handle h, const gs_boot_params *params /* nsims */, double
 int gs_boot_traces_blocked(gs_handle h, const gs_boot_params *params /* nsims */, const uint32_t *block_len /* nsims; NULL = all 1 */,
                            double *kernel_ms);
 int gs_fetch_trace(gs_handle h, int sim, gs_jobin *out /* n records */);
+
+/* ---- mixed bootstrap replicas: another job mix drawn from the same population ----------------------------
+ * gs_boot_mixes gives the handle nmix mixes of the current population (weights: nmix * k uint32, mix-major): mix m
+ * draws row i with probability w_i / T, T = sum over i of w_i >= 1.  Each mix becomes an exact integer alias table
+ * (Walker / Vose) on the host: with q_i = w_i * k (below 2^63, as is T), take FIFO worklists S = {i : q_i < T} and
+ * G = {i : q_i >= T} in ascending row order; while both are non-empty, take s from the front of S, let g be the front
+ * of G, set U_s = q_s, A_s = g and q_g -= T - q_s, and move g from the front of G to the back of S once q_g < T; every
+ * row still in G gets U_i = T, A_i = i.  The tables are uploaded as one device array; nmix = 0 clears them, and so does
+ * a new gs_boot_population.
+ * gs_boot_traces_mixed is gs_boot_traces_blocked where replica sim with mix[sim] = m >= 0 picks its rows through mix m:
+ * with c = floor(w0 * k / 2^64) and u = floor(w3 * T / 2^64), the row is c if u < U_c, else A_c (row m' has
+ * probability w_m' / T to within 2^-64 per column).  A blocked replica (L > 1) picks s_b this way at block starts only;
+ * a block still continues through the base trace in order, so it can copy rows of weight 0, and the shares of the
+ * rows equal the mix only at L = 1.  Gaps, arrivals, the arrival bound and every other field are those of
+ * gs_boot_traces_blocked, and the same (seed, stream) stays coupled across mixes, loads and block lengths.  Equal
+ * weights give U_i = T for every row: the unweighted replica byte for byte.  mix[sim] = -1 (mix NULL: all -1) is the
+ * unweighted replica, and a call without any mix >= 0 is gs_boot_traces_blocked exactly (the same launches).
+ * Errors (nothing changes): gs_boot_mixes: GS_ERR_ARG for nmix < 0, NULL weights with nmix > 0 or a mix with T = 0,
+ * GS_ERR_STATE without a population, GS_ERR_CUDA if the tables cannot be allocated; gs_boot_traces_mixed: the errors of
+ * gs_boot_traces_blocked, checked in the same order, then GS_ERR_ARG for mix[sim] outside [-1, nmix).          */
+int gs_boot_mixes(gs_handle h, int32_t nmix, const uint32_t *weights /* nmix * k, mix-major */);
+int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params /* nsims */, const uint32_t *block_len /* NULL = all 1 */,
+                         const int32_t *mix /* nsims, -1 = unweighted; NULL = all -1 */, double *kernel_ms);
 
 /* Stateless candidate scoring: evaluate b jobs against ONE cluster state.
  * first_node[i] = node of a single-node first fit, or the first node of a
