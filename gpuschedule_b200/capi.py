@@ -95,6 +95,25 @@ JCLASS_DTYPE = np.dtype([("jobs", "<i8"), ("wait_sum", "<i8"), ("turnaround_sum"
 assert JCLASS_DTYPE.itemsize == 160
 JOBDIST_MAX_CLASSES = 8
 JOBDIST_MAX_EDGES = 255
+# gs_sdclass (include/gsched.h): one class of a replica's finished jobs under a chosen key (GS_JKEY_*) -- its gs_jclass,
+# then the bounded slowdown sd (units of 1/1024): exact sum, 128-bit sum of squares, order statistics, minimum, the
+# jobs saturated at 2^31 - 1, and the exact 128-bit sum of the keys.  CDF counts come separately as uint32
+# (replica, class, 3 * (E + 1) + Esd + 1): the wait, turnaround and jct rows, then the sd row.
+SDCLASS_DTYPE = np.dtype([("jc", JCLASS_DTYPE), ("sd_sum", "<i8"), ("sd_sq_lo", "<u8"), ("sd_sq_hi", "<u8"), ("sd_q", "<i4", (5,)),
+                          ("sd_min", "<i4"), ("sd_clamped", "<i8"), ("key_sum_lo", "<u8"), ("key_sum_hi", "<u8")])
+assert SDCLASS_DTYPE.itemsize == 232
+JKEYS = {"gpus": 0, "length": 1, "gpu-time": 2}           # GS_JKEY_GPUS, GS_JKEY_LENGTH, GS_JKEY_GPU_TIME
+SLOWDOWN_MAX_EDGES = 255
+SLOWDOWN_ONE = 1024                                       # sd units per unit of slowdown
+SLOWDOWN_MAX = 2 ** 31 - 1                                # the saturated sd
+
+
+class GsSlowdownCfg(C.Structure):
+    _fields_ = [("key", C.c_int32), ("nclasses", C.c_int32), ("bounds", C.c_int64 * (JOBDIST_MAX_CLASSES - 1)), ("tau", C.c_int64),
+                ("nedges", C.c_int32), ("nsd_edges", C.c_int32), ("edges", C.c_void_p), ("sd_edges", C.c_void_p)]
+
+
+assert C.sizeof(GsSlowdownCfg) == 96
 # gs_jpair (include/gsched.h): one job-size class of a pair of replicas on the same trace -- per quantity (wait,
 # turnaround, jct) the per-job differences d = x_b - x_a over the jobs finished in both runs: counts by sign, exact
 # sums, 128-bit sums of squares, and the nearest-rank points of d ascending (q_hi) and descending (q_lo)
@@ -211,6 +230,9 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_compare.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
                                      C.c_void_p, C.c_void_p, f64p]
     lib.gs_horus_compare.restype = C.c_int
+    lib.gs_horus_set_slowdown.argtypes = [C.c_void_p, C.c_void_p]
+    lib.gs_horus_fetch_slowdown.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.gs_horus_set_slowdown.restype = lib.gs_horus_fetch_slowdown.restype = C.c_int
     for name in ("gs_horus_summarize", "gs_horus_set_timeline", "gs_horus_fetch_timeline", "gs_horus_set_jobdist", "gs_horus_fetch_jobdist", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
                  "gs_horus_run", "gs_horus_stats", "gs_horus_fetch"):
         getattr(lib, name).restype = C.c_int
@@ -282,6 +304,9 @@ def load_library():
     lib.gs_compare.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
                                C.c_void_p, C.c_void_p, f64p]
     lib.gs_compare.restype = C.c_int
+    lib.gs_set_slowdown.argtypes = [C.c_void_p, C.c_void_p]
+    lib.gs_fetch_slowdown.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.gs_set_slowdown.restype = lib.gs_fetch_slowdown.restype = C.c_int
     for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
                  "gs_boot_traces_blocked", "gs_boot_mixes", "gs_boot_traces_mixed", "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
         getattr(lib, name).restype = C.c_int
@@ -524,6 +549,17 @@ class HorusEngine:
         """(JCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3, E + 1)) as of the last summarize()"""
         return _fetch_jobdist(self, self.lib.gs_horus_fetch_jobdist, "gs_horus_fetch_jobdist", first, count)
 
+    def set_slowdown(self, key=None, bounds=(), tau=1, edges=(), sd_edges=()):
+        """job statistics by `key` ("gpus", "length" or "gpu-time") with bounded slowdown, filled by every summarize():
+        len(bounds) + 1 classes, tau the slowdown's lower bound on the run length, CDF counts at `edges` and `sd_edges`
+        (units of 1/1024); key=None turns it off (include/gsched_horus.h: gs_horus_set_slowdown)"""
+        _set_slowdown(self, self.lib.gs_horus_set_slowdown, "gs_horus_set_slowdown", key, bounds, tau, edges, sd_edges)
+
+    def slowdown(self, first=0, count=None):
+        """(SDCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3 * (E + 1) + Esd + 1)) as of the last
+        summarize()"""
+        return _fetch_slowdown(self, self.lib.gs_horus_fetch_slowdown, "gs_horus_fetch_slowdown", first, count)
+
     def compare(self, a, b, bounds=(), edges=(), with_time=False):
         """paired per-job comparison of replicas b[i] against a[i] on the same trace (include/gsched_horus.h:
         gs_horus_compare): (JPAIR_DTYPE records (P, C), uint32 CDF counts of d (P, C, 3, E + 1)); with_time: and the
@@ -552,6 +588,49 @@ def _set_jobdist(eng, fn, what, bounds, edges):
     eng._check(fn(eng.h, len(b) + 1, b.ctypes.data_as(C.c_void_p) if len(b) else None, len(e),
                   e.ctypes.data_as(C.c_void_p) if len(e) else None), what)
     eng._jd_shape = (len(b) + 1, len(e))
+
+
+def slowdown_cfg(key, bounds=(), tau=1, edges=(), sd_edges=()):
+    """(GsSlowdownCfg, the arrays it points to) of a setting; GsError(GS_ERR_ARG) for an unknown key or values that do
+    not fit the struct's fields (the library checks the rest)"""
+    if key not in JKEYS:
+        raise GsError(f"slowdown: key must be one of {sorted(JKEYS)}", GS_ERR_ARG)
+    b = np.asarray(bounds, dtype=object).reshape(-1)
+    e, se = (np.asarray(x, dtype=np.int64).reshape(-1) for x in (edges, sd_edges))
+    if len(b) > JOBDIST_MAX_CLASSES - 1 or any(not -2 ** 63 <= int(x) < 2 ** 63 for x in b) or not -2 ** 63 <= int(tau) < 2 ** 63:
+        raise GsError(f"slowdown: at most {JOBDIST_MAX_CLASSES - 1} int64 bounds and an int64 tau", GS_ERR_ARG)
+    for arr in (e, se):
+        if arr.size and (arr.min() < -2 ** 31 or arr.max() >= 2 ** 31):
+            raise GsError("slowdown: edges must be int32", GS_ERR_ARG)
+    e, se = np.ascontiguousarray(e, dtype=np.int32), np.ascontiguousarray(se, dtype=np.int32)
+    cfg = GsSlowdownCfg(JKEYS[key], len(b) + 1)
+    for i, x in enumerate(b):
+        cfg.bounds[i] = int(x)
+    cfg.tau = int(tau)
+    cfg.nedges, cfg.nsd_edges = len(e), len(se)
+    cfg.edges = e.ctypes.data if len(e) else None
+    cfg.sd_edges = se.ctypes.data if len(se) else None
+    return cfg, (e, se)
+
+
+def _set_slowdown(eng, fn, what, key, bounds, tau, edges, sd_edges):
+    if key is None:
+        eng._check(fn(eng.h, None), what)
+        eng._sd_shape = (0, 0)
+        return
+    cfg, keep = slowdown_cfg(key, bounds, tau, edges, sd_edges)
+    eng._check(fn(eng.h, C.byref(cfg)), what)
+    del keep
+    eng._sd_shape = (cfg.nclasses, 3 * (cfg.nedges + 1) + cfg.nsd_edges + 1)
+
+
+def _fetch_slowdown(eng, fn, what, first, count):
+    count = eng.nsims - first if count is None else int(count)
+    nc, row = getattr(eng, "_sd_shape", (0, 0))
+    recs = np.zeros((max(count, 1), max(nc, 1)), dtype=SDCLASS_DTYPE)
+    hist = np.zeros((max(count, 1), max(nc, 1), max(row, 1)), dtype=np.uint32)
+    eng._check(fn(eng.h, int(first), count, recs.ctypes.data_as(C.c_void_p), hist.ctypes.data_as(C.c_void_p)), what)
+    return recs[:count, :nc], hist[:count, :nc, :row]
 
 
 def _compare(eng, fn, what, a, b, bounds, edges, with_time):
@@ -919,6 +998,20 @@ class Engine:
         """(JCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3, E + 1)) of replicas [first, first+count)
         as of the last summarize(); count[..., m, b] = #(value m <= edges[b]) - #(value m <= edges[b - 1])"""
         return _fetch_jobdist(self, self.lib.gs_fetch_jobdist, "gs_fetch_jobdist", first, count)
+
+    def set_slowdown(self, key=None, bounds=(), tau=1, edges=(), sd_edges=()):
+        """while set, every summarize() also computes per-replica job statistics by `key` ("gpus", "length" = jct or
+        "gpu-time" = gpus * jct) on the device: len(bounds) + 1 classes (a job's class is the number of bounds <= its
+        key), bounded slowdown sd = 1024 * turnaround / max(jct, tau) in units of 1/1024 (at least 1024, at most
+        2^31 - 1), CDF counts of wait / turnaround / jct at `edges` and of sd at `sd_edges`; key=None turns it off.  May
+        be called at any time (include/gsched.h: gs_set_slowdown)"""
+        _set_slowdown(self, self.lib.gs_set_slowdown, "gs_set_slowdown", key, bounds, tau, edges, sd_edges)
+
+    def slowdown(self, first=0, count=None):
+        """(SDCLASS_DTYPE records (count, C), uint32 CDF counts (count, C, 3 * (E + 1) + Esd + 1): the wait, turnaround
+        and jct rows of E + 1 counts, then the sd row of Esd + 1) of replicas [first, first+count) as of the last
+        summarize()"""
+        return _fetch_slowdown(self, self.lib.gs_fetch_slowdown, "gs_fetch_slowdown", first, count)
 
     def compare(self, a, b, bounds=(), edges=(), with_time=False):
         """paired per-job comparison of replicas b[i] against a[i], which hold the same trace, over the jobs finished so

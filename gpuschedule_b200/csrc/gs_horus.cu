@@ -111,6 +111,7 @@ struct HorusSimHost {
   bool configured = false, loaded = false, prepared = false;
   bool tl_done = false;             // summarised with the timeline on since it was prepared
   bool jd_done = false;             // summarised with the current jobdist setting since it was prepared
+  bool sd_done = false;             // summarised with the current slowdown setting since it was prepared
   gs_cluster cl{};
   gs_horus_params par{};
   std::vector<HJob> jobs;
@@ -140,6 +141,9 @@ struct gs_horus_handle_s {
   gs_jclass *d_jd = nullptr; size_t jd_bytes = 0;       // gs_horus_set_jobdist: nsims x C class records
   unsigned *d_jd_hist = nullptr; size_t jd_hist_bytes = 0;   // and nsims x C x 3 x (E + 1) CDF counts
   GsJdCfg jd{};                                          // jd.nclasses = 0: off
+  gs_sdclass *d_sd = nullptr; size_t sd_bytes = 0;      // gs_horus_set_slowdown: nsims x C class records
+  unsigned *d_sd_hist = nullptr; size_t sd_hist_bytes = 0;   // and nsims x C x (3 (E + 1) + Esd + 1) CDF counts
+  GsSdCfg sd{};                                          // sd.nclasses = 0: off
   std::string err;
   std::vector<double> shared;       // one stream consumed by every replica that did not get its own
   double *d_shared = nullptr; size_t shared_cap = 0; bool shared_dirty = false;
@@ -191,6 +195,8 @@ extern "C" int gs_horus_destroy(gs_horus_handle h) {
   if (h->d_tl) cudaFree(h->d_tl);
   if (h->d_jd) cudaFree(h->d_jd);
   if (h->d_jd_hist) cudaFree(h->d_jd_hist);
+  if (h->d_sd) cudaFree(h->d_sd);
+  if (h->d_sd_hist) cudaFree(h->d_sd_hist);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -380,7 +386,7 @@ static int prepare(gs_horus_handle h, HorusSimHost &s, long long rows_cap) {
   D.rows_cap = rows_cap;
   D.current_remaining = (long long)n; D.running_jobs = 0;
   s.rows_cap = rows_cap;
-  s.prepared = true; s.tl_done = false; s.jd_done = false;
+  s.prepared = true; s.tl_done = false; s.jd_done = false; s.sd_done = false;
   return GS_OK;
 }
 
@@ -486,13 +492,13 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   HCU(cudaMemsetAsync(h->d_sum + first, 0, sizeof(gs_summary) * (size_t)count, h->stream));
   const int B = h->tl_nbins;
   if (B > 0) HCU(cudaMemsetAsync(h->d_tl + (size_t)first * B, 0, sizeof(gs_tbin) * (size_t)B * (size_t)count, h->stream));
-  const int C = h->jd.nclasses;
+  const int C = h->jd.nclasses, Csd = h->sd.nclasses;
 #ifdef __CUDACC__
   int per_sm = 1, sms = 132;
   HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_sum_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   const int grid = std::min(count, std::max(1, per_sm) * sms);
-  const size_t pitch = (size_t)(kmax + 63) / 64 * 64, need = 3 * sizeof(int) * pitch * (size_t)grid;
+  const size_t pitch = (size_t)(kmax + 63) / 64 * 64, need = (Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid;
   if (h->sum_scratch_bytes < need) {
     if (h->d_sum_scratch) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_sum_scratch); }
     h->d_sum_scratch = nullptr; h->sum_scratch_bytes = 0;
@@ -512,6 +518,15 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     const int grid_jd = std::min(grid, std::max(1, per_jd) * sms);
     gs_jd_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid_jd, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->jd,
                                                                                           h->d_jd, h->d_jd_hist, h->d_sum_scratch, (long long)pitch);
+    HCU(cudaGetLastError());
+    h->launches += 1;
+  }
+  if (Csd > 0) {          // after gs_sum_jobs_kernel, on the same scratch with a fourth row
+    int per_sd = 1;
+    HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sd, gs_sd_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
+    const int grid_sd = std::min(grid, std::max(1, per_sd) * sms);
+    gs_sd_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid_sd, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->sd,
+                                                                                          h->d_sd, h->d_sd_hist, h->d_sum_scratch, (long long)pitch);
     HCU(cudaGetLastError());
     h->launches += 1;
   }
@@ -538,6 +553,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     }
     gs_sum_jobs_serial(jobs.data(), S.nfin, A);
     if (C > 0) gs_jd_jobs_serial(jobs.data(), S.nfin, h->jd, h->d_jd + (size_t)r * C, h->d_jd_hist + (size_t)r * C * 3 * (h->jd.nedges + 1));
+    if (Csd > 0) gs_sd_serial(jobs.data(), S.nfin, h->sd, h->d_sd + (size_t)r * Csd, h->d_sd_hist + (size_t)r * Csd * gs_sd_row_len(h->sd));
     if (B > 0) gs_tl_fold_rows_serial(h->d_tl + (size_t)r * B, B, (long long)h->tl_width, S.rows, S.util, 0, 0, S.ticks);
   }
   (void)kmax;
@@ -552,6 +568,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   for (int i = first; i < first + count; ++i) {
     if (B > 0) h->sims[(size_t)i].tl_done = true;
     if (C > 0) h->sims[(size_t)i].jd_done = true;
+    if (Csd > 0) h->sims[(size_t)i].sd_done = true;
   }
   return GS_OK;
 }
@@ -632,6 +649,52 @@ extern "C" int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t 
     HCU(cudaMemcpyAsync(classes_out, h->d_jd + (size_t)first * C, sizeof(gs_jclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   if (hist_out)
     HCU(cudaMemcpyAsync(hist_out, h->d_jd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
+  return GS_OK;
+}
+
+extern "C" int gs_horus_set_slowdown(gs_horus_handle h, const gs_slowdown_cfg *in) {
+  if (!h) return GS_ERR_ARG;
+  GsSdCfg cfg;
+  const char *why = nullptr;
+  if (!gs_sd_make_cfg(in, cfg, &why)) return hfail(h, GS_ERR_ARG, std::string("gs_horus_set_slowdown: ") + why);
+  const size_t need = sizeof(gs_sdclass) * h->sims.size() * (size_t)cfg.nclasses;
+  const size_t need_hist = sizeof(unsigned) * h->sims.size() * (size_t)cfg.nclasses * (size_t)gs_sd_row_len(cfg);
+  if (need > h->sd_bytes || need_hist > h->sd_hist_bytes) {
+    HCU(cudaSetDevice(h->device));
+    gs_sdclass *d = nullptr;
+    unsigned *dh = nullptr;
+    HCU(cudaMalloc(&d, std::max(need, h->sd_bytes)));
+    if (cudaMalloc(&dh, std::max(need_hist, h->sd_hist_bytes)) != cudaSuccess) {
+      cudaFree(d);
+      return hfail(h, GS_ERR_CUDA, "gs_horus_set_slowdown: cudaMalloc failed");
+    }
+    HCU(cudaStreamSynchronize(h->stream));
+    if (h->d_sd) cudaFree(h->d_sd);
+    if (h->d_sd_hist) cudaFree(h->d_sd_hist);
+    h->d_sd = d; h->sd_bytes = std::max(need, h->sd_bytes);
+    h->d_sd_hist = dh; h->sd_hist_bytes = std::max(need_hist, h->sd_hist_bytes);
+  }
+  h->sd = cfg;
+  for (auto &s : h->sims) s.sd_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_fetch_slowdown(gs_horus_handle h, int32_t first, int32_t count, gs_sdclass *out, uint32_t *hist_out) {
+  if (!h) return GS_ERR_ARG;
+  const int nsims = (int)h->sims.size();
+  if (first < 0 || count < 0 || first > nsims - count) return hfail(h, GS_ERR_ARG, "gs_horus_fetch_slowdown: bad arguments");
+  if (h->sd.nclasses == 0) return hfail(h, GS_ERR_STATE, "gs_horus_fetch_slowdown: the slowdown statistics are off (gs_horus_set_slowdown)");
+  for (int i = first; i < first + count; ++i)
+    if (!h->sims[(size_t)i].prepared || !h->sims[(size_t)i].sd_done)
+      return hfail(h, GS_ERR_STATE, "gs_horus_fetch_slowdown: a replica has not been summarised with this setting since it was prepared");
+  if (count == 0) return GS_OK;
+  HCU(cudaSetDevice(h->device));
+  const size_t C = (size_t)h->sd.nclasses, per = C * (size_t)gs_sd_row_len(h->sd);
+  if (out)
+    HCU(cudaMemcpyAsync(out, h->d_sd + (size_t)first * C, sizeof(gs_sdclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  if (hist_out)
+    HCU(cudaMemcpyAsync(hist_out, h->d_sd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   HCU(cudaStreamSynchronize(h->stream));
   return GS_OK;
 }

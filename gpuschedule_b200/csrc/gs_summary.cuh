@@ -288,6 +288,72 @@ GS_SUM_HD void gs_jd_add_sq(uint64_t &lo, uint64_t &hi, int v) { gs_sum_add128(l
 
 static_assert(sizeof(gs_jpair) == 288, "gs_jpair is 288 bytes");
 
+// ---- job statistics by a chosen key, with bounded slowdown (gs_sdclass, include/gsched.h)
+static_assert(sizeof(gs_sdclass) == 232 && sizeof(gs_sdclass) % 8 == 0, "gs_sdclass is 232 bytes, a multiple of 8");
+#define GS_SD_MAX 0x7fffffffll       // the saturated slowdown, 2^31 - 1 (units of 1/1024)
+
+// A slowdown setting, passed to the kernel by value (2.1 KB of parameters; the edges are staged in shared memory).
+struct GsSdCfg {
+  int key, nclasses, nedges, nsd;
+  long long bounds[GS_JOBDIST_MAX_CLASSES - 1];
+  long long tau;
+  int edges[GS_JOBDIST_MAX_EDGES];
+  int sd_edges[GS_SLOWDOWN_MAX_EDGES];
+};
+
+// Key of a job (GS_JKEY_*): gpus, jct or gpus * jct.
+GS_SUM_HD long long gs_sd_key(int key, int gpus, int jct) {
+  return key == GS_JKEY_GPUS ? (long long)gpus : key == GS_JKEY_LENGTH ? (long long)jct : (long long)gpus * jct;
+}
+
+// Class of a key: the number of the nb = C - 1 increasing bounds that are <= key.
+GS_SUM_HD int gs_sd_class(const long long *bounds, int nb, long long key) {
+  int c = 0;
+  while (c < nb && bounds[c] <= key) ++c;
+  return c;
+}
+
+// Bounded slowdown in units of 1/1024: min(2^31 - 1, max(1024, floor(1024 * turn / max(jct, tau)))), in 64-bit
+// integers.  turn = end - arrive >= 0 and tau >= 1, so the quotient is a floor and the divisor is >= 1; 1024 * turn
+// < 2^41.
+GS_SUM_HD int gs_sd_value(int turn, int jct, long long tau) {
+  const long long den = (long long)jct > tau ? (long long)jct : tau;
+  const long long q = 1024ll * turn / den;
+  return q < 1024 ? 1024 : q > GS_SD_MAX ? (int)GS_SD_MAX : (int)q;
+}
+
+// A slowdown setting from the C ABI's struct, or false (the message in *why) when it is not valid.  cfg == NULL is off.
+static inline bool gs_sd_make_cfg(const gs_slowdown_cfg *in, GsSdCfg &cfg, const char **why) {
+  cfg = GsSdCfg{};
+  if (!in || in->nclasses == 0) return true;
+  *why = "key must be GS_JKEY_GPUS, GS_JKEY_LENGTH or GS_JKEY_GPU_TIME";
+  if (in->key != GS_JKEY_GPUS && in->key != GS_JKEY_LENGTH && in->key != GS_JKEY_GPU_TIME) return false;
+  *why = "nclasses must be in 0..8, nedges and nsd_edges in 0..255";
+  if (in->nclasses < 0 || in->nclasses > GS_JOBDIST_MAX_CLASSES || in->nedges < 0 || in->nedges > GS_JOBDIST_MAX_EDGES ||
+      in->nsd_edges < 0 || in->nsd_edges > GS_SLOWDOWN_MAX_EDGES) return false;
+  *why = "tau must be >= 1";
+  if (in->tau < 1) return false;
+  *why = "a NULL array with a positive count";
+  if ((in->nedges > 0 && !in->edges) || (in->nsd_edges > 0 && !in->sd_edges)) return false;
+  *why = "the class bounds must be >= 1 and strictly increasing";
+  for (int i = 0; i < in->nclasses - 1; ++i)
+    if (in->bounds[i] < 1 || (i > 0 && in->bounds[i] <= in->bounds[i - 1])) return false;
+  *why = "the edges must be strictly increasing";
+  for (int i = 1; i < in->nedges; ++i)
+    if (in->edges[i] <= in->edges[i - 1]) return false;
+  *why = "the sd edges must be strictly increasing";
+  for (int i = 1; i < in->nsd_edges; ++i)
+    if (in->sd_edges[i] <= in->sd_edges[i - 1]) return false;
+  cfg.key = in->key; cfg.nclasses = in->nclasses; cfg.nedges = in->nedges; cfg.nsd = in->nsd_edges; cfg.tau = in->tau;
+  for (int i = 0; i < in->nclasses - 1; ++i) cfg.bounds[i] = in->bounds[i];
+  for (int i = 0; i < in->nedges; ++i) cfg.edges[i] = in->edges[i];
+  for (int i = 0; i < in->nsd_edges; ++i) cfg.sd_edges[i] = in->sd_edges[i];
+  return true;
+}
+
+// uint32 counts per (replica, class): wait, turnaround and jct E + 1 each, then sd Esd + 1.
+GS_SUM_HD long long gs_sd_row_len(const GsSdCfg &cfg) { return 3ll * (cfg.nedges + 1) + cfg.nsd + 1; }
+
 #ifndef __CUDACC__
 #include <vector>
 // Host forms of the job part (the host-emulation build of gs_horus.cu, CPU tests): the same sums, and the same radix
@@ -426,6 +492,66 @@ static inline void gs_cmp_pair_serial(const GsSumJob *ja, const GsSumJob *jb, lo
       for (int t = 0; t < 5; ++t) P.q_lo[m][t] = -q[t];
     }
     off += kc;
+  }
+}
+
+// Slowdown statistics of k finished jobs: out[0 .. C) and hist[C][3 * (E + 1) + Esd + 1] (overwritten).  The kernel's
+// steps, serially: count per class (and sum the keys), write wait / turnaround / jct / sd into per-class segments, fold
+// each segment, select within it.
+static inline void gs_sd_serial(const GsSumJob *jobs, long long k, const GsSdCfg &cfg, gs_sdclass *out, uint32_t *hist) {
+  const int C = cfg.nclasses, nb = cfg.nedges + 1;
+  const long long row = gs_sd_row_len(cfg);
+  long long off[GS_JOBDIST_MAX_CLASSES + 1] = {0};
+  for (int c = 0; c < C; ++c) out[c] = gs_sdclass{};
+  for (long long i = 0; i < (long long)C * row; ++i) hist[i] = 0;
+  std::vector<int> cls((size_t)(k > 0 ? k : 1));
+  for (long long i = 0; i < k; ++i) {
+    const GsSumJob &v = jobs[i];
+    const long long key = gs_sd_key(cfg.key, v.gpus, v.jct);
+    const int c = gs_sd_class(cfg.bounds, C - 1, key);
+    cls[(size_t)i] = c;
+    off[c + 1] += 1;
+    gs_sdclass &S = out[c];
+    S.jc.preempt_sum += v.preempt; S.jc.gpu_ticks_sum += (long long)v.gpus * v.jct;
+    gs_sum_add128(S.key_sum_lo, S.key_sum_hi, (gs_i128)key);
+  }
+  for (int c = 0; c < C; ++c) off[c + 1] += off[c];
+  const long long pitch = k > 0 ? k : 1;
+  std::vector<int> vals((size_t)(4 * pitch));
+  long long cur[GS_JOBDIST_MAX_CLASSES];
+  for (int c = 0; c < C; ++c) cur[c] = off[c];
+  for (long long i = 0; i < k; ++i) {
+    const GsSumJob &v = jobs[i];
+    const long long pos = cur[cls[(size_t)i]]++;
+    vals[(size_t)pos] = v.wait; vals[(size_t)(pitch + pos)] = v.turn; vals[(size_t)(2 * pitch + pos)] = v.jct;
+    vals[(size_t)(3 * pitch + pos)] = gs_sd_value(v.turn, v.jct, cfg.tau);
+  }
+  for (int c = 0; c < C; ++c) {
+    gs_sdclass &S = out[c];
+    gs_jclass &J = S.jc;
+    const long long kc = off[c + 1] - off[c];
+    const int *seg = vals.data() + off[c];
+    J.jobs = kc;
+    uint32_t *hc = hist + (size_t)c * row;
+    for (long long i = 0; i < kc; ++i) {
+      const int w = seg[i], t = seg[pitch + i], j = seg[2 * pitch + i], sd = seg[3 * pitch + i];
+      J.wait_sum += w; J.turnaround_sum += t; J.jct_sum += j;
+      gs_jd_add_sq(J.wait_sq_lo, J.wait_sq_hi, w);
+      gs_jd_add_sq(J.turnaround_sq_lo, J.turnaround_sq_hi, t);
+      gs_jd_add_sq(J.jct_sq_lo, J.jct_sq_hi, j);
+      S.sd_sum += sd;
+      gs_jd_add_sq(S.sd_sq_lo, S.sd_sq_hi, sd);
+      S.sd_min = i == 0 || sd < S.sd_min ? sd : S.sd_min;
+      S.sd_clamped += sd == (int)GS_SD_MAX;
+      hc[gs_jd_bin(cfg.edges, cfg.nedges, w)] += 1;
+      hc[nb + gs_jd_bin(cfg.edges, cfg.nedges, t)] += 1;
+      hc[2 * nb + gs_jd_bin(cfg.edges, cfg.nedges, j)] += 1;
+      hc[3 * nb + gs_jd_bin(cfg.sd_edges, cfg.nsd, sd)] += 1;
+    }
+    gs_sum_select_serial(seg, kc, J.wait_q);
+    gs_sum_select_serial(seg + pitch, kc, J.turnaround_q);
+    gs_sum_select_serial(seg + 2 * pitch, kc, J.jct_q);
+    gs_sum_select_serial(seg + 3 * pitch, kc, S.sd_q);
   }
 }
 #endif
@@ -666,25 +792,28 @@ __device__ void gs_sum_block_vec(long long (&v)[N]) {
   __syncthreads();
 }
 
-// Radix select of the 15 order statistics (3 value columns x 5 ranks) of k values per column, vals[m * pitch + i]
-// (i < k), whose column minima are mn[0 .. 3) and whose largest column range is `span`.  prefix[t] (shared) receives
-// target t's value minus its column's minimum; hist: GS_SUM_TARGETS * GS_SUM_BINS shared counters.  k = 0: no pass is
-// run and prefix is not to be read.  Block-cooperative: every thread calls it with the same arguments, and the
+// Radix select of the 5 * M order statistics (M value columns x 5 ranks; M = 3 unless stated) of k values per column,
+// vals[m * pitch + i] (i < k), whose column minima are mn[0 .. M) and whose largest column range is `span`.  prefix[t]
+// (shared) receives target t's value minus its column's minimum; hist: 5 * M * GS_SUM_BINS shared counters.  k = 0: no
+// pass is run and prefix is not to be read.  Block-cooperative: every thread calls it with the same arguments, and the
 // scratch writes it reads must be published by a barrier before the call.
+template <int M = 3>
 __device__ __forceinline__ void gs_sum_select(unsigned *hist, unsigned long long *prefix, const int *vals, long long pitch, long long k,
                                               const long long *mn, long long span) {
-  __shared__ long long rank[GS_SUM_TARGETS];
-  __shared__ int leader[GS_SUM_TARGETS];
+  constexpr int T = 5 * M;
+  static_assert(T <= GS_SUM_TARGETS, "at most GS_SUM_TARGETS targets");
+  __shared__ long long rank[T];
+  __shared__ int leader[T];
   const int passes = k > 0 ? gs_sum_passes((unsigned long long)span) : 0;
-  if (threadIdx.x < GS_SUM_TARGETS) {
+  if (threadIdx.x < T) {
     prefix[threadIdx.x] = 0;
     rank[threadIdx.x] = k > 0 ? gs_sum_rank(gs_sum_permille(threadIdx.x % 5), k) : 0;
   }
   for (int p = 0; p < passes; ++p) {
     const int shift = (passes - 1 - p) * 9;
-    for (int i = threadIdx.x; i < GS_SUM_TARGETS * GS_SUM_BINS; i += blockDim.x) hist[i] = 0;
+    for (int i = threadIdx.x; i < T * GS_SUM_BINS; i += blockDim.x) hist[i] = 0;
     __syncthreads();
-    if (threadIdx.x < GS_SUM_TARGETS) {                    // targets of one value with the same prefix share a histogram
+    if (threadIdx.x < T) {                                 // targets of one value with the same prefix share a histogram
       const int t = threadIdx.x, m0 = (t / 5) * 5;
       int L = t;
       for (int u = m0; u < t; ++u) if (prefix[u] == prefix[t]) { L = u; break; }
@@ -693,7 +822,7 @@ __device__ __forceinline__ void gs_sum_select(unsigned *hist, unsigned long long
     __syncthreads();
     for (long long i = threadIdx.x; i < k; i += blockDim.x) {
 #pragma unroll
-      for (int m = 0; m < 3; ++m) {
+      for (int m = 0; m < M; ++m) {
         const unsigned long long u = (unsigned long long)((long long)vals[m * pitch + i] - mn[m]);
         const unsigned long long hp = u >> (shift + 9);
         const unsigned d = (unsigned)(u >> shift) & (GS_SUM_BINS - 1);
@@ -706,7 +835,7 @@ __device__ __forceinline__ void gs_sum_select(unsigned *hist, unsigned long long
       }
     }
     __syncthreads();
-    if (threadIdx.x < GS_SUM_TARGETS) {
+    if (threadIdx.x < T) {
       const int t = threadIdx.x;
       long long rk = rank[t];
       const unsigned d = gs_sum_pick(hist + leader[t] * GS_SUM_BINS, rk);
@@ -857,6 +986,148 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_jd_jobs_kernel(Src src, int
           J.jct_q[t] = kc > 0 ? (int)(s[11] + (long long)prefix[10 + t]) : 0;
         }
         classes[(size_t)r * C + c] = J;
+      }
+      __syncthreads();
+      off += kc;
+    }
+  }
+}
+
+// Slowdown statistics (gs_sdclass) of replicas first .. first + count - 1 (the jobs of gs_sum_jobs_kernel, whose
+// scratch it reuses with a fourth row), one block per replica in turn (grid-stride), in gs_jd_jobs_kernel's steps:
+// (1) per-class job counts, preempt / gpu-tick sums and key sums (as sums of the keys' 32-bit halves), kept in registers
+// per class and block-reduced; (2) class offsets; (3) every job's wait, turnaround, jct and sd written to its class's
+// segment of the scratch through warp-aggregated shared cursors; (4) per class in turn: jobdist's fold of the three
+// values (sums, 128-bit sums of squares as sums of 32-bit halves, min / max, CDF counts), then the same fold of sd
+// (with the count of saturated values), then gs_sum_select over the three rows and a second, one-row gs_sum_select
+// over the sd row (a widened 20-target select would need 40 KB of histogram counters on its own).
+// Outputs: recs[r * C + c], hists[(r * C + c) * (3 * (E + 1) + Esd + 1) + ...] ([wait, turnaround, jct, sd][bin]).
+template <class Src>
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_sd_jobs_kernel(Src src, int first, int count, GsSdCfg cfg, gs_sdclass *recs,
+                                                                   unsigned *hists, int *scratch, long long pitch) {
+  constexpr int NC = GS_JOBDIST_MAX_CLASSES;
+  __shared__ unsigned hist[GS_SUM_TARGETS * GS_SUM_BINS];
+  __shared__ unsigned long long prefix[GS_SUM_TARGETS];
+  __shared__ unsigned cdf[3 * (GS_JOBDIST_MAX_EDGES + 1) + GS_SLOWDOWN_MAX_EDGES + 1];
+  __shared__ int edges[GS_JOBDIST_MAX_EDGES], sd_edges[GS_SLOWDOWN_MAX_EDGES];
+  __shared__ long long cls_sum[5][NC];          // jobs, preempt_sum, gpu_ticks_sum, key low halves, key high halves
+  __shared__ long long cursor[NC];
+  __shared__ gs_sdclass rec;
+  const int C = cfg.nclasses, E = cfg.nedges, nb = E + 1, Es = cfg.nsd;
+  const int row = 3 * nb + Es + 1;
+  const int lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < E; i += blockDim.x) edges[i] = cfg.edges[i];
+  for (int i = threadIdx.x; i < Es; i += blockDim.x) sd_edges[i] = cfg.sd_edges[i];
+  int *vals = scratch + (size_t)blockIdx.x * 4 * (size_t)pitch;
+  for (int b = blockIdx.x; b < count; b += gridDim.x) {
+    const int r = first + b;
+    const long long k = src.finished(r);
+    long long red[5 * NC];
+#pragma unroll
+    for (int e = 0; e < 5 * NC; ++e) red[e] = 0;
+    for (long long i = threadIdx.x; i < k; i += blockDim.x) {
+      const GsSumJob v = src.job(r, i);
+      const long long key = gs_sd_key(cfg.key, v.gpus, v.jct);
+      const int c = gs_sd_class(cfg.bounds, C - 1, key);
+#pragma unroll
+      for (int u = 0; u < NC; ++u) {
+        if (c == u) {
+          red[u] += 1; red[NC + u] += v.preempt; red[2 * NC + u] += (long long)v.gpus * v.jct;
+          red[3 * NC + u] += key & 0xffffffffll; red[4 * NC + u] += key >> 32;
+        }
+      }
+    }
+    gs_sum_block_vec<5 * NC, 5 * NC, 0>(red);
+    if (threadIdx.x < NC) {
+      const int c = threadIdx.x;
+      long long off = 0;
+#pragma unroll
+      for (int u = 0; u < NC; ++u) off += u < c ? red[u] : 0;
+#pragma unroll
+      for (int u = 0; u < NC; ++u) {
+        if (u == c)
+          for (int m = 0; m < 5; ++m) cls_sum[m][c] = red[m * NC + u];
+      }
+      cursor[c] = off;
+    }
+    __syncthreads();
+    for (long long i0 = 0; i0 < k; i0 += blockDim.x) {     // (warp-uniform trip count: the shuffles see full warps)
+      const long long i = i0 + threadIdx.x;
+      const bool in = i < k;
+      GsSumJob v;
+      int c = -1;
+      if (in) { v = src.job(r, i); c = gs_sd_class(cfg.bounds, C - 1, gs_sd_key(cfg.key, v.gpus, v.jct)); }
+      const unsigned peers = __match_any_sync(0xffffffffu, c);
+      const int head = __ffs(peers) - 1;
+      long long base = 0;
+      if (in && lane == head) base = atomicAdd((unsigned long long *)&cursor[c], (unsigned long long)__popc(peers));
+      base = __shfl_sync(0xffffffffu, base, head);
+      if (in) {
+        const long long pos = base + __popc(peers & ((1u << lane) - 1u));
+        vals[pos] = v.wait; vals[pitch + pos] = v.turn; vals[2 * pitch + pos] = v.jct;
+        vals[3 * pitch + pos] = gs_sd_value(v.turn, v.jct, cfg.tau);
+      }
+    }
+    __syncthreads();
+    long long off = 0;
+    for (int c = 0; c < C; ++c) {
+      const long long kc = cls_sum[0][c];
+      const int *seg = vals + off;
+      for (int i = threadIdx.x; i < row; i += blockDim.x) cdf[i] = 0;
+      __syncthreads();
+      // wait, turnaround, jct: sums; squares as the sums of their high and low 32-bit halves; minima; maxima
+      long long s[15] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0x7fffffff, 0x7fffffff, 0x7fffffff, -0x80000000ll, -0x80000000ll, -0x80000000ll};
+      for (long long i = threadIdx.x; i < kc; i += blockDim.x) {
+#pragma unroll
+        for (int m = 0; m < 3; ++m) {
+          const int v = seg[m * pitch + i];
+          const unsigned long long sq = (unsigned long long)((long long)v * v);
+          s[m] += v; s[3 + m] += (long long)(sq >> 32); s[6 + m] += (long long)(sq & 0xffffffffull);
+          s[9 + m] = min(s[9 + m], (long long)v); s[12 + m] = max(s[12 + m], (long long)v);
+          atomicAdd(&cdf[m * nb + gs_jd_bin(edges, E, v)], 1u);
+        }
+      }
+      gs_sum_block_vec<15, 9, 3>(s);
+      // sd: sum, square halves, saturated count, minimum, maximum
+      long long t[6] = {0, 0, 0, 0, GS_SD_MAX, 0};
+      for (long long i = threadIdx.x; i < kc; i += blockDim.x) {
+        const int v = seg[3 * pitch + i];
+        const unsigned long long sq = (unsigned long long)((long long)v * v);
+        t[0] += v; t[1] += (long long)(sq >> 32); t[2] += (long long)(sq & 0xffffffffull); t[3] += v == (int)GS_SD_MAX;
+        t[4] = min(t[4], (long long)v); t[5] = max(t[5], (long long)v);
+        atomicAdd(&cdf[3 * nb + gs_jd_bin(sd_edges, Es, v)], 1u);
+      }
+      gs_sum_block_vec<6, 4, 1>(t);                         // (its barriers also publish the CDF counts)
+      unsigned *hout = hists + ((size_t)r * C + c) * (size_t)row;
+      for (int i = threadIdx.x; i < row; i += blockDim.x) hout[i] = cdf[i];
+      long long span = 0;
+#pragma unroll
+      for (int m = 0; m < 3; ++m) span = max(span, s[12 + m] - s[9 + m]);
+      gs_sum_select(hist, prefix, seg, pitch, kc, s + 9, span);
+      if (threadIdx.x == 0) {
+        rec = gs_sdclass{};
+        gs_jclass &J = rec.jc;
+        J.jobs = kc; J.wait_sum = s[0]; J.turnaround_sum = s[1]; J.jct_sum = s[2];
+        J.preempt_sum = cls_sum[1][c]; J.gpu_ticks_sum = cls_sum[2][c];
+        gs_sum_add128(J.wait_sq_lo, J.wait_sq_hi, ((gs_i128)s[3] << 32) + s[6]);
+        gs_sum_add128(J.turnaround_sq_lo, J.turnaround_sq_hi, ((gs_i128)s[4] << 32) + s[7]);
+        gs_sum_add128(J.jct_sq_lo, J.jct_sq_hi, ((gs_i128)s[5] << 32) + s[8]);
+        for (int q = 0; q < 5; ++q) {
+          J.wait_q[q] = kc > 0 ? (int)(s[9] + (long long)prefix[q]) : 0;
+          J.turnaround_q[q] = kc > 0 ? (int)(s[10] + (long long)prefix[5 + q]) : 0;
+          J.jct_q[q] = kc > 0 ? (int)(s[11] + (long long)prefix[10 + q]) : 0;
+        }
+        rec.sd_sum = t[0];
+        gs_sum_add128(rec.sd_sq_lo, rec.sd_sq_hi, ((gs_i128)t[1] << 32) + t[2]);
+        rec.sd_clamped = t[3];
+        rec.sd_min = kc > 0 ? (int)t[4] : 0;
+        gs_sum_add128(rec.key_sum_lo, rec.key_sum_hi, ((gs_i128)cls_sum[4][c] << 32) + cls_sum[3][c]);
+      }
+      __syncthreads();                                      // thread 0 has read prefix before the second select
+      gs_sum_select<1>(hist, prefix, seg + 3 * pitch, pitch, kc, t + 4, t[5] - t[4]);
+      if (threadIdx.x == 0) {
+        for (int q = 0; q < 5; ++q) rec.sd_q[q] = kc > 0 ? (int)(t[4] + (long long)prefix[q]) : 0;
+        recs[(size_t)r * C + c] = rec;
       }
       __syncthreads();
       off += kc;

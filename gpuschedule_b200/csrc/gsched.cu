@@ -86,6 +86,7 @@ struct SimHost {
   bool tl_fresh = true;                   // gs_set_timeline: the bins are to be zeroed before the next fold
   bool tl_done = false;                   // summarised with the timeline on since it was prepared
   bool jd_done = false;                   // summarised with the current jobdist setting since it was prepared
+  bool sd_done = false;                   // summarised with the current slowdown setting since it was prepared
   SimDev dev;
   SimLayout layout;
 };
@@ -125,6 +126,9 @@ struct gs_engine {
   gs_jclass *d_jd = nullptr; size_t jd_bytes = 0;       // gs_set_jobdist: nsims x C class records
   unsigned *d_jd_hist = nullptr; size_t jd_hist_bytes = 0;   // and nsims x C x 3 x (E + 1) CDF counts
   GsJdCfg jd{};                                          // jd.nclasses = 0: off
+  gs_sdclass *d_sd = nullptr; size_t sd_bytes = 0;      // gs_set_slowdown: nsims x C class records
+  unsigned *d_sd_hist = nullptr; size_t sd_hist_bytes = 0;   // and nsims x C x (3 (E + 1) + Esd + 1) CDF counts
+  GsSdCfg sd{};                                          // sd.nclasses = 0: off
   // gs_boot_population: the records of the base trace, then its k - 1 gaps (int32)
   void *d_pop = nullptr; int64_t pop_k = 0; int64_t pop_max_gap = 0; double pop_max_need = 1.0;
   // gs_boot_mixes: nmix alias tables of pop_k entries each, mix-major, and their weight sums
@@ -208,6 +212,8 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->d_tl) cudaFree(h->d_tl);
   if (h->d_jd) cudaFree(h->d_jd);
   if (h->d_jd_hist) cudaFree(h->d_jd_hist);
+  if (h->d_sd) cudaFree(h->d_sd);
+  if (h->d_sd_hist) cudaFree(h->d_sd_hist);
   if (h->d_pop) cudaFree(h->d_pop);
   if (h->d_mix) cudaFree(h->d_mix);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
@@ -538,7 +544,7 @@ static int bind_sim(gs_handle h, SimHost &s, const SimLayout &L, unsigned char *
   D.mem_busy = D.sum_arr = D.span_used = D.events = D.evals = D.started = D.ticks = D.row_first = 0;
   D.need_init = 1;
   s.sum_rows = 0; s.sum_fresh = true;
-  s.tl_fresh = true; s.tl_done = false; s.jd_done = false;
+  s.tl_fresh = true; s.tl_done = false; s.jd_done = false; s.sd_done = false;
   s.prepared = true;
   return GS_OK;
 }
@@ -1159,7 +1165,8 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   const int grid = std::min(count, std::max(1, per_sm) * sms);
   const size_t pitch = (size_t)align_up((size_t)kmax, 64);
-  int rc = ensure_scratch(h, 3 * sizeof(int) * pitch * (size_t)grid);
+  const int Csd = h->sd.nclasses;
+  int rc = ensure_scratch(h, (Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid);   // gs_sd_jobs_kernel: a fourth row
   if (rc) return rc;
   const int B = h->tl_nbins;
   for (int i = first; i < first + count; ++i) {
@@ -1190,6 +1197,15 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
     CU(cudaGetLastError());
     h->launches += 1;
   }
+  if (Csd > 0) {          // after gs_sum_jobs_kernel (and gs_jd_jobs_kernel), on the same scratch
+    int per_sd = 1;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sd, gs_sd_jobs_kernel<GsSumEngineJobs>, GS_SUM_THREADS, 0));
+    const int grid_sd = std::min(grid, std::max(1, per_sd) * sms);
+    gs_sd_jobs_kernel<GsSumEngineJobs><<<(unsigned)grid_sd, GS_SUM_THREADS, 0, h->stream>>>(src, first, count, h->sd, h->d_sd, h->d_sd_hist,
+                                                                                           (int *)h->d_scratch, (long long)pitch);
+    CU(cudaGetLastError());
+    h->launches += 1;
+  }
   CU(cudaEventRecord(h->e1, h->stream));
   CU(cudaMemcpyAsync(out, h->d_sum + first, sizeof(gs_summary) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
@@ -1199,6 +1215,7 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
     h->sims[(size_t)i].sum_rows = out[i - first].rows;
     if (B > 0) h->sims[(size_t)i].tl_done = true;
     if (C > 0) h->sims[(size_t)i].jd_done = true;
+    if (Csd > 0) h->sims[(size_t)i].sd_done = true;
   }
   return GS_OK;
 }
@@ -1283,6 +1300,53 @@ extern "C" int gs_fetch_jobdist(gs_handle h, int first, int count, gs_jclass *cl
     CU(cudaMemcpyAsync(classes_out, h->d_jd + (size_t)first * C, sizeof(gs_jclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   if (hist_out)
     CU(cudaMemcpyAsync(hist_out, h->d_jd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  CU(wait_stream(h));
+  return GS_OK;
+}
+
+extern "C" int gs_set_slowdown(gs_handle h, const gs_slowdown_cfg *in) {
+  if (!h) return GS_ERR_ARG;
+  GsSdCfg cfg;
+  const char *why = nullptr;
+  if (!gs_sd_make_cfg(in, cfg, &why)) return fail(h, GS_ERR_ARG, std::string("gs_set_slowdown: ") + why);
+  const size_t need = sizeof(gs_sdclass) * (size_t)h->nsims * (size_t)cfg.nclasses;
+  const size_t need_hist = sizeof(unsigned) * (size_t)h->nsims * (size_t)cfg.nclasses * (size_t)gs_sd_row_len(cfg);
+  if (need > h->sd_bytes || need_hist > h->sd_hist_bytes) {
+    CU(cudaSetDevice(h->device));
+    gs_sdclass *d = nullptr;
+    unsigned *dh = nullptr;
+    CU(cudaMalloc(&d, std::max(need, h->sd_bytes)));
+    if (cudaMalloc(&dh, std::max(need_hist, h->sd_hist_bytes)) != cudaSuccess) {
+      cudaFree(d);
+      return fail(h, GS_ERR_CUDA, "gs_set_slowdown: cudaMalloc failed");
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    if (h->d_sd) cudaFree(h->d_sd);
+    if (h->d_sd_hist) cudaFree(h->d_sd_hist);
+    h->d_sd = d; h->sd_bytes = std::max(need, h->sd_bytes);
+    h->d_sd_hist = dh; h->sd_hist_bytes = std::max(need_hist, h->sd_hist_bytes);
+  }
+  h->sd = cfg;
+  for (SimHost &s : h->sims) s.sd_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_fetch_slowdown(gs_handle h, int first, int count, gs_sdclass *out, uint32_t *hist_out) {
+  if (!h) return GS_ERR_ARG;
+  if (first < 0 || count < 0 || first + count > h->nsims) return fail(h, GS_ERR_ARG, "gs_fetch_slowdown: bad arguments");
+  if (h->sd.nclasses == 0) return fail(h, GS_ERR_STATE, "gs_fetch_slowdown: the slowdown statistics are off (gs_set_slowdown)");
+  for (int i = first; i < first + count; ++i) {
+    const SimHost &s = h->sims[(size_t)i];
+    if (!s.prepared || !s.sd_done)
+      return fail(h, GS_ERR_STATE, "gs_fetch_slowdown: a replica has not been summarised with this setting since it was prepared");
+  }
+  if (count == 0) return GS_OK;
+  CU(cudaSetDevice(h->device));
+  const size_t C = (size_t)h->sd.nclasses, per = C * (size_t)gs_sd_row_len(h->sd);
+  if (out)
+    CU(cudaMemcpyAsync(out, h->d_sd + (size_t)first * C, sizeof(gs_sdclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  if (hist_out)
+    CU(cudaMemcpyAsync(hist_out, h->d_sd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(wait_stream(h));
   return GS_OK;
 }

@@ -21,6 +21,11 @@ turnaround and jct, and their CDF at every edge -- job_analysis.ipynb's breakdow
 scheduler_analysis.ipynb's mean / median / std -- and `jobdist_spread` their spread per class over the replicas that
 have jobs in that class.
 
+Job statistics by a chosen key with bounded slowdown (capi.SDCLASS_DTYPE records and CDF counts from
+Engine.slowdown / HorusEngine.slowdown): `slowdown_derived` gives per class jobdist's numbers, the mean key and the
+mean, sample std, minimum and five quantiles of the bounded slowdown (in units of slowdown: the record's fixed point
+over 1024), and the four CDFs; `slowdown_spread` their spread per class over the replicas that have jobs in it.
+
 Paired comparisons (capi.JPAIR_DTYPE records and CDF counts from Engine.compare / HorusEngine.compare): `pair_derived`
 gives per class and quantity the per-job differences d = x_b - x_a of two configurations on the same trace -- their
 mean, sample std, shares below / at / above zero, ten order statistics and CDF --, `pair_spread` their spread over
@@ -318,6 +323,106 @@ def jobdist_spread_columns():
 
 def jobdist_spread_flat(sp, c):
     return [float(sp[name][s][c]) for name in JOBDIST_METRICS for s in SPREAD_STATS]
+
+
+# ---------------------------------------------------------------- job statistics by key with bounded slowdown
+SLOWDOWN_ONE = 1024                                       # fixed-point units of sd per unit of slowdown
+SLOWDOWN_QUANTITIES = JOBDIST_QUANTITIES + ("sd",)
+SLOWDOWN_METRICS = ("key_mean", "sd_mean", "sd_std") + tuple(f"sd_p{q}" for q in QUANTILES) + ("sd_min",) + JOBDIST_METRICS
+SLOWDOWN_COUNTS = ("jobs", "sd_clamped")
+
+
+def _sdclass_numbers(rec):
+    """the SLOWDOWN_METRICS of one SDCLASS_DTYPE record as a dict of floats (NaN for an empty class; std NaN below two
+    jobs).  The slowdown numbers are in units of slowdown; mean and sample variance are exact in Python ints and
+    rounded once (the division by 1024 is exact)."""
+    n = int(rec["jc"]["jobs"])
+    out = _jclass_numbers(rec["jc"])
+    s, sq = int(rec["sd_sum"]), u128(rec["sd_sq_lo"], rec["sd_sq_hi"])
+    out["key_mean"] = u128(rec["key_sum_lo"], rec["key_sum_hi"]) / n if n else math.nan
+    out["sd_mean"] = s / (n * SLOWDOWN_ONE) if n else math.nan
+    out["sd_std"] = math.sqrt(float(Fraction(n * sq - s * s, n * (n - 1)))) / SLOWDOWN_ONE if n > 1 else math.nan
+    for q, v in zip(QUANTILES, rec["sd_q"].tolist()):
+        out[f"sd_p{q}"] = v / SLOWDOWN_ONE if n else math.nan
+    out["sd_min"] = int(rec["sd_min"]) / SLOWDOWN_ONE if n else math.nan
+    return out
+
+
+def _sd_rows(hist, ne, nsd):
+    """the (C, 4, ...) CDF count rows of a (C, 3 * (ne + 1) + nsd + 1) slowdown histogram: three of ne + 1, one of nsd + 1"""
+    nb = ne + 1
+    return [hist[:, m * nb:(m + 1) * nb] for m in range(3)] + [hist[:, 3 * nb:3 * nb + nsd + 1]]
+
+
+def slowdown_derived(recs, hist, edges, sd_edges):
+    """Per class of one replica: `recs` SDCLASS_DTYPE (C,), `hist` CDF counts (C, 3 * (E + 1) + Esd + 1), `edges` the E
+    edges of wait / turnaround / jct, `sd_edges` the Esd edges of sd (units of 1/1024).  Returns {"jobs", "sd_clamped":
+    int arrays (C,), metric: float array (C,) for every SLOWDOWN_METRICS entry, "<quantity>_cdf": float array (C, E)
+    (C, Esd for sd) = #(value <= edge) / jobs}; NaN for an empty class."""
+    recs, hist = np.asarray(recs), np.asarray(hist, dtype=np.int64)
+    ne, nsd = len(edges), len(sd_edges)
+    if recs.ndim != 1 or hist.shape != (len(recs), 3 * (ne + 1) + nsd + 1):
+        raise ValueError("slowdown_derived: expected recs (C,) and hist (C, 3 * (len(edges) + 1) + len(sd_edges) + 1)")
+    jobs = recs["jc"]["jobs"].astype(np.int64)
+    out = {"jobs": jobs, "sd_clamped": recs["sd_clamped"].astype(np.int64)}
+    nums = [_sdclass_numbers(rec) for rec in recs]
+    for name in SLOWDOWN_METRICS:
+        out[name] = np.array([d[name] for d in nums], dtype=np.float64)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        for m, rows, n_e in zip(SLOWDOWN_QUANTITIES, _sd_rows(hist, ne, nsd), (ne, ne, ne, nsd)):
+            cum = np.cumsum(rows, axis=1)[:, :n_e]
+            out[m + "_cdf"] = np.where(jobs[:, None] > 0, cum / np.where(jobs > 0, jobs, 1)[:, None], np.nan)
+    return out
+
+
+def slowdown_spread(recs, hist, edges, sd_edges, level=0.95):
+    """Spread per class across replicas: `recs` (replicas, C), `hist` (replicas, C, 3 * (E + 1) + Esd + 1).  For every
+    class, over the replicas that have at least one job in it: {"replicas": int array (C,), metric: {mean, std, lo, hi:
+    float arrays (C,)} for every SLOWDOWN_METRICS entry, "<quantity>_cdf": {mean, std, lo, hi: float arrays (C, E)
+    (C, Esd for sd)}}, with spread's rules (sample std, nearest-rank interval holding the central `level`, NaN where a
+    value is NaN for any of those replicas or no replica has jobs in the class)."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    recs, hist = np.asarray(recs), np.asarray(hist)
+    if recs.ndim != 2 or hist.shape != recs.shape + (3 * (len(edges) + 1) + len(sd_edges) + 1,):
+        raise ValueError("slowdown_spread: expected recs (replicas, C) and hist (replicas, C, 3 * (len(edges) + 1) + len(sd_edges) + 1)")
+    per = [slowdown_derived(recs[r], hist[r], edges, sd_edges) for r in range(recs.shape[0])]
+    nc = recs.shape[1]
+    reach = recs["jc"]["jobs"] > 0
+    out = {"replicas": reach.sum(axis=0).astype(np.int64)}
+    for name in SLOWDOWN_METRICS:
+        cols = [_spread_of(np.array([d[name][c] for r, d in enumerate(per) if reach[r, c]], dtype=np.float64), level) for c in range(nc)]
+        out[name] = {s: np.array([col[s] for col in cols], dtype=np.float64) for s in SPREAD_STATS}
+    for m, ne in zip(SLOWDOWN_QUANTITIES, (len(edges),) * 3 + (len(sd_edges),)):
+        st = {s: np.full((nc, ne), math.nan) for s in SPREAD_STATS}
+        cdf = np.stack([d[m + "_cdf"] for d in per]) if per else np.zeros((0, nc, ne))
+        for c in range(nc):
+            sub = cdf[reach[:, c], c, :]
+            for e in range(ne):
+                sp = _spread_of(sub[:, e], level)
+                for s in SPREAD_STATS:
+                    st[s][c, e] = sp[s]
+        out[m + "_cdf"] = st
+    return out
+
+
+def slowdown_columns():
+    """names of the flat per-class columns `slowdown_flat` returns, in order"""
+    return list(SLOWDOWN_COUNTS) + list(SLOWDOWN_METRICS)
+
+
+def slowdown_flat(d, c):
+    """class c of a slowdown_derived dict as a list of Python values"""
+    return [int(d[k][c]) for k in SLOWDOWN_COUNTS] + [float(d[name][c]) for name in SLOWDOWN_METRICS]
+
+
+def slowdown_spread_columns():
+    return [f"{name}_{s}" for name in SLOWDOWN_METRICS for s in SPREAD_STATS]
+
+
+def slowdown_spread_flat(sp, c):
+    return [float(sp[name][s][c]) for name in SLOWDOWN_METRICS for s in SPREAD_STATS]
 
 
 # ---------------------------------------------------------------- paired comparisons of two configurations

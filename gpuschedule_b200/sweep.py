@@ -197,6 +197,40 @@ def check_jobdist(jobdist):
     return tuple(bounds), tuple(edges)
 
 
+DEFAULT_SD_EDGES = tuple(1024 * 2 ** i for i in range(21))      # slowdown 1, 2, 4, ... 2^20 in units of 1/1024
+
+
+def check_slowdown(slowdown):
+    """(key, class bounds, tau, CDF edges, sd CDF edges) of a slowdown argument, the sequences as tuples of ints, or
+    ValueError: key one of capi.JKEYS; at most 7 bounds, each >= 1, int64 and strictly increasing; tau >= 1 and int64;
+    at most 255 edges and 255 sd edges (units of 1/1024), each list int32 and strictly increasing"""
+    try:
+        key, bounds, tau, edges, sd_edges = slowdown
+        bounds, edges, sd_edges = ([int(x) for x in seq] for seq in (bounds, edges, sd_edges))
+        tau = int(tau)
+    except (TypeError, ValueError):
+        raise ValueError("slowdown: expected (key, class bounds, tau, CDF edges, sd CDF edges)") from None
+    if key not in capi.JKEYS:
+        raise ValueError(f"slowdown: the key must be one of {', '.join(capi.JKEYS)}")
+    if len(bounds) > capi.JOBDIST_MAX_CLASSES - 1:
+        raise ValueError(f"slowdown: at most {capi.JOBDIST_MAX_CLASSES - 1} class bounds")
+    if any(b < 1 or b >= 2 ** 63 for b in bounds) or any(b <= a for a, b in zip(bounds, bounds[1:])):
+        raise ValueError("slowdown: the class bounds must be >= 1, int64 and strictly increasing")
+    if not 1 <= tau < 2 ** 63:
+        raise ValueError("slowdown: tau must be >= 1 and int64")
+    for name, seq, cap in (("CDF edges", edges, capi.JOBDIST_MAX_EDGES), ("sd CDF edges", sd_edges, capi.SLOWDOWN_MAX_EDGES)):
+        if len(seq) > cap:
+            raise ValueError(f"slowdown: at most {cap} {name}")
+        if any(not -2 ** 31 <= e < 2 ** 31 for e in seq) or any(b <= a for a, b in zip(seq, seq[1:])):
+            raise ValueError(f"slowdown: the {name} must be int32 and strictly increasing")
+    return key, tuple(bounds), tau, tuple(edges), tuple(sd_edges)
+
+
+def _sd_row(sd):
+    """uint32 CDF counts per (replica, class) of a checked slowdown setting"""
+    return 3 * (len(sd[3]) + 1) + len(sd[4]) + 1
+
+
 DEFAULT_DIFF_EDGES = tuple(-2 ** i for i in range(30, -1, -1)) + (0,) + tuple(2 ** i for i in range(31))
 
 
@@ -231,7 +265,7 @@ def _compare_in(eng, pairs, members, bounds, edges):
     return eng.compare([pos[a] for a, _ in pairs], [pos[b] for _, b in pairs], bounds, edges)
 
 
-def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None, compare=None):
+def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None, compare=None, slowdown=None):
     """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
     same configurations and random streams as run_batched, but no row or job record is read back and nothing is
     written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus.
@@ -241,7 +275,15 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
     and append (JCLASS_DTYPE records (len(flag_sets), C), CDF counts (len(flag_sets), C, 3, E + 1)) to the result.
     compare=(pairs, bounds, edges): also compare every pair (a, b) of configuration indices job by job on the device
     (gs_compare, after the runs) and append (JPAIR_DTYPE records (len(pairs), C), CDF counts of d (len(pairs), C, 3,
-    E + 1)) as the last element; both configurations of a pair must share a trace file and an engine."""
+    E + 1)) as the last element; both configurations of a pair must share a trace file and an engine.
+    slowdown=(key, bounds, tau, edges, sd_edges): also compute every replica's job statistics by key with bounded
+    slowdown on the device (gs_set_slowdown) and append (SDCLASS_DTYPE records (len(flag_sets), C), CDF counts
+    (len(flag_sets), C, 3 * (E + 1) + Esd + 1)) after the jobdist element (before the compare element)."""
+    if slowdown is not None:
+        sd = check_slowdown(slowdown)
+        sd_nc = len(sd[1]) + 1
+        sd_recs = np.zeros((len(flag_sets), sd_nc), dtype=capi.SDCLASS_DTYPE)
+        sd_hist = np.zeros((len(flag_sets), sd_nc, _sd_row(sd)), dtype=np.uint32)
     if compare is not None:
         pairs, cmp_bounds, cmp_edges = check_compare(compare, flag_sets)
         cmp_recs = np.zeros((len(pairs), len(cmp_bounds) + 1), dtype=capi.JPAIR_DTYPE)
@@ -265,11 +307,15 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 eng.set_timeline(W, B)
             if jobdist is not None:
                 eng.set_jobdist(jd_bounds, jd_edges)
+            if slowdown is not None:
+                eng.set_slowdown(*sd)
             out[aware] = eng.summarize()
             if timeline is not None:
                 bins[aware] = eng.timeline()
             if jobdist is not None:
                 jd_cls[aware], jd_hist[aware] = eng.jobdist()
+            if slowdown is not None:
+                sd_recs[aware], sd_hist[aware] = eng.slowdown()
             sel = [k for k, (a, _) in enumerate(pairs) if a in set(aware)] if compare is not None else []
             if sel:
                 cmp_recs[sel], cmp_hist[sel] = _compare_in(eng, [pairs[k] for k in sel], aware, cmp_bounds, cmp_edges)
@@ -281,16 +327,20 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 eng.set_timeline(W, B)
             if jobdist is not None:
                 eng.set_jobdist(jd_bounds, jd_edges)
+            if slowdown is not None:
+                eng.set_slowdown(*sd)
             out[plain] = eng.run_summarized()
             if timeline is not None:
                 bins[plain] = eng.timeline()
             if jobdist is not None:
                 jd_cls[plain], jd_hist[plain] = eng.jobdist()
+            if slowdown is not None:
+                sd_recs[plain], sd_hist[plain] = eng.slowdown()
             sel = [k for k, (a, _) in enumerate(pairs) if a in set(plain)] if compare is not None else []
             if sel:
                 cmp_recs[sel], cmp_hist[sel] = _compare_in(eng, [pairs[k] for k in sel], plain, cmp_bounds, cmp_edges)
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
-           + (((cmp_recs, cmp_hist),) if compare is not None else ()))
+           + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -355,7 +405,7 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1, mix=None):
 
 
 def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1,
-                        compare=None, mix=None):
+                        compare=None, mix=None, slowdown=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -381,8 +431,13 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     Every returned array gains a mix axis right after the loads axis, (configurations, loads, mixes, replicas, ...),
     and compare pairs (a, L, mix, r) with (b, L, mix, r).  A mix whose weights sum to 0 on a base trace is a
     ValueError, raised before any engine is created.  A gittins replica still takes its index table from the base
-    trace: the policy is not told about the shift.  With L > 1, only block starts are drawn from the mix."""
+    trace: the policy is not told about the shift.  With L > 1, only block starts are drawn from the mix.
+    slowdown=(key, bounds, tau, edges, sd_edges): also append (SDCLASS_DTYPE records (..., C), CDF counts (..., C,
+    3 * (E + 1) + Esd + 1)) with the replicas' leading axes, after the jobdist element (before the compare element)."""
     _check_bootstrap_args(flag_sets, replicas, loads, n, block_len, mix)
+    if slowdown is not None:
+        sd = check_slowdown(slowdown)
+        sd_nc, sd_row = len(sd[1]) + 1, _sd_row(sd)
     if mix is not None:
         mix_bounds, mix_mults = check_mix(mix)
     if compare is not None:
@@ -403,6 +458,9 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     if jobdist is not None:
         jd_cls = np.zeros((len(flag_sets),) + lead + (nc,), dtype=capi.JCLASS_DTYPE)
         jd_hist = np.zeros((len(flag_sets),) + lead + (nc, 3, nb), dtype=np.uint32)
+    if slowdown is not None:
+        sd_recs = np.zeros((len(flag_sets),) + lead + (sd_nc,), dtype=capi.SDCLASS_DTYPE)
+        sd_hist = np.zeros((len(flag_sets),) + lead + (sd_nc, sd_row), dtype=np.uint32)
     if compare is not None:
         cmp_nc, cmp_nb = len(cmp_bounds) + 1, len(cmp_edges) + 1
         cmp_recs = np.zeros((len(pairs),) + lead + (cmp_nc,), dtype=capi.JPAIR_DTYPE)
@@ -447,9 +505,12 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
                 eng.set_timeline(W, B)
             if jobdist is not None:
                 eng.set_jobdist(jd_bounds, jd_edges)
+            if slowdown is not None:
+                eng.set_slowdown(*sd)
             recs = eng.run_summarized()
             tl = eng.timeline() if timeline is not None else None
             jd = eng.jobdist() if jobdist is not None else None
+            sdr = eng.slowdown() if slowdown is not None else None
             sel = [k for k, (a, _) in enumerate(pairs) if a in set(configs)] if compare is not None else []
             if sel:
                 pos = {c: k for k, c in enumerate(configs)}
@@ -467,8 +528,11 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
             if jd is not None:
                 jd_cls[c] = jd[0][part].reshape(lead + (nc,))
                 jd_hist[c] = jd[1][part].reshape(lead + (nc, 3, nb))
+            if sdr is not None:
+                sd_recs[c] = sdr[0][part].reshape(lead + (sd_nc,))
+                sd_hist[c] = sdr[1][part].reshape(lead + (sd_nc, sd_row))
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
-           + (((cmp_recs, cmp_hist),) if compare is not None else ()))
+           + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -634,6 +698,70 @@ def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edge
                                        + [float(sp[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS])
 
 
+def _sd_keys(fl, sd, c, lk=()):
+    """the flags, the load columns lk (bootstrap files), the key, the class, its key range and tau of a slowdown line"""
+    key, bounds, tau = sd[0], sd[1], sd[2]
+    return [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + list(lk) + [key, c] + _class_range(c, bounds) + [tau]
+
+
+def _sd_edges_of(sd):
+    """per SLOWDOWN_QUANTITIES entry, the edges in the quantity's own unit (ticks; slowdown for sd)"""
+    return [sd[3]] * 3 + [[e / summary.SLOWDOWN_ONE for e in sd[4]]]
+
+
+def write_slowdown_csv(path, flag_sets, recs, hist, sd):
+    """one line per (configuration, class): the flags, the key, the class, its key range, tau and
+    summary.slowdown_derived's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["key", "class", "key_min", "key_max", "tau"] + summary.slowdown_columns())
+        for fl, rc, hs in zip(flag_sets, recs, hist):
+            d = summary.slowdown_derived(rc, hs, sd[3], sd[4])
+            for c in range(len(rc)):
+                w.writerow(_sd_keys(fl, sd, c) + summary.slowdown_flat(d, c))
+
+
+def write_slowdown_ci_csv(path, flag_sets, loads, recs, hist, sd, level=0.95, block_len=None, mix=None):
+    """one line per (configuration, load[, block_len][, mix], class): the flags, the load, block_len (with a block
+    length), mix (with job mixes), the key, the class, its key range, tau, the replicas with jobs in the class and
+    summary.slowdown_spread's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["key", "class", "key_min", "key_max", "tau"]
+                   + ["replicas", "level"] + summary.slowdown_spread_columns())
+        for fl, per_rc, per_hs in zip(flag_sets, recs, hist):
+            for (keys, rc), (_, hs) in zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)):
+                sp = summary.slowdown_spread(rc, hs, sd[3], sd[4], level=level)
+                for c in range(rc.shape[1]):
+                    w.writerow(_sd_keys(fl, sd, c, keys) + [int(sp["replicas"][c]), level] + summary.slowdown_spread_flat(sp, c))
+
+
+def write_slowdown_cdf_csv(path, flag_sets, recs, hist, sd, loads=None, level=0.95, block_len=None, mix=None):
+    """one line per (configuration[, load[, block_len][, mix]], class, quantity, edge): the flags[, the load, block_len,
+    mix], the key, the class, its key range, tau, the quantity (wait, turnaround, jct in ticks; sd in units of slowdown),
+    the edge in that unit and the fraction of the class's jobs with a value <= the edge (with loads: the replicas with
+    jobs in the class and the spread of that fraction)"""
+    import csv
+    boot = loads is not None
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["key", "class", "key_min", "key_max", "tau"]
+                   + ["quantity", "edge"] + (["replicas", "level"] + [f"cdf_{s}" for s in summary.SPREAD_STATS] if boot else ["jobs", "cdf"]))
+        for fl, per_rc, per_hs in zip(flag_sets, recs, hist):
+            lines = (zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)) if boot
+                     else [(([], per_rc), ([], per_hs))])
+            for (lk, rc), (_, hs) in lines:
+                d = summary.slowdown_spread(rc, hs, sd[3], sd[4], level=level) if boot else summary.slowdown_derived(rc, hs, sd[3], sd[4])
+                for c in range(rc.shape[-1]):
+                    for m, edges in zip(summary.SLOWDOWN_QUANTITIES, _sd_edges_of(sd)):
+                        for e, edge in enumerate(edges):
+                            tail = ([int(d["replicas"][c]), level] + [float(d[m + "_cdf"][s][c, e]) for s in summary.SPREAD_STATS] if boot
+                                    else [int(d["jobs"][c]), float(d[m + "_cdf"][c, e])])
+                            w.writerow(_sd_keys(fl, sd, c, lk) + [m, edge] + tail)
+
+
 def _pair_keys(fl, base):
     return [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, base.schedule]
 
@@ -793,7 +921,38 @@ def main(argv=None):
     ap.add_argument("--paired-summary", default=None, metavar="FILE",
                     help="with --compare: one CSV line per configuration (with --bootstrap: per configuration and load) with the "
                          "replica-level differences from BASE of the makespan and of every derived number")
+    ap.add_argument("--slowdown", default=None, metavar="FILE",
+                    help="with --summary: also compute job statistics by --job-key classes with bounded slowdown on the GPU and "
+                         "write one CSV line per (configuration, class) to FILE; with --bootstrap one line per (configuration, "
+                         "load, class) with the spread across replicas")
+    ap.add_argument("--job-key", choices=tuple(capi.JKEYS), default=None,
+                    help="with --slowdown: the class key, num_gpu, the run length jct or gpus * jct (default length)")
+    ap.add_argument("--key-classes", type=int, nargs="+", default=None, metavar="B",
+                    help="with --slowdown: class bounds B1 < ... < Bk (a job's class is the number of bounds <= its key; at most "
+                         f"{capi.JOBDIST_MAX_CLASSES - 1}); default: one class")
+    ap.add_argument("--slowdown-bound", type=int, default=None, metavar="TAU",
+                    help="with --slowdown: bounded slowdown turnaround / max(jct, TAU), TAU >= 1 in ticks (default 1: plain slowdown)")
+    ap.add_argument("--slowdown-cdf", default=None, metavar="FILE",
+                    help="with --slowdown: one CSV line per (configuration[, load], class, quantity, edge) with the CDF value or its "
+                         "spread; wait / turnaround / jct at --cdf-edges, slowdown at --sd-edges")
+    ap.add_argument("--sd-edges", type=int, nargs="+", default=None, metavar="E",
+                    help=f"with --slowdown: CDF edges of the slowdown in units of 1/1024 (strictly increasing, at most "
+                         f"{capi.SLOWDOWN_MAX_EDGES}; default 1024 * 2^i for i = 0 ... 20)")
     a = ap.parse_args(argv)
+    slowdown = None
+    if a.slowdown is not None:
+        if not a.summary:
+            ap.error("--slowdown needs --summary FILE")
+        try:
+            slowdown = check_slowdown(("length" if a.job_key is None else a.job_key, a.key_classes or (),
+                                       1 if a.slowdown_bound is None else a.slowdown_bound,
+                                       DEFAULT_CDF_EDGES if a.cdf_edges is None else a.cdf_edges,
+                                       DEFAULT_SD_EDGES if a.sd_edges is None else a.sd_edges))
+        except ValueError as e:
+            ap.error(str(e))
+    elif (a.job_key is not None or a.key_classes is not None or a.slowdown_bound is not None or a.slowdown_cdf is not None
+          or a.sd_edges is not None):
+        ap.error("--job-key, --key-classes, --slowdown-bound, --slowdown-cdf and --sd-edges need --slowdown FILE")
     jobdist = None
     if a.jobdist is not None:
         if not a.summary:
@@ -802,8 +961,10 @@ def main(argv=None):
             jobdist = check_jobdist((a.gpu_classes or (), DEFAULT_CDF_EDGES if a.cdf_edges is None else a.cdf_edges))
         except ValueError as e:
             ap.error(str(e))
-    elif a.cdf_edges is not None or a.jobdist_cdf is not None or (a.gpu_classes is not None and a.paired is None):
-        ap.error("--gpu-classes, --cdf-edges and --jobdist-cdf need --jobdist FILE (--gpu-classes: or --paired FILE)")
+    elif ((a.cdf_edges is not None and a.slowdown is None) or a.jobdist_cdf is not None
+          or (a.gpu_classes is not None and a.paired is None)):
+        ap.error("--gpu-classes, --cdf-edges and --jobdist-cdf need --jobdist FILE (--gpu-classes: or --paired FILE; "
+                 "--cdf-edges: or --slowdown FILE)")
     if a.compare is None:
         if a.paired is not None or a.paired_cdf is not None or a.diff_edges is not None or a.paired_summary is not None:
             ap.error("--paired, --paired-cdf, --diff-edges and --paired-summary need --compare BASE")
@@ -877,8 +1038,8 @@ def main(argv=None):
             ap.error(str(e))
         bl = a.block_len
         res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist,
-                                  block_len=1 if bl is None else bl, compare=compare, mix=mix)
-        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None else (res[0], res[1:])
+                                  block_len=1 if bl is None else bl, compare=compare, mix=mix, slowdown=slowdown)
+        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None and slowdown is None else (res[0], res[1:])
         if compare is not None:
             pairs, cmp_bounds, cmp_edges = compare
             prec, phist = rest[-1]
@@ -889,6 +1050,12 @@ def main(argv=None):
                 write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges, loads=loads, block_len=bl, mix=mix_text)
             if a.paired_summary:
                 write_paired_summary_csv(a.paired_summary, sets, pairs, recs, loads=loads, block_len=bl, mix=mix_text)
+        if slowdown is not None:
+            srec, shist = rest[-1]
+            rest = rest[:-1]
+            write_slowdown_ci_csv(a.slowdown, sets, loads, srec, shist, slowdown, block_len=bl, mix=mix_text)
+            if a.slowdown_cdf:
+                write_slowdown_cdf_csv(a.slowdown_cdf, sets, srec, shist, slowdown, loads=loads, block_len=bl, mix=mix_text)
         if timeline is not None:
             write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0], block_len=bl, mix=mix_text)
         if jobdist is not None:
@@ -903,8 +1070,8 @@ def main(argv=None):
               + (f" x {len(mix_text)} mixes" if mix_text else "") + f" x {a.bootstrap} replicas")
         return
     if a.summary:
-        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare)
-        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None else (res[0], res[1:])
+        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare, slowdown=slowdown)
+        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None and slowdown is None else (res[0], res[1:])
         if compare is not None:
             pairs, cmp_bounds, cmp_edges = compare
             prec, phist = rest[-1]
@@ -915,6 +1082,12 @@ def main(argv=None):
                 write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges)
             if a.paired_summary:
                 write_paired_summary_csv(a.paired_summary, sets, pairs, recs)
+        if slowdown is not None:
+            srec, shist = rest[-1]
+            rest = rest[:-1]
+            write_slowdown_csv(a.slowdown, sets, srec, shist, slowdown)
+            if a.slowdown_cdf:
+                write_slowdown_cdf_csv(a.slowdown_cdf, sets, srec, shist, slowdown)
         if timeline is not None:
             write_timeline_csv(a.timeline, sets, rest[0], timeline[0])
         if jobdist is not None:

@@ -453,6 +453,61 @@ typedef struct gs_jclass {
 int gs_set_jobdist(gs_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges);
 int gs_fetch_jobdist(gs_handle h, int first, int count, gs_jclass *classes_out, uint32_t *hist_out);
 
+/* ---- job statistics by a chosen key, with bounded slowdown (slowdown) ------------------------------------------
+ * The jobs are jobdist's: the finished jobs of gs_summary's job part with arrive, start, end, jct and gpus, wait =
+ * start - arrive and turnaround = end - arrive.  jct is the job's run length in ticks: max(1, ceil(duration)) in the
+ * fifo and policy engines, the largest time_processed of the job's tasks in the horus engine.
+ * Key of a job, chosen per setting: GS_JKEY_GPUS: gpus (jobdist's key); GS_JKEY_LENGTH: jct; GS_JKEY_GPU_TIME:
+ * gpus * jct (int64).  C classes (1 <= C <= GS_JOBDIST_MAX_CLASSES) from C - 1 strictly increasing int64 bounds, each
+ * >= 1: a job's class is the number of bounds <= its key.
+ * Bounded slowdown of a job, in fixed point (units of 1/1024), for an integer tau >= 1:
+ *     sd = min(2^31 - 1, max(1024, floor(1024 * turnaround / max(jct, tau))))
+ * computed in 64-bit integer arithmetic (no floating point).  tau = 1 gives plain slowdown, turnaround / jct.  The
+ * value saturates at 2^31 - 1, a slowdown of about 2.1 million; sd_clamped counts the class's jobs whose sd is that
+ * value.  Per class one gs_sdclass: `jc` is the class's gs_jclass with jobdist's meaning field for field (with
+ * key = gpus and jobdist's bounds it is byte-equal to gs_fetch_jobdist's), then the same statistics of sd, and the
+ * exact sum of the class's keys.
+ * CDF histograms: wait, turnaround and jct at E strictly increasing int32 edges (0 <= E <= GS_JOBDIST_MAX_EDGES,
+ * jobdist's edges and rule: value v in bin #{i : e_i < v}); sd at its own Esd strictly increasing int32 edges
+ * (0 <= Esd <= GS_SLOWDOWN_MAX_EDGES, in units of 1/1024, the same rule).  Layout per replica
+ * [class][wait, turnaround, jct, sd][bin]: per class 3 * (E + 1) + (Esd + 1) uint32 counts, the rows of wait,
+ * turnaround and jct E + 1 long each, then the sd row Esd + 1 long.  Every field is an integer; a repeated call gives
+ * the same bytes.                                                                                              */
+#define GS_JKEY_GPUS 0
+#define GS_JKEY_LENGTH 1
+#define GS_JKEY_GPU_TIME 2
+#define GS_SLOWDOWN_MAX_EDGES 255
+typedef struct gs_sdclass {
+  gs_jclass jc;                      /* the class's jobdist record                                                   */
+  int64_t sd_sum;                    /* sum of sd (units of 1/1024)                                                  */
+  uint64_t sd_sq_lo, sd_sq_hi;       /* exact 128-bit sum of sd^2                                                    */
+  int32_t sd_q[5];                   /* 50 / 90 / 95 / 99 / 100 %, gs_summary's rank rule; 0 for an empty class      */
+  int32_t sd_min;                    /* smallest sd; 0 for an empty class                                            */
+  int64_t sd_clamped;                /* jobs with sd = 2^31 - 1                                                      */
+  uint64_t key_sum_lo, key_sum_hi;   /* exact 128-bit sum of the keys (gpus * jct < 2^55 per job)                    */
+} gs_sdclass;                        /* 232 bytes */
+typedef struct gs_slowdown_cfg {
+  int32_t key;                       /* GS_JKEY_*                                                                   */
+  int32_t nclasses;                  /* 0: off; 1..GS_JOBDIST_MAX_CLASSES                                           */
+  int64_t bounds[GS_JOBDIST_MAX_CLASSES - 1];   /* the first nclasses - 1 are used                                 */
+  int64_t tau;                       /* >= 1, ticks                                                                 */
+  int32_t nedges, nsd_edges;         /* E, Esd                                                                      */
+  const int32_t *edges;              /* E edges of wait, turnaround and jct (may be NULL when E = 0)                */
+  const int32_t *sd_edges;           /* Esd edges of sd (may be NULL when Esd = 0)                                  */
+} gs_slowdown_cfg;
+/* gs_set_slowdown: while cfg->nclasses > 0, every gs_summarize also computes the class records and CDF histograms of
+ * the replicas it summarises (the job part is recomputed in full on every call, so this may be called at any time);
+ * cfg == NULL or nclasses = 0 (the default) turns it off.  Every replica is marked as not summarised with this
+ * setting.  Jobdist and slowdown may both be on; each keeps its own arrays and state.  GS_ERR_ARG for a key other than
+ * GS_JKEY_*, nclasses outside 0..8, bounds that are not strictly increasing or below 1, tau < 1, E or Esd outside
+ * 0..255, edges that are not strictly increasing, or a NULL array with a positive count; nothing changes on an error.
+ * gs_fetch_slowdown copies count * C records and count * C * (3 * (E + 1) + Esd + 1) counts (replica-major; either
+ * output may be NULL) as of the last gs_summarize (synchronous).  GS_ERR_ARG for a bad range, GS_ERR_STATE when the
+ * feature is off or a replica has not been summarised since it was prepared (first gs_run, gs_reset, a new trace,
+ * gs_boot_traces) or since the last gs_set_slowdown.                                                         */
+int gs_set_slowdown(gs_handle h, const gs_slowdown_cfg *cfg);
+int gs_fetch_slowdown(gs_handle h, int first, int count, gs_sdclass *out, uint32_t *hist_out);
+
 /* ---- paired per-job comparison of two replicas on the same trace ------------------------------------------
  * A pair (a, b) is two replicas of one handle that hold the same trace: the same job count n and, for every j < n,
  * a byte-equal gs_jobin record (gs_horus_compare: equal fields as taken by gs_horus_load_trace).  They may differ in

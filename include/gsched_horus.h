@@ -108,6 +108,10 @@ int gs_horus_fetch_timeline(gs_horus_handle h, int32_t first, int32_t count, gs_
  * finished jobs as its job part.  Same meaning and errors as gs_set_jobdist / gs_fetch_jobdist.                 */
 int gs_horus_set_jobdist(gs_horus_handle h, int32_t nclasses, const int32_t *bounds, int32_t nedges, const int32_t *edges);
 int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t count, gs_jclass *classes_out, uint32_t *hist_out);
+/* Job statistics by a chosen key with bounded slowdown (gs_sdclass and CDF histograms, gsched.h) filled by
+ * gs_horus_summarize from the same finished jobs.  Same meaning and errors as gs_set_slowdown / gs_fetch_slowdown. */
+int gs_horus_set_slowdown(gs_horus_handle h, const gs_slowdown_cfg *cfg);
+int gs_horus_fetch_slowdown(gs_horus_handle h, int32_t first, int32_t count, gs_sdclass *out, uint32_t *hist_out);
 /* Paired per-job comparison (gs_jpair, gsched.h: gs_compare) of replicas of this handle that hold the same trace: equal
  * arrival, gpus, gpu_per_container, duration, memory, utilisation and mean-memory fields for every job.  The same
  * outputs, launches and errors as gs_compare; a replica has run once gs_horus_run has prepared it.           */
