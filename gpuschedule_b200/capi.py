@@ -106,6 +106,15 @@ JKEYS = {"gpus": 0, "length": 1, "gpu-time": 2}           # GS_JKEY_GPUS, GS_JKE
 SLOWDOWN_MAX_EDGES = 255
 SLOWDOWN_ONE = 1024                                       # sd units per unit of slowdown
 SLOWDOWN_MAX = 2 ** 31 - 1                                # the saturated sd
+# gs_occ (include/gsched.h): a replica's rows weighed by the ticks they stand for -- rows weighed, T, the sums of
+# w * busy_gpus / running / queued, the ticks with a queue, the idle GPU-ticks while jobs wait, the maxima and M * G.
+# Histograms come separately as uint64 ticks: busy (replica, [all, waiting], total_gpus + 1), queue (replica, E + 1).
+OCC_DTYPE = np.dtype([("rows", "<i8"), ("ticks", "<i8"), ("busy_sum", "<i8"), ("running_sum", "<i8"), ("queued_sum", "<i8"),
+                      ("wait_ticks", "<i8"), ("idle_wait_sum", "<i8"), ("running_max", "<i4"), ("queued_max", "<i4"),
+                      ("total_gpus", "<i4"), ("reserved", "<i4")])
+assert OCC_DTYPE.itemsize == 72
+OCC_MAX_EDGES = 255
+OCC_MAX_GPUS = 65535
 
 
 class GsSlowdownCfg(C.Structure):
@@ -233,6 +242,9 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_set_slowdown.argtypes = [C.c_void_p, C.c_void_p]
     lib.gs_horus_fetch_slowdown.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.gs_horus_set_slowdown.restype = lib.gs_horus_fetch_slowdown.restype = C.c_int
+    lib.gs_horus_set_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+    lib.gs_horus_fetch_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    lib.gs_horus_set_occupancy.restype = lib.gs_horus_fetch_occupancy.restype = C.c_int
     for name in ("gs_horus_summarize", "gs_horus_set_timeline", "gs_horus_fetch_timeline", "gs_horus_set_jobdist", "gs_horus_fetch_jobdist", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
                  "gs_horus_run", "gs_horus_stats", "gs_horus_fetch"):
         getattr(lib, name).restype = C.c_int
@@ -307,6 +319,9 @@ def load_library():
     lib.gs_set_slowdown.argtypes = [C.c_void_p, C.c_void_p]
     lib.gs_fetch_slowdown.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.gs_set_slowdown.restype = lib.gs_fetch_slowdown.restype = C.c_int
+    lib.gs_set_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+    lib.gs_fetch_occupancy.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    lib.gs_set_occupancy.restype = lib.gs_fetch_occupancy.restype = C.c_int
     for name in ("gs_load_traces_packed", "gs_result_layout", "gs_fetch_results", "gs_summarize", "gs_boot_population", "gs_boot_traces",
                  "gs_boot_traces_blocked", "gs_boot_mixes", "gs_boot_traces_mixed", "gs_fetch_trace", "gs_set_timeline", "gs_fetch_timeline", "gs_set_jobdist", "gs_fetch_jobdist"):
         getattr(lib, name).restype = C.c_int
@@ -560,6 +575,16 @@ class HorusEngine:
         summarize()"""
         return _fetch_slowdown(self, self.lib.gs_horus_fetch_slowdown, "gs_horus_fetch_slowdown", first, count)
 
+    def set_occupancy(self, queue_edges=None):
+        """time-weighted occupancy filled by every summarize(), with queue-length CDF counts at `queue_edges`;
+        None turns it off (include/gsched_horus.h: gs_horus_set_occupancy)"""
+        _set_occupancy(self, self.lib.gs_horus_set_occupancy, "gs_horus_set_occupancy", queue_edges)
+
+    def occupancy(self, first=0, count=None):
+        """(OCC_DTYPE records (count,), uint64 busy histograms (count, 2, max total_gpus + 1): all time, waiting time,
+        uint64 queue histograms (count, E + 1)) as of the last summarize()"""
+        return _fetch_occupancy(self, self.lib.gs_horus_fetch_occupancy, "gs_horus_fetch_occupancy", first, count)
+
     def compare(self, a, b, bounds=(), edges=(), with_time=False):
         """paired per-job comparison of replicas b[i] against a[i] on the same trace (include/gsched_horus.h:
         gs_horus_compare): (JPAIR_DTYPE records (P, C), uint32 CDF counts of d (P, C, 3, E + 1)); with_time: and the
@@ -631,6 +656,31 @@ def _fetch_slowdown(eng, fn, what, first, count):
     hist = np.zeros((max(count, 1), max(nc, 1), max(row, 1)), dtype=np.uint32)
     eng._check(fn(eng.h, int(first), count, recs.ctypes.data_as(C.c_void_p), hist.ctypes.data_as(C.c_void_p)), what)
     return recs[:count, :nc], hist[:count, :nc, :row]
+
+
+def _set_occupancy(eng, fn, what, queue_edges):
+    if queue_edges is None:
+        eng._check(fn(eng.h, 0, 0, None), what)
+        eng._occ_edges = 0
+        return
+    e = np.asarray(queue_edges, dtype=np.int64).reshape(-1)
+    if e.size and (e.min() < -2 ** 31 or e.max() >= 2 ** 31):
+        raise GsError(f"{what}: queue edges must be int32", GS_ERR_ARG)
+    e = np.ascontiguousarray(e, dtype=np.int32)
+    eng._check(fn(eng.h, 1, len(e), e.ctypes.data_as(C.c_void_p) if len(e) else None), what)
+    eng._occ_edges = len(e)
+
+
+def _fetch_occupancy(eng, fn, what, first, count):
+    count = eng.nsims - first if count is None else int(count)
+    E = getattr(eng, "_occ_edges", 0)
+    recs = np.zeros(max(count, 1), dtype=OCC_DTYPE)
+    eng._check(fn(eng.h, int(first), count, recs.ctypes.data_as(C.c_void_p), None, 0, None), what)
+    pitch = int(recs["total_gpus"][:count].max()) + 1 if count else 1
+    busy = np.zeros((max(count, 1), 2, pitch), dtype=np.uint64)
+    queue = np.zeros((max(count, 1), E + 1), dtype=np.uint64)
+    eng._check(fn(eng.h, int(first), count, None, busy.ctypes.data_as(C.c_void_p), pitch, queue.ctypes.data_as(C.c_void_p)), what)
+    return recs[:count], busy[:count], queue[:count]
 
 
 def _compare(eng, fn, what, a, b, bounds, edges, with_time):
@@ -1012,6 +1062,17 @@ class Engine:
         and jct rows of E + 1 counts, then the sd row of Esd + 1) of replicas [first, first+count) as of the last
         summarize()"""
         return _fetch_slowdown(self, self.lib.gs_fetch_slowdown, "gs_fetch_slowdown", first, count)
+
+    def set_occupancy(self, queue_edges=None):
+        """time-weighted occupancy filled by every summarize(): each row weighed by the ticks it stands for, busy-GPU
+        histograms over all time and over the ticks with a queue, queue-length CDF counts at `queue_edges`; None turns it
+        off.  Set it before the first summarize() of a run (include/gsched.h: gs_set_occupancy)"""
+        _set_occupancy(self, self.lib.gs_set_occupancy, "gs_set_occupancy", queue_edges)
+
+    def occupancy(self, first=0, count=None):
+        """(OCC_DTYPE records (count,), uint64 busy histograms (count, 2, max total_gpus + 1): all time, waiting time,
+        uint64 queue histograms (count, E + 1)) of replicas [first, first+count) as of the last summarize()"""
+        return _fetch_occupancy(self, self.lib.gs_fetch_occupancy, "gs_fetch_occupancy", first, count)
 
     def compare(self, a, b, bounds=(), edges=(), with_time=False):
         """paired per-job comparison of replicas b[i] against a[i], which hold the same trace, over the jobs finished so

@@ -72,6 +72,18 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_htl_rows_kernel(const HSim 
   gs_tl_fold_rows(bins + (size_t)r * (size_t)B, B, W, S.rows, S.util, 0, 0, S.ticks);
 }
 
+// Occupancy of gs_horus_summarize: the same rows [0, ticks), one tick each, into zeroed records and histograms.  The
+// shared counters are static here: a dynamic shared array in this file would round every kernel's static shared memory
+// up to 16 bytes.
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_occ_hsum(const HSim *sims, int first, GsOccCfg cfg, gs_occ *occ,
+                                                              unsigned long long *busy, long long pitch, unsigned long long *queue) {
+  __shared__ unsigned long long occ_sh[GS_OCC_SMEM_COUNTERS];
+  const int r = first + blockIdx.x;
+  const HSim &S = sims[r];
+  unsigned long long *hall = busy + (size_t)r * 2 * (size_t)pitch, *hq = queue + (size_t)r * (size_t)(cfg.nedges + 1);
+  gs_occ_fold(GS_OCC_PER_TICK, occ_sh, occ + r, nullptr, hall, hall + pitch, hq, cfg, S.M * S.G, nullptr, 0, 0, 0, S.rows, 0, 0, S.ticks, S.done);
+}
+
 #endif  // __CUDACC__
 
 // The trace fields gs_horus_load_trace takes of job j are equal in both jobs (doubles compared bit for bit).
@@ -112,6 +124,7 @@ struct HorusSimHost {
   bool tl_done = false;             // summarised with the timeline on since it was prepared
   bool jd_done = false;             // summarised with the current jobdist setting since it was prepared
   bool sd_done = false;             // summarised with the current slowdown setting since it was prepared
+  bool occ_done = false;            // summarised with the occupancy on since it was prepared
   gs_cluster cl{};
   gs_horus_params par{};
   std::vector<HJob> jobs;
@@ -144,6 +157,10 @@ struct gs_horus_handle_s {
   gs_sdclass *d_sd = nullptr; size_t sd_bytes = 0;      // gs_horus_set_slowdown: nsims x C class records
   unsigned *d_sd_hist = nullptr; size_t sd_hist_bytes = 0;   // and nsims x C x (3 (E + 1) + Esd + 1) CDF counts
   GsSdCfg sd{};                                          // sd.nclasses = 0: off
+  bool occ_on = false; GsOccCfg occ{};                   // gs_horus_set_occupancy
+  gs_occ *d_occ = nullptr;                               // nsims records
+  unsigned long long *d_occ_busy = nullptr; int64_t occ_pitch = 0;   // nsims x [H_all, H_wait] x occ_pitch counters
+  unsigned long long *d_occ_q = nullptr; size_t occ_q_bytes = 0;     // nsims x (E + 1) queue counters
   std::string err;
   std::vector<double> shared;       // one stream consumed by every replica that did not get its own
   double *d_shared = nullptr; size_t shared_cap = 0; bool shared_dirty = false;
@@ -197,6 +214,9 @@ extern "C" int gs_horus_destroy(gs_horus_handle h) {
   if (h->d_jd_hist) cudaFree(h->d_jd_hist);
   if (h->d_sd) cudaFree(h->d_sd);
   if (h->d_sd_hist) cudaFree(h->d_sd_hist);
+  if (h->d_occ) cudaFree(h->d_occ);
+  if (h->d_occ_busy) cudaFree(h->d_occ_busy);
+  if (h->d_occ_q) cudaFree(h->d_occ_q);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -386,7 +406,7 @@ static int prepare(gs_horus_handle h, HorusSimHost &s, long long rows_cap) {
   D.rows_cap = rows_cap;
   D.current_remaining = (long long)n; D.running_jobs = 0;
   s.rows_cap = rows_cap;
-  s.prepared = true; s.tl_done = false; s.jd_done = false; s.sd_done = false;
+  s.prepared = true; s.tl_done = false; s.jd_done = false; s.sd_done = false; s.occ_done = false;
   return GS_OK;
 }
 
@@ -486,8 +506,26 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   for (int i = first; i < first + count; ++i) {
     if (!h->sims[(size_t)i].prepared) return hfail(h, GS_ERR_STATE, "gs_horus_summarize: a replica has not run yet");
     kmax = std::max(kmax, (long long)h->sims[(size_t)i].dev.nfin);
+    if (h->occ_on && (int64_t)h->sims[(size_t)i].dev.M * h->sims[(size_t)i].dev.G > GS_OCC_MAX_GPUS)
+      return hfail(h, GS_ERR_ARG, "gs_horus_summarize: the occupancy statistics take clusters of at most 65535 GPUs");
   }
   HCU(cudaSetDevice(h->device));
+  if (h->occ_on) {        // the pitch of the busy histograms
+    int64_t need = 1;
+    for (int i = first; i < first + count; ++i) need = std::max(need, (int64_t)h->sims[(size_t)i].dev.M * h->sims[(size_t)i].dev.G + 1);
+    if (need > h->occ_pitch) {                             // every replica is folded again from zero: nothing to move
+      HCU(cudaStreamSynchronize(h->stream));
+      if (h->d_occ_busy) cudaFree(h->d_occ_busy);
+      h->d_occ_busy = nullptr; h->occ_pitch = 0;
+      for (auto &s : h->sims) s.occ_done = false;
+      HCU(cudaMalloc(&h->d_occ_busy, 16 * (size_t)need * h->sims.size()));
+      h->occ_pitch = need;
+    }
+    const size_t E1 = (size_t)h->occ.nedges + 1;
+    HCU(cudaMemsetAsync(h->d_occ + first, 0, sizeof(gs_occ) * (size_t)count, h->stream));
+    HCU(cudaMemsetAsync(h->d_occ_busy + (size_t)first * 2 * (size_t)h->occ_pitch, 0, 16 * (size_t)h->occ_pitch * (size_t)count, h->stream));
+    HCU(cudaMemsetAsync(h->d_occ_q + (size_t)first * E1, 0, 8 * E1 * (size_t)count, h->stream));
+  }
   if (!h->d_sum) HCU(cudaMalloc(&h->d_sum, sizeof(gs_summary) * (size_t)nsims));
   HCU(cudaMemsetAsync(h->d_sum + first, 0, sizeof(gs_summary) * (size_t)count, h->stream));
   const int B = h->tl_nbins;
@@ -535,6 +573,12 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     HCU(cudaGetLastError());
     h->launches += 1;
   }
+  if (h->occ_on) {
+    gs_occ_hsum<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->occ, h->d_occ, h->d_occ_busy,
+                                                                                         (long long)h->occ_pitch, h->d_occ_q);
+    HCU(cudaGetLastError());
+    h->launches += 1;
+  }
   HCU(cudaEventRecord(h->ev1, h->stream));
 #else   // host build for tests/emu: the same folds, one replica after the other
   for (int r = first; r < first + count; ++r) {
@@ -555,6 +599,14 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     if (C > 0) gs_jd_jobs_serial(jobs.data(), S.nfin, h->jd, h->d_jd + (size_t)r * C, h->d_jd_hist + (size_t)r * C * 3 * (h->jd.nedges + 1));
     if (Csd > 0) gs_sd_serial(jobs.data(), S.nfin, h->sd, h->d_sd + (size_t)r * Csd, h->d_sd_hist + (size_t)r * Csd * gs_sd_row_len(h->sd));
     if (B > 0) gs_tl_fold_rows_serial(h->d_tl + (size_t)r * B, B, (long long)h->tl_width, S.rows, S.util, 0, 0, S.ticks);
+    if (h->occ_on) {
+      gs_occ &o = h->d_occ[r];
+      o.total_gpus = S.M * S.G;
+      unsigned long long *hall = h->d_occ_busy + (size_t)r * 2 * (size_t)h->occ_pitch;
+      const GsOccHist H{hall, hall + h->occ_pitch, h->d_occ_q + (size_t)r * (size_t)(h->occ.nedges + 1)};
+      GsOccCarry c{0, 0, 0, 0, 0};
+      gs_occ_serial(o, c, H, h->occ, S.rows, 0, 0, S.ticks, S.done, 1);
+    }
   }
   (void)kmax;
 #endif
@@ -569,6 +621,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     if (B > 0) h->sims[(size_t)i].tl_done = true;
     if (C > 0) h->sims[(size_t)i].jd_done = true;
     if (Csd > 0) h->sims[(size_t)i].sd_done = true;
+    if (h->occ_on) h->sims[(size_t)i].occ_done = true;
   }
   return GS_OK;
 }
@@ -695,6 +748,62 @@ extern "C" int gs_horus_fetch_slowdown(gs_horus_handle h, int32_t first, int32_t
     HCU(cudaMemcpyAsync(out, h->d_sd + (size_t)first * C, sizeof(gs_sdclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   if (hist_out)
     HCU(cudaMemcpyAsync(hist_out, h->d_sd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
+  return GS_OK;
+}
+
+extern "C" int gs_horus_set_occupancy(gs_horus_handle h, int32_t on, int32_t nedges, const int32_t *edges) {
+  if (!h) return GS_ERR_ARG;
+  GsOccCfg cfg{};
+  const char *why = nullptr;
+  if (on && !gs_occ_make_cfg(nedges, edges, cfg, &why)) return hfail(h, GS_ERR_ARG, std::string("gs_horus_set_occupancy: ") + why);
+  if (on) {
+    HCU(cudaSetDevice(h->device));
+    if (!h->d_occ) HCU(cudaMalloc(&h->d_occ, sizeof(gs_occ) * h->sims.size()));
+    const size_t need_q = 8 * h->sims.size() * (size_t)(cfg.nedges + 1);
+    if (need_q > h->occ_q_bytes) {
+      unsigned long long *d = nullptr;
+      HCU(cudaMalloc(&d, need_q));
+      if (h->d_occ_q) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_occ_q); }
+      h->d_occ_q = d; h->occ_q_bytes = need_q;
+    }
+  }
+  h->occ_on = on != 0;
+  h->occ = cfg;
+  for (auto &s : h->sims) s.occ_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_fetch_occupancy(gs_horus_handle h, int32_t first, int32_t count, gs_occ *out, uint64_t *busy_hist, int32_t busy_pitch,
+                                        uint64_t *queue_hist) {
+  if (!h) return GS_ERR_ARG;
+  const int nsims = (int)h->sims.size();
+  if (first < 0 || count < 0 || first > nsims - count) return hfail(h, GS_ERR_ARG, "gs_horus_fetch_occupancy: bad arguments");
+  if (!h->occ_on) return hfail(h, GS_ERR_STATE, "gs_horus_fetch_occupancy: the occupancy statistics are off (gs_horus_set_occupancy)");
+  int64_t width = 1;
+  for (int i = first; i < first + count; ++i) {
+    const HorusSimHost &s = h->sims[(size_t)i];
+    if (!s.prepared || !s.occ_done)
+      return hfail(h, GS_ERR_STATE, "gs_horus_fetch_occupancy: a replica has not been summarised with the occupancy on since it was prepared");
+    width = std::max(width, (int64_t)s.dev.M * s.dev.G + 1);
+  }
+  if (busy_hist && count > 0 && busy_pitch < width)
+    return hfail(h, GS_ERR_CAPACITY, "gs_horus_fetch_occupancy: busy_pitch is smaller than total_gpus + 1 of a fetched replica");
+  if (count == 0) return GS_OK;
+  HCU(cudaSetDevice(h->device));
+  if (out) HCU(cudaMemcpyAsync(out, h->d_occ + first, sizeof(gs_occ) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  if (busy_hist) {
+    const unsigned long long *src = h->d_occ_busy + (size_t)first * 2 * (size_t)h->occ_pitch;
+    const size_t w = 8 * (size_t)std::min(width, h->occ_pitch);
+#ifdef __CUDACC__
+    HCU(cudaMemcpy2DAsync(busy_hist, 8 * (size_t)busy_pitch, src, 8 * (size_t)h->occ_pitch, w, 2 * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+#else
+    for (size_t k = 0; k < 2 * (size_t)count; ++k)
+      HCU(cudaMemcpyAsync(busy_hist + k * (size_t)busy_pitch, src + k * (size_t)h->occ_pitch, w, cudaMemcpyDeviceToHost, h->stream));
+#endif
+  }
+  const size_t E1 = (size_t)h->occ.nedges + 1;
+  if (queue_hist) HCU(cudaMemcpyAsync(queue_hist, h->d_occ_q + (size_t)first * E1, 8 * E1 * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   HCU(cudaStreamSynchronize(h->stream));
   return GS_OK;
 }

@@ -354,6 +354,112 @@ static inline bool gs_sd_make_cfg(const gs_slowdown_cfg *in, GsSdCfg &cfg, const
 // uint32 counts per (replica, class): wait, turnaround and jct E + 1 each, then sd Esd + 1.
 GS_SUM_HD long long gs_sd_row_len(const GsSdCfg &cfg) { return 3ll * (cfg.nedges + 1) + cfg.nsd + 1; }
 
+// ---- time-weighted occupancy (gs_occ, include/gsched.h)
+static_assert(sizeof(gs_occ) == 72, "gs_occ is 72 bytes");
+#define GS_OCC_MAX_GPUS 65535
+#define GS_OCC_SMEM_COUNTERS 3072   // H_all and H_wait in shared memory when 2 * (G + 1) counters fit (24 KB)
+
+// The queue edges, passed to the kernel by value (the edges are staged in shared memory).
+struct GsOccCfg {
+  int nedges;
+  int edges[GS_OCC_MAX_EDGES];
+};
+
+// The last row of an unfinished window of an event-driven run, weighed once its successor (or the end) is seen.
+struct GsOccCarry {
+  long long delta;
+  int busy, running, queued, valid;
+};
+
+// Partial sums of a fold: GS_OCC_NSUM sums, then two maxima (gs_sum_block_vec's layout).
+enum { GS_OCC_ROWS, GS_OCC_TICKS, GS_OCC_BUSY, GS_OCC_RUNNING, GS_OCC_QUEUED, GS_OCC_WAIT, GS_OCC_IDLE, GS_OCC_NSUM,
+       GS_OCC_RMAX = GS_OCC_NSUM, GS_OCC_QMAX, GS_OCC_N };
+
+// A queue edge setting from the C ABI's array, or false (the message in *why) when it is not valid.
+static inline bool gs_occ_make_cfg(int32_t nedges, const int32_t *edges, GsOccCfg &cfg, const char **why) {
+  *why = "nedges must be in 0..255";
+  if (nedges < 0 || nedges > GS_OCC_MAX_EDGES) return false;
+  *why = "a NULL array with a positive count";
+  if (nedges > 0 && !edges) return false;
+  *why = "the edges must be >= 0 and strictly increasing";
+  for (int i = 0; i < nedges; ++i)
+    if (edges[i] < 0 || (i > 0 && edges[i] <= edges[i - 1])) return false;
+  cfg = GsOccCfg{};
+  cfg.nedges = nedges;
+  for (int i = 0; i < nedges; ++i) cfg.edges[i] = edges[i];
+  return true;
+}
+
+GS_SUM_HD void gs_occ_zero(long long (&v)[GS_OCC_N]) {
+  for (int e = 0; e < GS_OCC_N; ++e) v[e] = 0;
+}
+
+// `nrows` rows that hold (busy, running, queued) for w ticks in all, into the partial sums.
+GS_SUM_HD void gs_occ_part(long long (&v)[GS_OCC_N], int G, int busy, int running, int queued, long long nrows, long long w) {
+  v[GS_OCC_ROWS] += nrows;
+  if (w <= 0) return;
+  v[GS_OCC_TICKS] += w;
+  v[GS_OCC_BUSY] += w * busy; v[GS_OCC_RUNNING] += w * running; v[GS_OCC_QUEUED] += w * queued;
+  if (queued > 0) { v[GS_OCC_WAIT] += w; v[GS_OCC_IDLE] += w * (G - busy); }
+  v[GS_OCC_RMAX] = running > v[GS_OCC_RMAX] ? running : v[GS_OCC_RMAX];
+  v[GS_OCC_QMAX] = queued > v[GS_OCC_QMAX] ? queued : v[GS_OCC_QMAX];
+}
+
+GS_SUM_HD void gs_occ_add(gs_occ &o, const long long (&v)[GS_OCC_N]) {
+  o.rows += v[GS_OCC_ROWS]; o.ticks += v[GS_OCC_TICKS];
+  o.busy_sum += v[GS_OCC_BUSY]; o.running_sum += v[GS_OCC_RUNNING]; o.queued_sum += v[GS_OCC_QUEUED];
+  o.wait_ticks += v[GS_OCC_WAIT]; o.idle_wait_sum += v[GS_OCC_IDLE];
+  o.running_max = (int)(v[GS_OCC_RMAX] > o.running_max ? v[GS_OCC_RMAX] : o.running_max);
+  o.queued_max = (int)(v[GS_OCC_QMAX] > o.queued_max ? v[GS_OCC_QMAX] : o.queued_max);
+}
+
+// Histograms of one replica: H_all and H_wait (G + 1 counters each) and the queue's E + 1 counters.
+struct GsOccHist {
+  unsigned long long *all, *wait, *q;
+};
+
+// One stretch of w ticks into the partial sums and, serially, the histograms.
+GS_SUM_HD void gs_occ_stretch(long long (&v)[GS_OCC_N], const GsOccHist &H, const GsOccCfg &cfg, int G, int busy, int running, int queued,
+                              long long nrows, long long w) {
+  gs_occ_part(v, G, busy, running, queued, nrows, w);
+  if (w <= 0) return;
+  H.all[busy] += (unsigned long long)w;
+  if (queued > 0) H.wait[busy] += (unsigned long long)w;
+  H.q[gs_jd_bin(cfg.edges, cfg.nedges, queued)] += (unsigned long long)w;
+}
+
+// Host and device serial fold, `gs_occ_serial`: rows lo .. hi - 1 (rows[i - base]) into one replica's record and
+// histograms.  per_tick (horus): every row weighs 1.  Otherwise (event-driven policies) a row weighs the step of
+// `delta` to its successor, clamped at 0: the carry holds the last row seen, which the next row -- of this call or of
+// a later one -- weighs; at the end of a finished run (done) it weighs 1 and the carry is cleared.
+GS_SUM_HD void gs_occ_serial(gs_occ &o, GsOccCarry &c, const GsOccHist &H, const GsOccCfg &cfg, const gs_tick_row *rows, long long base,
+                             long long lo, long long hi, int done, int per_tick) {
+  long long v[GS_OCC_N];
+  gs_occ_zero(v);
+  const int G = o.total_gpus;
+  for (long long i = lo; i < hi; ++i) {
+    const gs_tick_row &r = rows[i - base];
+    if (per_tick) { gs_occ_stretch(v, H, cfg, G, r.busy_gpus, r.running, r.queued, 1, 1); continue; }
+    if (c.valid) gs_occ_stretch(v, H, cfg, G, c.busy, c.running, c.queued, 1, r.now > c.delta ? r.now - c.delta : 0);
+    c.delta = r.now; c.busy = r.busy_gpus; c.running = r.running; c.queued = r.queued; c.valid = 1;
+  }
+  if (!per_tick && c.valid && done) { gs_occ_stretch(v, H, cfg, G, c.busy, c.running, c.queued, 1, 1); c.valid = 0; }
+  gs_occ_add(o, v);
+}
+
+// fifo: the records of a window, rows with `delta` <= wm skipped (gs_sum_fold_records' rows), every row one tick.
+GS_SUM_HD void gs_occ_records_serial(gs_occ &o, const GsOccHist &H, const GsOccCfg &cfg, const gs_evrow *ev, int nev, long long ticks,
+                                     long long wm) {
+  long long v[GS_OCC_N];
+  gs_occ_zero(v);
+  for (int k = 0; k < nev; ++k) {
+    const long long t_last = k + 1 < nev ? (long long)ev[k + 1].now - 1 : ticks;
+    const long long v_lo = ev[k].now > wm + 1 ? (long long)ev[k].now : wm + 1;
+    if (t_last >= v_lo) gs_occ_stretch(v, H, cfg, o.total_gpus, ev[k].busy_gpus, ev[k].running, ev[k].queued, t_last - v_lo + 1, t_last - v_lo + 1);
+  }
+  gs_occ_add(o, v);
+}
+
 #ifndef __CUDACC__
 #include <vector>
 // Host forms of the job part (the host-emulation build of gs_horus.cu, CPU tests): the same sums, and the same radix
@@ -790,6 +896,117 @@ __device__ void gs_sum_block_vec(long long (&v)[N]) {
 #pragma unroll
   for (int e = 0; e < N; ++e) v[e] = res[e];
   __syncthreads();
+}
+
+// ---- occupancy block function.  One block per replica; every thread folds one fifo record or one row at a time into
+// its partial sums and the histograms.  H_all / H_wait live in dynamic shared memory when their 2 * (G + 1) counters
+// fit GS_OCC_SMEM_COUNTERS, else in the replica's global slot.  Lanes of a warp that
+// add to the same counter sum their weights first and the lowest of them adds once: on a nearly full cluster most
+// stretches hit one busy bin.  Integer adds only, so the result does not depend on the order.
+enum { GS_OCC_FIFO = 0, GS_OCC_EVENTS = 1, GS_OCC_PER_TICK = 2 };
+
+__device__ __forceinline__ void gs_occ_warp_hist(unsigned long long *stage, unsigned long long *all, unsigned long long *wait,
+                                                 unsigned long long *q, const int *edges, int E, bool has, int busy, int queued,
+                                                 long long w) {
+  const int lane = threadIdx.x & 31;
+  unsigned long long *st = stage + (threadIdx.x & ~31);
+  st[lane] = has ? (unsigned long long)w : 0ull;
+  __syncwarp();
+  const int kb = has ? 2 * busy + (queued > 0) : -1;
+  unsigned g = __match_any_sync(0xffffffffu, kb);
+  if (kb >= 0 && lane == __ffs(g) - 1) {
+    unsigned long long s = 0;
+    for (unsigned m = g; m; m &= m - 1) s += st[__ffs(m) - 1];
+    atomicAdd(all + busy, s);
+    if (queued > 0) atomicAdd(wait + busy, s);
+  }
+  const int kq = has ? gs_jd_bin(edges, E, queued) : -1;
+  g = __match_any_sync(0xffffffffu, kq);
+  if (kq >= 0 && lane == __ffs(g) - 1) {
+    unsigned long long s = 0;
+    for (unsigned m = g; m; m &= m - 1) s += st[__ffs(m) - 1];
+    atomicAdd(q + kq, s);
+  }
+  __syncwarp();
+}
+
+// Block-cooperative fold of one replica into rec, its carry (GS_OCC_EVENTS), and its histograms hall[0 .. G] /
+// hwait[0 .. G] / hq[0 .. E] in global memory (added to); sh: the kernel's GS_OCC_SMEM_COUNTERS shared counters.  GS_OCC_FIFO: the records ev[0 .. nev) past `delta` = wm
+// (gs_occ_records_serial); otherwise rows lo .. hi - 1 (rows[i - base]) as gs_occ_serial folds them: thread i reads rows
+// i and i + 1, and thread 0 weighs the carry.
+__device__ void gs_occ_fold(int mode, unsigned long long *occ_dyn, gs_occ *rec, GsOccCarry *carry, unsigned long long *hall,
+                            unsigned long long *hwait, unsigned long long *hq, const GsOccCfg &cfg, int G, const gs_evrow *ev, int nev,
+                            long long ticks, long long wm, const gs_tick_row *rows, long long base, long long lo, long long hi, int done) {
+  __shared__ unsigned long long q_sh[GS_OCC_MAX_EDGES + 1];
+  __shared__ unsigned long long stage[GS_SUM_THREADS];
+  __shared__ int e_sh[GS_OCC_MAX_EDGES];
+  const int E = cfg.nedges;
+  const bool sm = 2 * (G + 1) <= GS_OCC_SMEM_COUNTERS;
+  for (int i = threadIdx.x; i < E; i += blockDim.x) e_sh[i] = cfg.edges[i];
+  for (int i = threadIdx.x; i <= E; i += blockDim.x) q_sh[i] = 0;
+  if (sm)
+    for (int i = threadIdx.x; i < 2 * (G + 1); i += blockDim.x) occ_dyn[i] = 0;
+  __syncthreads();
+  unsigned long long *all = sm ? occ_dyn : hall, *wait = sm ? occ_dyn + G + 1 : hwait;
+  long long v[GS_OCC_N];
+  gs_occ_zero(v);
+  if (mode == GS_OCC_FIFO) {
+    for (int t0 = 0; t0 < nev; t0 += blockDim.x) {
+      const int k = t0 + threadIdx.x;
+      int busy = 0, running = 0, queued = 0;
+      long long L = 0;
+      if (k < nev) {
+        const gs_evrow e = ev[k];
+        const long long t_last = k + 1 < nev ? (long long)ev[k + 1].now - 1 : ticks;
+        const long long v_lo = e.now > wm + 1 ? (long long)e.now : wm + 1;
+        L = t_last >= v_lo ? t_last - v_lo + 1 : 0;
+        busy = e.busy_gpus; running = e.running; queued = e.queued;
+      }
+      gs_occ_part(v, G, busy, running, queued, L, L);
+      gs_occ_warp_hist(stage, all, wait, q_sh, e_sh, E, L > 0, busy, queued, L);
+    }
+  } else {
+    GsOccCarry c{0, 0, 0, 0, 0};
+    if (mode == GS_OCC_EVENTS && threadIdx.x < 32) {        // warp 0: the carry, weighed by its successor or the end
+      if (threadIdx.x == 0) c = *carry;
+      const bool has = threadIdx.x == 0 && c.valid && (hi > lo || done);
+      const long long w = !has ? 0 : hi > lo ? (rows[lo - base].now > c.delta ? rows[lo - base].now - c.delta : 0) : 1;
+      if (has) gs_occ_part(v, G, c.busy, c.running, c.queued, 1, w);
+      gs_occ_warp_hist(stage, all, wait, q_sh, e_sh, E, has && w > 0, c.busy, c.queued, w);
+    }
+    for (long long t0 = lo; t0 < hi; t0 += blockDim.x) {
+      const long long i = t0 + threadIdx.x;
+      int busy = 0, running = 0, queued = 0;
+      long long n = 0, w = 0;
+      if (i < hi) {
+        const gs_tick_row &r = rows[i - base];
+        busy = r.busy_gpus; running = r.running; queued = r.queued;
+        if (mode == GS_OCC_PER_TICK) { n = 1; w = 1; }
+        else if (i + 1 < hi) { const long long d = (long long)rows[i + 1 - base].now - r.now; n = 1; w = d > 0 ? d : 0; }
+        else if (done) { n = 1; w = 1; }                    // the last row of a finished run; otherwise it becomes the carry
+      }
+      gs_occ_part(v, G, busy, running, queued, n, w);
+      gs_occ_warp_hist(stage, all, wait, q_sh, e_sh, E, w > 0, busy, queued, w);
+    }
+    if (mode == GS_OCC_EVENTS && threadIdx.x == 0) {
+      if (hi > lo && !done) {
+        const gs_tick_row &r = rows[hi - 1 - base];
+        c.delta = r.now; c.busy = r.busy_gpus; c.running = r.running; c.queued = r.queued; c.valid = 1;
+      } else if (done) {
+        c.valid = 0;
+      }
+      *carry = c;
+    }
+  }
+  gs_sum_block_vec<GS_OCC_N, GS_OCC_NSUM, 0>(v);            // ends with a barrier: the shared counters are complete
+  if (threadIdx.x == 0) { gs_occ_add(*rec, v); rec->total_gpus = G; }
+  if (sm)
+    for (int i = threadIdx.x; i < 2 * (G + 1); i += blockDim.x) {
+      const unsigned long long x = occ_dyn[i];
+      if (x) (i <= G ? hall[i] : hwait[i - G - 1]) += x;
+    }
+  for (int i = threadIdx.x; i <= E; i += blockDim.x)
+    if (q_sh[i]) hq[i] += q_sh[i];
 }
 
 // Radix select of the 5 * M order statistics (M value columns x 5 ranks; M = 3 unless stated) of k values per column,

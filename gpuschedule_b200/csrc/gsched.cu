@@ -87,6 +87,8 @@ struct SimHost {
   bool tl_done = false;                   // summarised with the timeline on since it was prepared
   bool jd_done = false;                   // summarised with the current jobdist setting since it was prepared
   bool sd_done = false;                   // summarised with the current slowdown setting since it was prepared
+  bool occ_fresh = true;                  // the occupancy record, carry and histograms are to be zeroed before the next fold
+  bool occ_done = false;                  // summarised with the occupancy on since it was prepared
   SimDev dev;
   SimLayout layout;
 };
@@ -129,6 +131,10 @@ struct gs_engine {
   gs_sdclass *d_sd = nullptr; size_t sd_bytes = 0;      // gs_set_slowdown: nsims x C class records
   unsigned *d_sd_hist = nullptr; size_t sd_hist_bytes = 0;   // and nsims x C x (3 (E + 1) + Esd + 1) CDF counts
   GsSdCfg sd{};                                          // sd.nclasses = 0: off
+  bool occ_on = false; GsOccCfg occ{};                   // gs_set_occupancy
+  gs_occ *d_occ = nullptr; GsOccCarry *d_occ_carry = nullptr;   // nsims records and carries
+  unsigned long long *d_occ_busy = nullptr; int64_t occ_pitch = 0;   // nsims x [H_all, H_wait] x occ_pitch counters
+  unsigned long long *d_occ_q = nullptr; size_t occ_q_bytes = 0;     // nsims x (E + 1) queue counters
   // gs_boot_population: the records of the base trace, then its k - 1 gaps (int32)
   void *d_pop = nullptr; int64_t pop_k = 0; int64_t pop_max_gap = 0; double pop_max_need = 1.0;
   // gs_boot_mixes: nmix alias tables of pop_k entries each, mix-major, and their weight sums
@@ -214,6 +220,10 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->d_jd_hist) cudaFree(h->d_jd_hist);
   if (h->d_sd) cudaFree(h->d_sd);
   if (h->d_sd_hist) cudaFree(h->d_sd_hist);
+  if (h->d_occ) cudaFree(h->d_occ);
+  if (h->d_occ_carry) cudaFree(h->d_occ_carry);
+  if (h->d_occ_busy) cudaFree(h->d_occ_busy);
+  if (h->d_occ_q) cudaFree(h->d_occ_q);
   if (h->d_pop) cudaFree(h->d_pop);
   if (h->d_mix) cudaFree(h->d_mix);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
@@ -545,6 +555,7 @@ static int bind_sim(gs_handle h, SimHost &s, const SimLayout &L, unsigned char *
   D.need_init = 1;
   s.sum_rows = 0; s.sum_fresh = true;
   s.tl_fresh = true; s.tl_done = false; s.jd_done = false; s.sd_done = false;
+  s.occ_fresh = true; s.occ_done = false;
   s.prepared = true;
   return GS_OK;
 }
@@ -1113,6 +1124,23 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_tl_rows_kernel(const SimDev
   gs_tl_util_nan(T, B);
 }
 
+// Occupancy: the same rows as gs_sum_rows_kernel into the replica's gs_occ, carry and histograms.  Launched before it,
+// like gs_tl_rows_kernel.  fifo folds the records alone: busy, running and queued are constant over a record.
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_occ_rows_kernel(const SimDev *sims, int first, const gs_summary *acc, GsOccCfg cfg,
+                                                                     gs_occ *occ, GsOccCarry *carry, unsigned long long *busy,
+                                                                     long long pitch, unsigned long long *queue) {
+  extern __shared__ unsigned long long occ_dyn[];          // 2 * (G + 1) counters where they fit GS_OCC_SMEM_COUNTERS
+  const int r = first + blockIdx.x;
+  const SimDev &S = sims[r];
+  const long long wm = acc[r].rows;
+  unsigned long long *hall = busy + (size_t)r * 2 * (size_t)pitch, *hq = queue + (size_t)r * (size_t)(cfg.nedges + 1);
+  if (S.policy == GS_SCHED_FIFO)
+    gs_occ_fold(GS_OCC_FIFO, occ_dyn, occ + r, nullptr, hall, hall + pitch, hq, cfg, S.M * S.G, S.evrows, S.nev, S.ticks, wm, nullptr, 0, 0, 0, 1);
+  else
+    gs_occ_fold(GS_OCC_EVENTS, occ_dyn, occ + r, carry + r, hall, hall + pitch, hq, cfg, S.M * S.G, nullptr, 0, 0, 0, S.rows, S.row_first,
+                wm > S.row_first ? wm : S.row_first, S.ticks, S.done);
+}
+
 // The finished jobs as job.csv prints them (gs_expand_jobs_kernel for fifo, the job records otherwise).  job(r, i) is
 // the i-th job of the finish order, job_at(r, j) job j of the trace (meaningful once it has finished).
 struct GsSumEngineJobs {
@@ -1142,6 +1170,26 @@ struct GsSumEngineJobs {
   }
 };
 
+// The busy histograms' pitch: G + 1 counters of the largest cluster summarised so far.  A larger one moves every
+// replica's counters to the new pitch.
+static int ensure_occ_pitch(gs_handle h, int first, int count) {
+  int64_t need = 1;
+  for (int i = first; i < first + count; ++i) need = std::max(need, (int64_t)h->sims[(size_t)i].dev.M * h->sims[(size_t)i].dev.G + 1);
+  if (need <= h->occ_pitch) return GS_OK;
+  const size_t bytes = 16 * (size_t)need * (size_t)h->nsims;
+  unsigned long long *d = nullptr;
+  CU(cudaMalloc(&d, bytes));
+  CU(cudaMemsetAsync(d, 0, bytes, h->stream));
+  if (h->d_occ_busy) {
+    CU(cudaMemcpy2DAsync(d, 8 * (size_t)need, h->d_occ_busy, 8 * (size_t)h->occ_pitch, 8 * (size_t)h->occ_pitch, 2 * (size_t)h->nsims,
+                         cudaMemcpyDeviceToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_occ_busy);
+  }
+  h->d_occ_busy = d; h->occ_pitch = need;
+  return GS_OK;
+}
+
 extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, double *kernel_ms) {
   if (!h) return GS_ERR_ARG;
   if (first < 0 || count < 0 || first + count > h->nsims || (count > 0 && !out)) return fail(h, GS_ERR_ARG, "gs_summarize: bad arguments");
@@ -1154,8 +1202,11 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
     if (s.sum_rows < s.dev.row_first)
       return fail(h, GS_ERR_STATE, "gs_summarize: a replica ran a window that was not summarised (call gs_summarize after every gs_run)");
     kmax = std::max(kmax, (int64_t)s.dev.finished);
+    if (h->occ_on && (int64_t)s.dev.M * s.dev.G > GS_OCC_MAX_GPUS)
+      return fail(h, GS_ERR_ARG, "gs_summarize: the occupancy statistics take clusters of at most 65535 GPUs");
   }
   CU(cudaSetDevice(h->device));
+  if (h->occ_on) { const int rc = ensure_occ_pitch(h, first, count); if (rc) return rc; }
   if (!h->d_sum) {
     CU(cudaMalloc(&h->d_sum, sizeof(gs_summary) * (size_t)h->nsims));
     CU(cudaMemset(h->d_sum, 0, sizeof(gs_summary) * (size_t)h->nsims));
@@ -1173,8 +1224,26 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
     SimHost &s = h->sims[(size_t)i];
     if (s.sum_fresh) { CU(cudaMemsetAsync(h->d_sum + i, 0, sizeof(gs_summary), h->stream)); s.sum_fresh = false; }
     if (B > 0 && s.tl_fresh) { CU(cudaMemsetAsync(h->d_tl + (size_t)i * B, 0, sizeof(gs_tbin) * (size_t)B, h->stream)); s.tl_fresh = false; }
+    if (h->occ_on && s.occ_fresh) {
+      CU(cudaMemsetAsync(h->d_occ + i, 0, sizeof(gs_occ), h->stream));
+      CU(cudaMemsetAsync(h->d_occ_carry + i, 0, sizeof(GsOccCarry), h->stream));
+      CU(cudaMemsetAsync(h->d_occ_busy + (size_t)i * 2 * (size_t)h->occ_pitch, 0, 16 * (size_t)h->occ_pitch, h->stream));
+      CU(cudaMemsetAsync(h->d_occ_q + (size_t)i * (h->occ.nedges + 1), 0, 8 * (size_t)(h->occ.nedges + 1), h->stream));
+      s.occ_fresh = false;
+    }
   }
   CU(cudaEventRecord(h->e0, h->stream));
+  if (h->occ_on) {        // before gs_sum_rows_kernel, which advances the watermark
+    int gsm = 0;          // dynamic shared memory for the replicas whose busy histograms fit it
+    for (int i = first; i < first + count; ++i) {
+      const int g = h->sims[(size_t)i].dev.M * h->sims[(size_t)i].dev.G;
+      if (2 * (g + 1) <= GS_OCC_SMEM_COUNTERS) gsm = std::max(gsm, g);
+    }
+    gs_occ_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 16 * (size_t)(gsm + 1), h->stream>>>(
+        h->d_sims, first, h->d_sum, h->occ, h->d_occ, h->d_occ_carry, h->d_occ_busy, (long long)h->occ_pitch, h->d_occ_q);
+    CU(cudaGetLastError());
+    h->launches += 1;
+  }
   if (B > 0) {            // before gs_sum_rows_kernel, which advances the watermark
     gs_tl_rows_kernel<<<(unsigned)count, GS_SUM_THREADS, 0, h->stream>>>(h->d_sims, first, h->d_sum, h->d_tl, (long long)h->tl_width, B);
     CU(cudaGetLastError());
@@ -1216,6 +1285,7 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
     if (B > 0) h->sims[(size_t)i].tl_done = true;
     if (C > 0) h->sims[(size_t)i].jd_done = true;
     if (Csd > 0) h->sims[(size_t)i].sd_done = true;
+    if (h->occ_on) h->sims[(size_t)i].occ_done = true;
   }
   return GS_OK;
 }
@@ -1347,6 +1417,62 @@ extern "C" int gs_fetch_slowdown(gs_handle h, int first, int count, gs_sdclass *
     CU(cudaMemcpyAsync(out, h->d_sd + (size_t)first * C, sizeof(gs_sdclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   if (hist_out)
     CU(cudaMemcpyAsync(hist_out, h->d_sd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  CU(wait_stream(h));
+  return GS_OK;
+}
+
+extern "C" int gs_set_occupancy(gs_handle h, int32_t on, int32_t nedges, const int32_t *edges) {
+  if (!h) return GS_ERR_ARG;
+  GsOccCfg cfg{};
+  const char *why = nullptr;
+  if (on && !gs_occ_make_cfg(nedges, edges, cfg, &why)) return fail(h, GS_ERR_ARG, std::string("gs_set_occupancy: ") + why);
+  for (const SimHost &s : h->sims)
+    if (s.prepared && !s.sum_fresh && s.sum_rows > 0)
+      return fail(h, GS_ERR_STATE, "gs_set_occupancy: a replica has already folded rows (set the occupancy before summarising a run, or after gs_reset)");
+  if (on) {
+    CU(cudaSetDevice(h->device));
+    const size_t need_q = 8 * (size_t)h->nsims * (size_t)(cfg.nedges + 1);
+    if (!h->d_occ) {
+      gs_occ *d = nullptr;
+      GsOccCarry *c = nullptr;
+      CU(cudaMalloc(&d, sizeof(gs_occ) * (size_t)h->nsims));
+      if (cudaMalloc(&c, sizeof(GsOccCarry) * (size_t)h->nsims) != cudaSuccess) { cudaFree(d); return fail(h, GS_ERR_CUDA, "gs_set_occupancy: cudaMalloc failed"); }
+      h->d_occ = d; h->d_occ_carry = c;
+    }
+    if (need_q > h->occ_q_bytes) {
+      unsigned long long *d = nullptr;
+      CU(cudaMalloc(&d, need_q));
+      if (h->d_occ_q) { CU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_occ_q); }
+      h->d_occ_q = d; h->occ_q_bytes = need_q;
+    }
+  }
+  h->occ_on = on != 0;
+  h->occ = cfg;
+  for (SimHost &s : h->sims) { s.occ_fresh = true; s.occ_done = false; }
+  return GS_OK;
+}
+
+extern "C" int gs_fetch_occupancy(gs_handle h, int first, int count, gs_occ *out, uint64_t *busy_hist, int32_t busy_pitch, uint64_t *queue_hist) {
+  if (!h) return GS_ERR_ARG;
+  if (first < 0 || count < 0 || first + count > h->nsims) return fail(h, GS_ERR_ARG, "gs_fetch_occupancy: bad arguments");
+  if (!h->occ_on) return fail(h, GS_ERR_STATE, "gs_fetch_occupancy: the occupancy statistics are off (gs_set_occupancy)");
+  int64_t width = 1;
+  for (int i = first; i < first + count; ++i) {
+    const SimHost &s = h->sims[(size_t)i];
+    if (!s.prepared || !s.occ_done)
+      return fail(h, GS_ERR_STATE, "gs_fetch_occupancy: a replica has not been summarised with the occupancy on since it was prepared");
+    width = std::max(width, (int64_t)s.dev.M * s.dev.G + 1);
+  }
+  if (busy_hist && count > 0 && busy_pitch < width)
+    return fail(h, GS_ERR_CAPACITY, "gs_fetch_occupancy: busy_pitch is smaller than total_gpus + 1 of a fetched replica");
+  if (count == 0) return GS_OK;
+  CU(cudaSetDevice(h->device));
+  if (out) CU(cudaMemcpyAsync(out, h->d_occ + first, sizeof(gs_occ) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  if (busy_hist)
+    CU(cudaMemcpy2DAsync(busy_hist, 8 * (size_t)busy_pitch, h->d_occ_busy + (size_t)first * 2 * (size_t)h->occ_pitch, 8 * (size_t)h->occ_pitch,
+                         8 * (size_t)std::min(width, h->occ_pitch), 2 * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  const size_t E1 = (size_t)h->occ.nedges + 1;
+  if (queue_hist) CU(cudaMemcpyAsync(queue_hist, h->d_occ_q + (size_t)first * E1, 8 * E1 * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(wait_stream(h));
   return GS_OK;
 }

@@ -26,6 +26,11 @@ Engine.slowdown / HorusEngine.slowdown): `slowdown_derived` gives per class jobd
 mean, sample std, minimum and five quantiles of the bounded slowdown (in units of slowdown: the record's fixed point
 over 1024), and the four CDFs; `slowdown_spread` their spread per class over the replicas that have jobs in it.
 
+Time-weighted occupancy (capi.OCC_DTYPE records and histograms from Engine.occupancy / HorusEngine.occupancy):
+`occupancy_derived` gives the time-weighted GPU share, the shares of time saturated and with jobs waiting, the GPU
+time left idle while jobs waited, mean running and queued jobs, busy-GPU points over all time and over waiting time,
+and the queue-length CDF; `occupancy_spread` their spread over replicas.
+
 Paired comparisons (capi.JPAIR_DTYPE records and CDF counts from Engine.compare / HorusEngine.compare): `pair_derived`
 gives per class and quantity the per-job differences d = x_b - x_a of two configurations on the same trace -- their
 mean, sample std, shares below / at / above zero, ten order statistics and CDF --, `pair_spread` their spread over
@@ -425,8 +430,96 @@ def slowdown_spread_flat(sp, c):
     return [float(sp[name][s][c]) for name in SLOWDOWN_METRICS for s in SPREAD_STATS]
 
 
+# ---------------------------------------------------------------- time-weighted occupancy
+OCC_METRICS = (("gpu_share", "saturated_share", "wait_share", "idle_wait_share", "idle_in_wait_share", "running_mean", "queued_mean")
+               + tuple(f"busy_p{q}" for q in QUANTILES) + tuple(f"busy_wait_p{q}" for q in QUANTILES))
+
+
+def _hist_point(hist, q):
+    """the value at fraction q of the multiset that holds hist[b] copies of b (nearest rank); NaN when it is empty"""
+    hist = [int(x) for x in hist]
+    k = sum(hist)
+    if k == 0:
+        return math.nan
+    r, acc = nearest_rank(q, k), 0
+    for b, c in enumerate(hist):
+        acc += c
+        if acc > r:
+            return float(b)
+    raise AssertionError("unreachable")
+
+
+def occupancy_derived(rec, busy_hist, queue_hist, edges):
+    """Numbers of one replica's time-weighted occupancy: `rec` OCC_DTYPE, `busy_hist` (2, P) with P > total_gpus (the
+    ticks with b busy GPUs over all time, then over the ticks with a queue), `queue_hist` (E + 1,), `edges` the E queue
+    edges.  With T = ticks and G = total_gpus:
+        gpu_share            busy_sum / (T G)                the time-weighted mean of num_busy_gpus over the GPUs
+        saturated_share      H_all[G] / T                    share of time with every GPU busy
+        wait_share           wait_ticks / T                  share of time with jobs queued
+        idle_wait_share      idle_wait_sum / (T G)           GPU time left idle while jobs waited, over all GPU time
+        idle_in_wait_share   idle_wait_sum / (wait_ticks G)  the same over the GPU time while jobs waited
+        running_mean, queued_mean                            running_sum / T, queued_sum / T
+        busy_p<q>, busy_wait_p<q>                            nearest-rank points of busy GPUs, each tick one value, over
+                                                             all time / over the ticks with a queue
+        queue_cdf            (E,)                            share of time with queue length <= each edge
+    NaN where a denominator is 0."""
+    T, G, W = int(rec["ticks"]), int(rec["total_gpus"]), int(rec["wait_ticks"])
+    busy_hist, queue_hist = np.asarray(busy_hist), np.asarray(queue_hist)
+    if busy_hist.ndim != 2 or busy_hist.shape[0] != 2 or busy_hist.shape[1] <= G or queue_hist.shape != (len(edges) + 1,):
+        raise ValueError("occupancy_derived: expected busy_hist (2, > total_gpus) and queue_hist (len(edges) + 1,)")
+    out = dict(
+        gpu_share=_div(int(rec["busy_sum"]), T * G),
+        saturated_share=_div(int(busy_hist[0, G]), T),
+        wait_share=_div(W, T),
+        idle_wait_share=_div(int(rec["idle_wait_sum"]), T * G),
+        idle_in_wait_share=_div(int(rec["idle_wait_sum"]), W * G),
+        running_mean=_div(int(rec["running_sum"]), T),
+        queued_mean=_div(int(rec["queued_sum"]), T),
+    )
+    for q in QUANTILES:
+        out[f"busy_p{q}"] = _hist_point(busy_hist[0, :G + 1], Fraction(q, 100))
+        out[f"busy_wait_p{q}"] = _hist_point(busy_hist[1, :G + 1], Fraction(q, 100))
+    cum = np.cumsum(queue_hist.astype(np.int64))[:len(edges)]
+    out["queue_cdf"] = cum / T if T else np.full(len(edges), math.nan)
+    return out
+
+
+def occupancy_spread(recs, busy_hists, queue_hists, edges, level=0.95):
+    """Spread across replicas (records (replicas,), busy_hists (replicas, 2, P), queue_hists (replicas, E + 1)) of every
+    OCC_METRICS entry and of the queue CDF at each edge: {metric: {mean, std, lo, hi}, "queue_cdf": {mean, std, lo, hi:
+    float arrays (E,)}}, with spread's rules (NaN throughout where a replica's value is NaN)."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    per = [occupancy_derived(recs[r], busy_hists[r], queue_hists[r], edges) for r in range(len(recs))]
+    out = {m: _spread_of(np.array([d[m] for d in per], dtype=np.float64), level) for m in OCC_METRICS}
+    cdf = np.stack([d["queue_cdf"] for d in per]) if per else np.zeros((0, len(edges)))
+    cols = [_spread_of(cdf[:, e], level) for e in range(len(edges))]
+    out["queue_cdf"] = {s: np.array([c[s] for c in cols], dtype=np.float64) for s in SPREAD_STATS}
+    return out
+
+
+def occupancy_columns():
+    """names of the flat columns `occupancy_flat` returns, in order"""
+    return ["rows", "ticks", "busy_sum", "running_sum", "queued_sum", "wait_ticks", "idle_wait_sum", "running_max", "queued_max",
+            "total_gpus"] + list(OCC_METRICS)
+
+
+def occupancy_flat(rec, d):
+    """one OCC_DTYPE record and its occupancy_derived dict as a list of Python values"""
+    return [int(rec[k]) for k in occupancy_columns()[:10]] + [float(d[m]) for m in OCC_METRICS]
+
+
+def occupancy_spread_columns():
+    return [f"{m}_{s}" for m in OCC_METRICS for s in SPREAD_STATS]
+
+
+def occupancy_spread_flat(sp):
+    return [float(sp[m][s]) for m in OCC_METRICS for s in SPREAD_STATS]
+
+
 # ---------------------------------------------------------------- paired comparisons of two configurations
-PAIR_POINTS = ("p0", "p1", "p5", "p10", "p50_lo", "p50", "p90", "p95", "p99", "p100")
+PAIR_POINTS =("p0", "p1", "p5", "p10", "p50_lo", "p50", "p90", "p95", "p99", "p100")
 PAIR_STATS = ("d_mean", "d_std", "lt_share", "eq_share", "gt_share") + tuple(f"d_{p}" for p in PAIR_POINTS)
 PAIR_METRICS = tuple(f"{m}_{s}" for m in JOBDIST_QUANTITIES for s in PAIR_STATS)
 PAIR_COUNTS = ("jobs", "only_a", "only_b")

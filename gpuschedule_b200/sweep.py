@@ -231,6 +231,32 @@ def _sd_row(sd):
     return 3 * (len(sd[3]) + 1) + len(sd[4]) + 1
 
 
+DEFAULT_QUEUE_EDGES = (0,) + tuple(2 ** i for i in range(31))      # queue length 0, 1, 2, 4, ... 2^30
+
+
+def check_occupancy(edges):
+    """the queue edges of an occupancy argument as a tuple of ints, or ValueError: at most 255, each >= 0, int32 and
+    strictly increasing"""
+    try:
+        edges = tuple(int(x) for x in edges)
+    except (TypeError, ValueError):
+        raise ValueError("occupancy: expected a sequence of queue edges") from None
+    if len(edges) > capi.OCC_MAX_EDGES:
+        raise ValueError(f"occupancy: at most {capi.OCC_MAX_EDGES} queue edges")
+    if any(not 0 <= e < 2 ** 31 for e in edges) or any(b <= a for a, b in zip(edges, edges[1:])):
+        raise ValueError("occupancy: the queue edges must be >= 0, int32 and strictly increasing")
+    return edges
+
+
+def _occ_pitch(flag_sets):
+    """busy histogram entries per row of a sweep's occupancy arrays: the largest M * G of its configurations, plus 1"""
+    pitch = 1
+    for fl in flag_sets:
+        cl = Infrastructure(fl).gs_cluster()
+        pitch = max(pitch, cl.num_switch * cl.num_node_p_switch * cl.num_gpu_p_node + 1)
+    return pitch
+
+
 DEFAULT_DIFF_EDGES = tuple(-2 ** i for i in range(30, -1, -1)) + (0,) + tuple(2 ** i for i in range(31))
 
 
@@ -265,7 +291,8 @@ def _compare_in(eng, pairs, members, bounds, edges):
     return eng.compare([pos[a] for a, _ in pairs], [pos[b] for _, b in pairs], bounds, edges)
 
 
-def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None, compare=None, slowdown=None):
+def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None, compare=None, slowdown=None,
+                      occupancy=None):
     """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
     same configurations and random streams as run_batched, but no row or job record is read back and nothing is
     written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus.
@@ -278,7 +305,15 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
     E + 1)) as the last element; both configurations of a pair must share a trace file and an engine.
     slowdown=(key, bounds, tau, edges, sd_edges): also compute every replica's job statistics by key with bounded
     slowdown on the device (gs_set_slowdown) and append (SDCLASS_DTYPE records (len(flag_sets), C), CDF counts
-    (len(flag_sets), C, 3 * (E + 1) + Esd + 1)) after the jobdist element (before the compare element)."""
+    (len(flag_sets), C, 3 * (E + 1) + Esd + 1)) after the jobdist element (before the compare element).
+    occupancy=queue edges: also compute every replica's time-weighted occupancy on the device (gs_set_occupancy) and
+    append (OCC_DTYPE records (len(flag_sets),), busy histograms (len(flag_sets), 2, P), queue histograms
+    (len(flag_sets), E + 1)) as the last element, P the largest M * G of the configurations plus 1."""
+    if occupancy is not None:
+        occ_edges = check_occupancy(occupancy)
+        occ_recs = np.zeros(len(flag_sets), dtype=capi.OCC_DTYPE)
+        occ_busy = np.zeros((len(flag_sets), 2, _occ_pitch(flag_sets)), dtype=np.uint64)
+        occ_q = np.zeros((len(flag_sets), len(occ_edges) + 1), dtype=np.uint64)
     if slowdown is not None:
         sd = check_slowdown(slowdown)
         sd_nc = len(sd[1]) + 1
@@ -309,7 +344,12 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 eng.set_jobdist(jd_bounds, jd_edges)
             if slowdown is not None:
                 eng.set_slowdown(*sd)
+            if occupancy is not None:
+                eng.set_occupancy(occ_edges)
             out[aware] = eng.summarize()
+            if occupancy is not None:
+                occ_recs[aware], ob, occ_q[aware] = eng.occupancy()
+                occ_busy[aware, :, :ob.shape[2]] = ob
             if timeline is not None:
                 bins[aware] = eng.timeline()
             if jobdist is not None:
@@ -329,7 +369,12 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 eng.set_jobdist(jd_bounds, jd_edges)
             if slowdown is not None:
                 eng.set_slowdown(*sd)
+            if occupancy is not None:
+                eng.set_occupancy(occ_edges)
             out[plain] = eng.run_summarized()
+            if occupancy is not None:
+                occ_recs[plain], ob, occ_q[plain] = eng.occupancy()
+                occ_busy[plain, :, :ob.shape[2]] = ob
             if timeline is not None:
                 bins[plain] = eng.timeline()
             if jobdist is not None:
@@ -340,7 +385,8 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
             if sel:
                 cmp_recs[sel], cmp_hist[sel] = _compare_in(eng, [pairs[k] for k in sel], plain, cmp_bounds, cmp_edges)
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
-           + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ()))
+           + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ())
+           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -405,7 +451,7 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1, mix=None):
 
 
 def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1,
-                        compare=None, mix=None, slowdown=None):
+                        compare=None, mix=None, slowdown=None, occupancy=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -433,7 +479,11 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     ValueError, raised before any engine is created.  A gittins replica still takes its index table from the base
     trace: the policy is not told about the shift.  With L > 1, only block starts are drawn from the mix.
     slowdown=(key, bounds, tau, edges, sd_edges): also append (SDCLASS_DTYPE records (..., C), CDF counts (..., C,
-    3 * (E + 1) + Esd + 1)) with the replicas' leading axes, after the jobdist element (before the compare element)."""
+    3 * (E + 1) + Esd + 1)) with the replicas' leading axes, after the jobdist element (before the compare element).
+    occupancy=queue edges: also append (OCC_DTYPE records (...), busy histograms (..., 2, P), queue histograms
+    (..., E + 1)) with the replicas' leading axes as the last element, P as in summarize_batched."""
+    if occupancy is not None:
+        occ_edges = check_occupancy(occupancy)
     _check_bootstrap_args(flag_sets, replicas, loads, n, block_len, mix)
     if slowdown is not None:
         sd = check_slowdown(slowdown)
@@ -458,6 +508,11 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     if jobdist is not None:
         jd_cls = np.zeros((len(flag_sets),) + lead + (nc,), dtype=capi.JCLASS_DTYPE)
         jd_hist = np.zeros((len(flag_sets),) + lead + (nc, 3, nb), dtype=np.uint32)
+    if occupancy is not None:
+        occ_pitch = _occ_pitch(flag_sets)
+        occ_recs = np.zeros((len(flag_sets),) + lead, dtype=capi.OCC_DTYPE)
+        occ_busy = np.zeros((len(flag_sets),) + lead + (2, occ_pitch), dtype=np.uint64)
+        occ_q = np.zeros((len(flag_sets),) + lead + (len(occ_edges) + 1,), dtype=np.uint64)
     if slowdown is not None:
         sd_recs = np.zeros((len(flag_sets),) + lead + (sd_nc,), dtype=capi.SDCLASS_DTYPE)
         sd_hist = np.zeros((len(flag_sets),) + lead + (sd_nc, sd_row), dtype=np.uint32)
@@ -507,7 +562,10 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
                 eng.set_jobdist(jd_bounds, jd_edges)
             if slowdown is not None:
                 eng.set_slowdown(*sd)
+            if occupancy is not None:
+                eng.set_occupancy(occ_edges)
             recs = eng.run_summarized()
+            occ = eng.occupancy() if occupancy is not None else None
             tl = eng.timeline() if timeline is not None else None
             jd = eng.jobdist() if jobdist is not None else None
             sdr = eng.slowdown() if slowdown is not None else None
@@ -531,8 +589,14 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
             if sdr is not None:
                 sd_recs[c] = sdr[0][part].reshape(lead + (sd_nc,))
                 sd_hist[c] = sdr[1][part].reshape(lead + (sd_nc, sd_row))
+            if occ is not None:
+                ob = occ[1][part]
+                occ_recs[c] = occ[0][part].reshape(lead)
+                occ_busy[c][..., :ob.shape[2]] = ob.reshape(lead + (2, ob.shape[2]))
+                occ_q[c] = occ[2][part].reshape(lead + (len(occ_edges) + 1,))
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
-           + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ()))
+           + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ())
+           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -762,6 +826,73 @@ def write_slowdown_cdf_csv(path, flag_sets, recs, hist, sd, loads=None, level=0.
                             w.writerow(_sd_keys(fl, sd, c, lk) + [m, edge] + tail)
 
 
+def write_occupancy_csv(path, flag_sets, recs, busy, queue, edges):
+    """one line per configuration: the flags, summary.occupancy_columns() (the record, then occupancy_derived's numbers)"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + summary.occupancy_columns())
+        for fl, rc, bh, qh in zip(flag_sets, recs, busy, queue):
+            w.writerow(_occ_keys(fl) + summary.occupancy_flat(rc, summary.occupancy_derived(rc, bh, qh, edges)))
+
+
+def write_occupancy_ci_csv(path, flag_sets, loads, recs, busy, queue, edges, level=0.95, block_len=None, mix=None):
+    """one line per (configuration, load[, block_len][, mix]): the flags, the load columns, the replica count and
+    summary.occupancy_spread's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["replicas", "level"] + summary.occupancy_spread_columns())
+        for fl, per_rc, per_bh, per_qh in zip(flag_sets, recs, busy, queue):
+            lines = zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_bh), _load_lines(loads, block_len, mix, per_qh))
+            for (keys, rc), (_, bh), (_, qh) in lines:
+                sp = summary.occupancy_spread(rc, bh, qh, edges, level=level)
+                w.writerow(_occ_keys(fl) + keys + [len(rc), level] + summary.occupancy_spread_flat(sp))
+
+
+def _occ_keys(fl):
+    return [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed]
+
+
+def _cdf_points(hist):
+    """(ticks, share of ticks <= each bin) of a histogram; NaN shares when it is empty"""
+    t = int(np.asarray(hist, dtype=np.uint64).sum())
+    cum = np.cumsum(np.asarray(hist, dtype=np.uint64))
+    return t, (cum / t if t else np.full(len(cum), np.nan))
+
+
+def write_occupancy_cdf_csv(path, flag_sets, recs, busy, queue, edges, loads=None, level=0.95, block_len=None, mix=None):
+    """one line per (configuration[, load[, block_len][, mix]], quantity, point): quantity busy (every b = 0 .. M * G,
+    all time), busy_wait (the same over the ticks with a queue) or queue (at every queue edge), the point and the
+    share of time at or below it (with loads: the replicas and the spread of that share)"""
+    import csv
+    boot = loads is not None
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["quantity", "point"]
+                   + (["replicas", "level"] + [f"cdf_{s}" for s in summary.SPREAD_STATS] if boot else ["ticks", "cdf"]))
+        for fl, per_rc, per_bh, per_qh in zip(flag_sets, recs, busy, queue):
+            G = Infrastructure(fl).gs_cluster()
+            G = G.num_switch * G.num_node_p_switch * G.num_gpu_p_node
+            lines = (zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_bh),
+                         _load_lines(loads, block_len, mix, per_qh)) if boot else [(([], per_rc), ([], per_bh), ([], per_qh))])
+            for (lk, rc), (_, bh), (_, qh) in lines:
+                if not boot:
+                    rc, bh, qh = rc[None], bh[None], qh[None]
+                rows = [("busy", b, bh[:, 0, :G + 1], b) for b in range(G + 1)] + [("busy_wait", b, bh[:, 1, :G + 1], b) for b in range(G + 1)]
+                rows += [("queue", e, qh, i) for i, e in enumerate(edges)]
+                cdfs = {}
+                for m, point, h, i in rows:
+                    if m not in cdfs:
+                        cdfs[m] = [_cdf_points(x) for x in h]
+                    vals = np.array([c[1][i] for c in cdfs[m]], dtype=np.float64)
+                    if boot:
+                        sp = summary._spread_of(vals, Fraction(str(level)))
+                        w.writerow(_occ_keys(fl) + lk + [m, point, len(vals), level] + [float(sp[s]) for s in summary.SPREAD_STATS])
+                    else:
+                        w.writerow(_occ_keys(fl) + [m, point, cdfs[m][0][0], float(vals[0])])
+
+
 def _pair_keys(fl, base):
     return [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, base.schedule]
 
@@ -938,7 +1069,28 @@ def main(argv=None):
     ap.add_argument("--sd-edges", type=int, nargs="+", default=None, metavar="E",
                     help=f"with --slowdown: CDF edges of the slowdown in units of 1/1024 (strictly increasing, at most "
                          f"{capi.SLOWDOWN_MAX_EDGES}; default 1024 * 2^i for i = 0 ... 20)")
+    ap.add_argument("--occupancy", default=None, metavar="FILE",
+                    help="with --summary: also compute each run's time-weighted occupancy on the GPU (busy GPUs, queue length and "
+                         "GPUs left idle while jobs wait, every row weighed by the ticks it stands for) and write one CSV line per "
+                         "configuration to FILE; with --bootstrap one line per (configuration, load) with the spread across replicas")
+    ap.add_argument("--queue-edges", type=int, nargs="+", default=None, metavar="E",
+                    help=f"with --occupancy: queue-length CDF edges (>= 0, strictly increasing, at most {capi.OCC_MAX_EDGES}; "
+                         "default 0 and 2^i for i = 0 ... 30)")
+    ap.add_argument("--occupancy-cdf", default=None, metavar="FILE",
+                    help="with --occupancy: one CSV line per (configuration[, load], quantity, point): the time share with at most "
+                         "b busy GPUs for every b, over all time and over the time with jobs queued, and with a queue length at "
+                         "most each queue edge")
     a = ap.parse_args(argv)
+    occupancy = None
+    if a.occupancy is not None:
+        if not a.summary:
+            ap.error("--occupancy needs --summary FILE")
+        try:
+            occupancy = check_occupancy(DEFAULT_QUEUE_EDGES if a.queue_edges is None else a.queue_edges)
+        except ValueError as e:
+            ap.error(str(e))
+    elif a.queue_edges is not None or a.occupancy_cdf is not None:
+        ap.error("--queue-edges and --occupancy-cdf need --occupancy FILE")
     slowdown = None
     if a.slowdown is not None:
         if not a.summary:
@@ -1038,8 +1190,15 @@ def main(argv=None):
             ap.error(str(e))
         bl = a.block_len
         res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist,
-                                  block_len=1 if bl is None else bl, compare=compare, mix=mix, slowdown=slowdown)
-        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None and slowdown is None else (res[0], res[1:])
+                                  block_len=1 if bl is None else bl, compare=compare, mix=mix, slowdown=slowdown, occupancy=occupancy)
+        recs, rest = (res, ()) if (timeline is None and jobdist is None and compare is None and slowdown is None
+                                   and occupancy is None) else (res[0], res[1:])
+        if occupancy is not None:
+            orec, obusy, oq = rest[-1]
+            rest = rest[:-1]
+            write_occupancy_ci_csv(a.occupancy, sets, loads, orec, obusy, oq, occupancy, block_len=bl, mix=mix_text)
+            if a.occupancy_cdf:
+                write_occupancy_cdf_csv(a.occupancy_cdf, sets, orec, obusy, oq, occupancy, loads=loads, block_len=bl, mix=mix_text)
         if compare is not None:
             pairs, cmp_bounds, cmp_edges = compare
             prec, phist = rest[-1]
@@ -1070,8 +1229,15 @@ def main(argv=None):
               + (f" x {len(mix_text)} mixes" if mix_text else "") + f" x {a.bootstrap} replicas")
         return
     if a.summary:
-        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare, slowdown=slowdown)
-        recs, rest = (res, ()) if timeline is None and jobdist is None and compare is None and slowdown is None else (res[0], res[1:])
+        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare, slowdown=slowdown, occupancy=occupancy)
+        recs, rest = (res, ()) if (timeline is None and jobdist is None and compare is None and slowdown is None
+                                   and occupancy is None) else (res[0], res[1:])
+        if occupancy is not None:
+            orec, obusy, oq = rest[-1]
+            rest = rest[:-1]
+            write_occupancy_csv(a.occupancy, sets, orec, obusy, oq, occupancy)
+            if a.occupancy_cdf:
+                write_occupancy_cdf_csv(a.occupancy_cdf, sets, orec, obusy, oq, occupancy)
         if compare is not None:
             pairs, cmp_bounds, cmp_edges = compare
             prec, phist = rest[-1]

@@ -508,6 +508,49 @@ typedef struct gs_slowdown_cfg {
 int gs_set_slowdown(gs_handle h, const gs_slowdown_cfg *cfg);
 int gs_fetch_slowdown(gs_handle h, int first, int count, gs_sdclass *out, uint32_t *hist_out);
 
+/* ---- time-weighted occupancy (occupancy) -----------------------------------------------------------------------
+ * The rows of gs_summary's row part, each weighed by the ticks it stands for.  busy = busy_gpus as the row holds it
+ * (horus: devices with at least one task), G = M * G of the replica's cluster (at most 65535).
+ * Weights: a row of the fifo or horus engine is one tick (a fifo record k stands for the now_(k+1) - now_k rows up to
+ * the next record, the last one for the rows up to `ticks`).  Row i of an event-driven policy weighs
+ * max(0, delta_(i+1) - delta_i) ticks: a row whose successor's delta is smaller or equal (dlas can emit such rows)
+ * weighs 0.  The last row of a finished run (done) weighs 1; the last row of an unfinished window is kept in a
+ * per-replica carry (its delta, busy, running and queued) and weighed when a later gs_summarize sees its successor
+ * or the run done.  Rows folded once are not folded again (gs_summarize's watermark).
+ * Per replica one gs_occ, all integers (w the weight of a row; T = ticks < 2^31; sums cannot overflow int64):
+ *   rows (rows weighed), ticks = T = sum of w, busy_sum / running_sum / queued_sum = sum of w * value,
+ *   running_max / queued_max over rows with w > 0, wait_ticks = sum of w over rows with queued > 0,
+ *   idle_wait_sum = sum of w * (G - busy) over rows with queued > 0, total_gpus = G.
+ * Histograms of ticks (uint64): H_all[b], b = 0..G, ticks with busy == b; H_wait[b], ticks with busy == b and
+ * queued > 0; Q[k], k = 0..E, ticks whose queue length v lies in bin #{i : e_i < v} of E strictly increasing edges
+ * e_0 < ... < e_{E-1}, each >= 0 (0 <= E <= GS_OCC_MAX_EDGES; jobdist's rule).  Sum of H_all = sum of Q = T,
+ * sum of H_wait = wait_ticks.  Integer adds only: a repeated call gives the same bytes.                       */
+#define GS_OCC_MAX_EDGES 255
+typedef struct gs_occ {
+  int64_t rows;                      /* rows weighed so far                                                         */
+  int64_t ticks;                     /* T, the sum of the weights                                                   */
+  int64_t busy_sum, running_sum, queued_sum;   /* sums of w * busy_gpus / running / queued                         */
+  int64_t wait_ticks;                /* sum of w over rows with queued > 0                                          */
+  int64_t idle_wait_sum;             /* sum of w * (total_gpus - busy_gpus) over rows with queued > 0               */
+  int32_t running_max, queued_max;   /* over rows with w > 0                                                        */
+  int32_t total_gpus;                /* M * G                                                                       */
+  int32_t reserved;
+} gs_occ;                            /* 72 bytes */
+/* gs_set_occupancy: while on != 0, every gs_summarize also folds the rows it folds into the replicas' gs_occ records
+ * and histograms, with queue edges edges[0 .. nedges); on = 0 (the default) turns it off, and the edges are then
+ * ignored.  Every replica starts again from zero.  GS_ERR_ARG for nedges outside 0..255, edges that are negative or
+ * not strictly increasing, or a NULL array with a positive count; GS_ERR_STATE when a replica has folded rows since it
+ * was last prepared (gs_set_timeline's rule); nothing changes on an error.  While it is on, gs_summarize returns
+ * GS_ERR_ARG, before anything changes, for a replica with more than 65535 GPUs.
+ * gs_fetch_occupancy copies, as of the last gs_summarize (synchronous; any output may be NULL), count records to out,
+ * replica first + i's H_all to busy_hist + i * 2 * busy_pitch and its H_wait busy_pitch entries further (entries past
+ * its total_gpus are 0 up to the widest fetched replica's, and not written beyond), and count * (E + 1) queue counts to queue_hist.  GS_ERR_ARG for a bad range,
+ * GS_ERR_CAPACITY for busy_hist with busy_pitch < total_gpus + 1 of a fetched replica, GS_ERR_STATE when the feature is
+ * off or a replica has not been summarised with it on since it was prepared (first gs_run, gs_reset, a new trace,
+ * gs_boot_traces*).                                                                                            */
+int gs_set_occupancy(gs_handle h, int32_t on, int32_t nedges, const int32_t *edges);
+int gs_fetch_occupancy(gs_handle h, int first, int count, gs_occ *out, uint64_t *busy_hist, int32_t busy_pitch, uint64_t *queue_hist);
+
 /* ---- paired per-job comparison of two replicas on the same trace ------------------------------------------
  * A pair (a, b) is two replicas of one handle that hold the same trace: the same job count n and, for every j < n,
  * a byte-equal gs_jobin record (gs_horus_compare: equal fields as taken by gs_horus_load_trace).  They may differ in

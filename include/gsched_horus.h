@@ -112,6 +112,13 @@ int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t count, gs_j
  * gs_horus_summarize from the same finished jobs.  Same meaning and errors as gs_set_slowdown / gs_fetch_slowdown. */
 int gs_horus_set_slowdown(gs_horus_handle h, const gs_slowdown_cfg *cfg);
 int gs_horus_fetch_slowdown(gs_horus_handle h, int32_t first, int32_t count, gs_sdclass *out, uint32_t *hist_out);
+/* Time-weighted occupancy (gs_occ and histograms, gsched.h) filled by gs_horus_summarize from the same rows [0, ticks),
+ * every row one tick.  gs_horus_summarize folds every row again on every call, so no carry is kept and the feature may
+ * be set at any time; setting it marks every replica as not summarised.  Otherwise the same meaning and errors as
+ * gs_set_occupancy / gs_fetch_occupancy.                                                                      */
+int gs_horus_set_occupancy(gs_horus_handle h, int32_t on, int32_t nedges, const int32_t *edges);
+int gs_horus_fetch_occupancy(gs_horus_handle h, int32_t first, int32_t count, gs_occ *out, uint64_t *busy_hist, int32_t busy_pitch,
+                             uint64_t *queue_hist);
 /* Paired per-job comparison (gs_jpair, gsched.h: gs_compare) of replicas of this handle that hold the same trace: equal
  * arrival, gpus, gpu_per_container, duration, memory, utilisation and mean-memory fields for every job.  The same
  * outputs, launches and errors as gs_compare; a replica has run once gs_horus_run has prepared it.           */
