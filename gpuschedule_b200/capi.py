@@ -114,6 +114,16 @@ OCC_DTYPE = np.dtype([("rows", "<i8"), ("ticks", "<i8"), ("busy_sum", "<i8"), ("
                       ("total_gpus", "<i4"), ("reserved", "<i4")])
 assert OCC_DTYPE.itemsize == 72
 OCC_MAX_EDGES = 255
+# gs_ifclass (include/gsched_horus.h): one job-size class of a horus-engine replica's finished jobs split by
+# interference -- jobdist's record of the degraded jobs (actual > original) and of the clean ones, then the
+# fixed-point (units of 2^-10 tick) actual durations' sum, 128-bit sum of squares and order statistics, the original
+# durations' sum, the degraded jobs' excess and lost GPU time, the jobs gandiva preempted, and the saturated jobs.
+IFCLASS_DTYPE = np.dtype([("degraded", JCLASS_DTYPE), ("clean", JCLASS_DTYPE), ("actual_sum", "<i8"), ("actual_sq_lo", "<u8"),
+                          ("actual_sq_hi", "<u8"), ("original_sum", "<i8"), ("excess_sum", "<i8"), ("lost_gpu_time_lo", "<u8"),
+                          ("lost_gpu_time_hi", "<u8"), ("preempted_jobs", "<i8"), ("clamped", "<i8"), ("degraded_jct_mid", "<i4", (2,)),
+                          ("actual_q", "<i4", (5,)), ("actual_mid", "<i4", (2,)), ("excess_max", "<i4"), ("preempt_max", "<i4"),
+                          ("reserved", "<i4")])
+assert IFCLASS_DTYPE.itemsize == 440
 OCC_MAX_GPUS = 65535
 
 
@@ -245,6 +255,9 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_set_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.gs_horus_fetch_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     lib.gs_horus_set_occupancy.restype = lib.gs_horus_fetch_occupancy.restype = C.c_int
+    lib.gs_horus_set_interference.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+    lib.gs_horus_fetch_interference.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+    lib.gs_horus_set_interference.restype = lib.gs_horus_fetch_interference.restype = C.c_int
     for name in ("gs_horus_summarize", "gs_horus_set_timeline", "gs_horus_fetch_timeline", "gs_horus_set_jobdist", "gs_horus_fetch_jobdist", "gs_horus_create", "gs_horus_destroy", "gs_horus_config", "gs_horus_load_trace", "gs_horus_load_stream", "gs_horus_load_words",
                  "gs_horus_run", "gs_horus_stats", "gs_horus_fetch"):
         getattr(lib, name).restype = C.c_int
@@ -584,6 +597,31 @@ class HorusEngine:
         """(OCC_DTYPE records (count,), uint64 busy histograms (count, 2, max total_gpus + 1): all time, waiting time,
         uint64 queue histograms (count, E + 1)) as of the last summarize()"""
         return _fetch_occupancy(self, self.lib.gs_horus_fetch_occupancy, "gs_horus_fetch_occupancy", first, count)
+
+    def set_interference(self, bounds):
+        """interference statistics filled by every summarize(): len(bounds) + 1 classes by num_gpu, each split into
+        degraded (actual > original) and clean jobs; bounds=None turns it off (include/gsched_horus.h:
+        gs_horus_set_interference)"""
+        if bounds is None:
+            self._check(self.lib.gs_horus_set_interference(self.h, 0, None), "gs_horus_set_interference")
+            self._if_classes = 0
+            return
+        b = np.asarray(bounds, dtype=np.int64).reshape(-1)
+        if b.size and (b.min() < -2 ** 31 or b.max() >= 2 ** 31):
+            raise GsError("gs_horus_set_interference: bounds must be int32", GS_ERR_ARG)
+        b = np.ascontiguousarray(b, dtype=np.int32)
+        self._check(self.lib.gs_horus_set_interference(self.h, len(b) + 1, b.ctypes.data_as(C.c_void_p) if len(b) else None),
+                    "gs_horus_set_interference")
+        self._if_classes = len(b) + 1
+
+    def interference(self, first=0, count=None):
+        """IFCLASS_DTYPE records (count, C) as of the last summarize()"""
+        count = self.nsims - first if count is None else int(count)
+        nc = getattr(self, "_if_classes", 0)
+        out = np.zeros((max(count, 1), max(nc, 1)), dtype=IFCLASS_DTYPE)
+        self._check(self.lib.gs_horus_fetch_interference(self.h, int(first), count, out.ctypes.data_as(C.c_void_p)),
+                    "gs_horus_fetch_interference")
+        return out[:count, :nc]
 
     def compare(self, a, b, bounds=(), edges=(), with_time=False):
         """paired per-job comparison of replicas b[i] against a[i] on the same trace (include/gsched_horus.h:

@@ -108,6 +108,10 @@ struct GsSumHorusJobs {
     const gs_horus_job_rec rec = S.recs[j];
     return gs_sum_job(S.jobs[j].arrive, rec.start, rec.end, rec.jct, rec.preempt, S.jobs[j].gpus);
   }
+  __device__ GsIfDur if_at(int r, int j) const {
+    const HSim &S = sims[r];
+    return GsIfDur{S.jobs[j].gpus, S.recs[j].original, S.recs[j].actual};
+  }
 };
 
 #endif  // __CUDACC__
@@ -125,6 +129,7 @@ struct HorusSimHost {
   bool jd_done = false;             // summarised with the current jobdist setting since it was prepared
   bool sd_done = false;             // summarised with the current slowdown setting since it was prepared
   bool occ_done = false;            // summarised with the occupancy on since it was prepared
+  bool if_done = false;             // summarised with the current interference setting since it was prepared
   gs_cluster cl{};
   gs_horus_params par{};
   std::vector<HJob> jobs;
@@ -161,6 +166,8 @@ struct gs_horus_handle_s {
   gs_occ *d_occ = nullptr;                               // nsims records
   unsigned long long *d_occ_busy = nullptr; int64_t occ_pitch = 0;   // nsims x [H_all, H_wait] x occ_pitch counters
   unsigned long long *d_occ_q = nullptr; size_t occ_q_bytes = 0;     // nsims x (E + 1) queue counters
+  gs_ifclass *d_if = nullptr; size_t if_bytes = 0;      // gs_horus_set_interference: nsims x C class records
+  GsJdCfg ifc{};                                         // ifc.nclasses = 0: off (bounds only)
   std::string err;
   std::vector<double> shared;       // one stream consumed by every replica that did not get its own
   double *d_shared = nullptr; size_t shared_cap = 0; bool shared_dirty = false;
@@ -217,6 +224,7 @@ extern "C" int gs_horus_destroy(gs_horus_handle h) {
   if (h->d_occ) cudaFree(h->d_occ);
   if (h->d_occ_busy) cudaFree(h->d_occ_busy);
   if (h->d_occ_q) cudaFree(h->d_occ_q);
+  if (h->d_if) cudaFree(h->d_if);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -406,7 +414,7 @@ static int prepare(gs_horus_handle h, HorusSimHost &s, long long rows_cap) {
   D.rows_cap = rows_cap;
   D.current_remaining = (long long)n; D.running_jobs = 0;
   s.rows_cap = rows_cap;
-  s.prepared = true; s.tl_done = false; s.jd_done = false; s.sd_done = false; s.occ_done = false;
+  s.prepared = true; s.tl_done = false; s.jd_done = false; s.sd_done = false; s.occ_done = false; s.if_done = false;
   return GS_OK;
 }
 
@@ -530,13 +538,13 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   HCU(cudaMemsetAsync(h->d_sum + first, 0, sizeof(gs_summary) * (size_t)count, h->stream));
   const int B = h->tl_nbins;
   if (B > 0) HCU(cudaMemsetAsync(h->d_tl + (size_t)first * B, 0, sizeof(gs_tbin) * (size_t)B * (size_t)count, h->stream));
-  const int C = h->jd.nclasses, Csd = h->sd.nclasses;
+  const int C = h->jd.nclasses, Csd = h->sd.nclasses, Cif = h->ifc.nclasses;
 #ifdef __CUDACC__
   int per_sm = 1, sms = 132;
   HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_sum_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   const int grid = std::min(count, std::max(1, per_sm) * sms);
-  const size_t pitch = (size_t)(kmax + 63) / 64 * 64, need = (Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid;
+  const size_t pitch = (size_t)(kmax + 63) / 64 * 64, need = (Cif > 0 ? GS_IF_ROWS : Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid;
   if (h->sum_scratch_bytes < need) {
     if (h->d_sum_scratch) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_sum_scratch); }
     h->d_sum_scratch = nullptr; h->sum_scratch_bytes = 0;
@@ -565,6 +573,15 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     const int grid_sd = std::min(grid, std::max(1, per_sd) * sms);
     gs_sd_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid_sd, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->sd,
                                                                                           h->d_sd, h->d_sd_hist, h->d_sum_scratch, (long long)pitch);
+    HCU(cudaGetLastError());
+    h->launches += 1;
+  }
+  if (Cif > 0) {          // after gs_sum_jobs_kernel, on the same scratch with GS_IF_ROWS rows
+    int per_if = 1;
+    HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_if, gs_if_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
+    const int grid_if = std::min(grid, std::max(1, per_if) * sms);
+    gs_if_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid_if, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->ifc,
+                                                                                          h->d_if, h->d_sum_scratch, (long long)pitch);
     HCU(cudaGetLastError());
     h->launches += 1;
   }
@@ -598,6 +615,14 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     gs_sum_jobs_serial(jobs.data(), S.nfin, A);
     if (C > 0) gs_jd_jobs_serial(jobs.data(), S.nfin, h->jd, h->d_jd + (size_t)r * C, h->d_jd_hist + (size_t)r * C * 3 * (h->jd.nedges + 1));
     if (Csd > 0) gs_sd_serial(jobs.data(), S.nfin, h->sd, h->d_sd + (size_t)r * Csd, h->d_sd_hist + (size_t)r * Csd * gs_sd_row_len(h->sd));
+    if (Cif > 0) {
+      std::vector<GsIfDur> durs((size_t)S.nfin);
+      for (int i = 0; i < S.nfin; ++i) {
+        const int j = S.fin[i];
+        durs[(size_t)i] = GsIfDur{S.jobs[j].gpus, S.recs[j].original, S.recs[j].actual};
+      }
+      gs_if_serial(jobs.data(), durs.data(), S.nfin, h->ifc, h->d_if + (size_t)r * Cif);
+    }
     if (B > 0) gs_tl_fold_rows_serial(h->d_tl + (size_t)r * B, B, (long long)h->tl_width, S.rows, S.util, 0, 0, S.ticks);
     if (h->occ_on) {
       gs_occ &o = h->d_occ[r];
@@ -622,6 +647,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     if (C > 0) h->sims[(size_t)i].jd_done = true;
     if (Csd > 0) h->sims[(size_t)i].sd_done = true;
     if (h->occ_on) h->sims[(size_t)i].occ_done = true;
+    if (Cif > 0) h->sims[(size_t)i].if_done = true;
   }
   return GS_OK;
 }
@@ -804,6 +830,41 @@ extern "C" int gs_horus_fetch_occupancy(gs_horus_handle h, int32_t first, int32_
   }
   const size_t E1 = (size_t)h->occ.nedges + 1;
   if (queue_hist) HCU(cudaMemcpyAsync(queue_hist, h->d_occ_q + (size_t)first * E1, 8 * E1 * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
+  return GS_OK;
+}
+
+extern "C" int gs_horus_set_interference(gs_horus_handle h, int32_t nclasses, const int32_t *bounds) {
+  if (!h) return GS_ERR_ARG;
+  GsJdCfg cfg;
+  const char *why = "nclasses must be in 0..8";
+  if (nclasses < 0 || nclasses > GS_JOBDIST_MAX_CLASSES || !gs_jd_make_cfg(nclasses, bounds, 0, nullptr, cfg, &why))
+    return hfail(h, GS_ERR_ARG, std::string("gs_horus_set_interference: ") + why);
+  const size_t need = sizeof(gs_ifclass) * h->sims.size() * (size_t)cfg.nclasses;
+  if (need > h->if_bytes) {
+    HCU(cudaSetDevice(h->device));
+    gs_ifclass *d = nullptr;
+    HCU(cudaMalloc(&d, need));
+    if (h->d_if) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_if); }
+    h->d_if = d; h->if_bytes = need;
+  }
+  h->ifc = cfg;
+  for (auto &s : h->sims) s.if_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_fetch_interference(gs_horus_handle h, int32_t first, int32_t count, gs_ifclass *out) {
+  if (!h) return GS_ERR_ARG;
+  const int nsims = (int)h->sims.size();
+  if (first < 0 || count < 0 || first > nsims - count || (count > 0 && !out)) return hfail(h, GS_ERR_ARG, "gs_horus_fetch_interference: bad arguments");
+  if (h->ifc.nclasses == 0) return hfail(h, GS_ERR_STATE, "gs_horus_fetch_interference: the interference statistics are off (gs_horus_set_interference)");
+  for (int i = first; i < first + count; ++i)
+    if (!h->sims[(size_t)i].prepared || !h->sims[(size_t)i].if_done)
+      return hfail(h, GS_ERR_STATE, "gs_horus_fetch_interference: a replica has not been summarised with this setting since it was prepared");
+  if (count == 0) return GS_OK;
+  HCU(cudaSetDevice(h->device));
+  const size_t C = (size_t)h->ifc.nclasses;
+  HCU(cudaMemcpyAsync(out, h->d_if + (size_t)first * C, sizeof(gs_ifclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   HCU(cudaStreamSynchronize(h->stream));
   return GS_OK;
 }

@@ -17,6 +17,7 @@
 #include <stdint.h>
 
 #include "gsched.h"
+#include "gsched_horus.h"
 
 #ifndef __CUDACC__
 #ifndef __host__
@@ -460,7 +461,45 @@ GS_SUM_HD void gs_occ_records_serial(gs_occ &o, const GsOccHist &H, const GsOccC
   gs_occ_add(o, v);
 }
 
+// ---- interference statistics of the utilisation-aware engine (gs_ifclass, include/gsched_horus.h)
+static_assert(sizeof(gs_ifclass) == 440 && sizeof(gs_ifclass) % 8 == 0, "gs_ifclass is 440 bytes, a multiple of 8");
+#define GS_IF_MAX 0x7fffffffll       // the saturated fixed-point duration, 2^31 - 1 (units of 2^-10 tick)
+#define GS_IF_ROWS 8                 // scratch rows per job: wait, turnaround, jct, a, o, e, gpus, preempt
+
+// What the engine's record says of a finished job: its GPUs, Job.duration and Job.get_duration().
+struct GsIfDur { int gpus; double original, actual; };
+// Its fixed-point values: a = fp(actual), o = fp(original), e = fp(actual - original) when degraded (else 0).
+struct GsIfVal { int a, o, e, degraded, clamped; };
+
+// fp(x) = min(2^31 - 1, max(0, round-half-even(1024 * x))); clamped |= 1 when the bound applies or x is NaN.
+GS_SUM_HD int gs_if_fp(double x, int &clamped) {
+#ifdef __CUDA_ARCH__
+  const long long r = __double2ll_rn(__dmul_rn(1024.0, x));            // NaN gives -2^63
+#else
+  const double d = nearbyint(1024.0 * x);                              // the default rounding mode: to nearest, ties to even
+  const long long r = d != d || d < -9.0e18 ? (long long)(-0x7fffffffffffffffll - 1) : d > 9.0e18 ? 0x7fffffffffffffffll : (long long)d;
+#endif
+  if (r < 0) { clamped = 1; return 0; }
+  if (r > GS_IF_MAX) { clamped = 1; return (int)GS_IF_MAX; }
+  return (int)r;
+}
+
+GS_SUM_HD GsIfVal gs_if_value(double original, double actual) {
+  GsIfVal v;
+  v.clamped = 0;
+  v.degraded = actual > original;
+  v.a = gs_if_fp(actual, v.clamped);
+  v.o = gs_if_fp(original, v.clamped);
+#ifdef __CUDA_ARCH__
+  v.e = v.degraded ? gs_if_fp(__dsub_rn(actual, original), v.clamped) : 0;
+#else
+  v.e = v.degraded ? gs_if_fp(actual - original, v.clamped) : 0;
+#endif
+  return v;
+}
+
 #ifndef __CUDACC__
+#include <algorithm>
 #include <vector>
 // Host forms of the job part (the host-emulation build of gs_horus.cu, CPU tests): the same sums, and the same radix
 // select run serially, one target at a time.
@@ -658,6 +697,54 @@ static inline void gs_sd_serial(const GsSumJob *jobs, long long k, const GsSdCfg
     gs_sum_select_serial(seg + pitch, kc, J.turnaround_q);
     gs_sum_select_serial(seg + 2 * pitch, kc, J.jct_q);
     gs_sum_select_serial(seg + 3 * pitch, kc, S.sd_q);
+  }
+}
+// Interference statistics of k finished jobs (jobs[i] and durs[i] of the same job): out[0 .. C) (overwritten).  Each
+// group (class, degraded or clean) takes gs_jd_jobs_serial's record as a class of its own; the rest are plain sums
+// and order statistics, the middle ones by std::nth_element.
+static inline void gs_if_serial(const GsSumJob *jobs, const GsIfDur *durs, long long k, const GsJdCfg &cfg, gs_ifclass *out) {
+  const int C = cfg.nclasses;
+  GsJdCfg one{};
+  one.nclasses = 1;
+  std::vector<GsSumJob> grp[2 * GS_JOBDIST_MAX_CLASSES];
+  std::vector<int> av[GS_JOBDIST_MAX_CLASSES], djct[GS_JOBDIST_MAX_CLASSES];
+  for (int c = 0; c < C; ++c) out[c] = gs_ifclass{};
+  for (long long i = 0; i < k; ++i) {
+    const GsSumJob &v = jobs[i];
+    const int c = gs_jd_class(cfg.bounds, C - 1, durs[i].gpus);
+    const GsIfVal x = gs_if_value(durs[i].original, durs[i].actual);
+    gs_ifclass &F = out[c];
+    grp[2 * c + x.degraded].push_back(v);
+    av[c].push_back(x.a);
+    if (x.degraded) {
+      djct[c].push_back(v.jct);
+      F.excess_sum += x.e;
+      F.excess_max = x.e > F.excess_max ? x.e : F.excess_max;
+      gs_sum_add128(F.lost_gpu_time_lo, F.lost_gpu_time_hi, (gs_i128)((long long)v.gpus * x.e));
+    }
+    F.actual_sum += x.a;
+    gs_jd_add_sq(F.actual_sq_lo, F.actual_sq_hi, x.a);
+    F.original_sum += x.o;
+    F.preempted_jobs += v.preempt > 1;
+    F.preempt_max = v.preempt > F.preempt_max ? v.preempt : F.preempt_max;
+    F.clamped += x.clamped;
+  }
+  auto mid = [](std::vector<int> v, int out2[2]) {
+    const long long n = (long long)v.size();
+    if (n == 0) { out2[0] = out2[1] = 0; return; }
+    std::nth_element(v.begin(), v.begin() + (n - 1) / 2, v.end());
+    out2[0] = v[(size_t)((n - 1) / 2)];
+    std::nth_element(v.begin(), v.begin() + n / 2, v.end());
+    out2[1] = v[(size_t)(n / 2)];
+  };
+  uint32_t hist[3];
+  for (int c = 0; c < C; ++c) {
+    gs_ifclass &F = out[c];
+    gs_jd_jobs_serial(grp[2 * c].data(), (long long)grp[2 * c].size(), one, &F.clean, hist);
+    gs_jd_jobs_serial(grp[2 * c + 1].data(), (long long)grp[2 * c + 1].size(), one, &F.degraded, hist);
+    gs_sum_select_serial(av[c].data(), (long long)av[c].size(), F.actual_q);
+    mid(av[c], F.actual_mid);
+    mid(djct[c], F.degraded_jct_mid);
   }
 }
 #endif
@@ -1488,6 +1575,192 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_cmp_pairs_kernel(Src src, i
       }
       __syncthreads();
       off += kc;
+    }
+  }
+}
+
+// Element `rank` (0 <= rank < k) of vals[0 .. k) sorted ascending, whose minimum is mn and range `span`: the passes of
+// gs_sum_select for one target at any rank.  Block-cooperative (every thread returns the value); hist: GS_SUM_BINS
+// shared counters.  The scratch writes it reads must be published by a barrier before the call.
+__device__ long long gs_if_select1(unsigned *hist, const int *vals, long long k, long long mn, long long span, long long rank) {
+  __shared__ unsigned long long pre;
+  __shared__ long long rk;
+  const int passes = gs_sum_passes((unsigned long long)span);
+  if (threadIdx.x == 0) { pre = 0; rk = rank; }
+  for (int p = 0; p < passes; ++p) {
+    const int shift = (passes - 1 - p) * 9;
+    for (int i = threadIdx.x; i < GS_SUM_BINS; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    const unsigned long long hp = pre;
+    for (long long i = threadIdx.x; i < k; i += blockDim.x) {
+      const unsigned long long u = (unsigned long long)((long long)vals[i] - mn);
+      if ((u >> (shift + 9)) == hp) atomicAdd(&hist[(u >> shift) & (GS_SUM_BINS - 1)], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { long long r = rk; const unsigned d = gs_sum_pick(hist, r); rk = r; pre = (hp << 9) | d; }
+    __syncthreads();
+  }
+  const long long out = mn + (long long)pre;
+  __syncthreads();                                          // every thread has read `pre` before a later call resets it
+  return out;
+}
+
+// Interference statistics (gs_ifclass) of replicas first .. first + count - 1, one block per replica in turn
+// (grid-stride), jobdist's steps over 2C groups, group = 2 * class + degraded: (1) per-group job counts and per-class
+// clamped counts, kept in registers and block-reduced; (2) group offsets: a class's clean and degraded segments are
+// adjacent; (3) every job's wait, turnaround, jct, a, o, e, gpus and preempt written to its group's segment of the
+// scratch (GS_IF_ROWS rows of `pitch` ints per block) through warp-aggregated shared cursors; (4) per group: jobdist's
+// fold of wait / turnaround / jct, then the fold of the other rows (sums, squares of a as sums of 32-bit halves,
+// gpus * e as sums of 32-bit halves, minima, maxima), gs_sum_select over the three rows and, for the degraded group,
+// the upper middle jct; (5) per class: gs_sum_select<1> and the upper middle over the a row of both segments.
+template <class Src>
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_if_jobs_kernel(Src src, int first, int count, GsJdCfg cfg, gs_ifclass *recs,
+                                                                   int *scratch, long long pitch) {
+  constexpr int NC = GS_JOBDIST_MAX_CLASSES, NG = 2 * NC;
+  __shared__ unsigned hist[GS_SUM_TARGETS * GS_SUM_BINS];
+  __shared__ unsigned long long prefix[GS_SUM_TARGETS];
+  __shared__ long long grp_cnt[NG], cls_clamped[NC];
+  __shared__ long long cursor[NG];
+  __shared__ gs_ifclass rec;                                // thread 0's alone
+  const int C = cfg.nclasses;
+  const int lane = threadIdx.x & 31;
+  int *vals = scratch + (size_t)blockIdx.x * GS_IF_ROWS * (size_t)pitch;
+  for (int b = blockIdx.x; b < count; b += gridDim.x) {
+    const int r = first + b;
+    const long long k = src.finished(r);
+    long long red[NG + NC];
+#pragma unroll
+    for (int e = 0; e < NG + NC; ++e) red[e] = 0;
+    for (long long i = threadIdx.x; i < k; i += blockDim.x) {
+      const GsIfDur d = src.if_at(r, src.order(r, i));
+      const GsIfVal x = gs_if_value(d.original, d.actual);
+      const int g = 2 * gs_jd_class(cfg.bounds, C - 1, d.gpus) + x.degraded;
+#pragma unroll
+      for (int u = 0; u < NG; ++u) {
+        if (g == u) { red[u] += 1; red[NG + u / 2] += x.clamped; }
+      }
+    }
+    gs_sum_block_vec<NG + NC, NG + NC, 0>(red);
+    if (threadIdx.x < NG) {
+      const int g = threadIdx.x;
+      long long off = 0;
+#pragma unroll
+      for (int u = 0; u < NG; ++u) off += u < g ? red[u] : 0;
+#pragma unroll
+      for (int u = 0; u < NG; ++u) {
+        if (u == g) { grp_cnt[g] = red[u]; if ((g & 1) == 0) cls_clamped[g / 2] = red[NG + u / 2]; }
+      }
+      cursor[g] = off;
+    }
+    __syncthreads();
+    for (long long i0 = 0; i0 < k; i0 += blockDim.x) {     // (warp-uniform trip count: the shuffles see full warps)
+      const long long i = i0 + threadIdx.x;
+      const bool in = i < k;
+      GsSumJob v;
+      GsIfVal x;
+      int g = -1;
+      if (in) {
+        const int j = src.order(r, i);
+        const GsIfDur d = src.if_at(r, j);
+        v = src.job_at(r, j);
+        x = gs_if_value(d.original, d.actual);
+        g = 2 * gs_jd_class(cfg.bounds, C - 1, d.gpus) + x.degraded;
+      }
+      const unsigned peers = __match_any_sync(0xffffffffu, g);
+      const int head = __ffs(peers) - 1;
+      long long base = 0;
+      if (in && lane == head) base = atomicAdd((unsigned long long *)&cursor[g], (unsigned long long)__popc(peers));
+      base = __shfl_sync(0xffffffffu, base, head);
+      if (in) {
+        const long long pos = base + __popc(peers & ((1u << lane) - 1u));
+        vals[pos] = v.wait; vals[pitch + pos] = v.turn; vals[2 * pitch + pos] = v.jct;
+        vals[3 * pitch + pos] = x.a; vals[4 * pitch + pos] = x.o; vals[5 * pitch + pos] = x.e;
+        vals[6 * pitch + pos] = v.gpus; vals[7 * pitch + pos] = v.preempt;
+      }
+    }
+    __syncthreads();
+    long long off = 0;
+    for (int c = 0; c < C; ++c) {
+      const long long off_c = off;
+      long long amin = 0x7fffffff, amax = -0x80000000ll;
+      if (threadIdx.x == 0) { rec = gs_ifclass{}; rec.clamped = cls_clamped[c]; }
+      for (int deg = 0; deg < 2; ++deg) {
+        const long long kg = grp_cnt[2 * c + deg];
+        const int *seg = vals + off;
+        // wait, turnaround, jct: jobdist's sums, square halves, minima and maxima
+        long long s[15] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0x7fffffff, 0x7fffffff, 0x7fffffff, -0x80000000ll, -0x80000000ll, -0x80000000ll};
+        for (long long i = threadIdx.x; i < kg; i += blockDim.x) {
+#pragma unroll
+          for (int m = 0; m < 3; ++m) {
+            const int v = seg[m * pitch + i];
+            const unsigned long long sq = (unsigned long long)((long long)v * v);
+            s[m] += v; s[3 + m] += (long long)(sq >> 32); s[6 + m] += (long long)(sq & 0xffffffffull);
+            s[9 + m] = min(s[9 + m], (long long)v); s[12 + m] = max(s[12 + m], (long long)v);
+          }
+        }
+        gs_sum_block_vec<15, 9, 3>(s);
+        // preempt_sum, gpu_ticks_sum, preempted jobs, a sum, a^2 halves, o sum, e sum, (gpus * e) halves | a min | a max,
+        // e max, preempt max
+        long long t[14] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0x7fffffff, -0x80000000ll, 0, 0};
+        for (long long i = threadIdx.x; i < kg; i += blockDim.x) {
+          const int jct = seg[2 * pitch + i], a = seg[3 * pitch + i], o = seg[4 * pitch + i], e = seg[5 * pitch + i];
+          const int gpus = seg[6 * pitch + i], pre = seg[7 * pitch + i];
+          const unsigned long long sq = (unsigned long long)((long long)a * a);
+          const unsigned long long lost = (unsigned long long)((long long)gpus * e);
+          t[0] += pre; t[1] += (long long)gpus * jct; t[2] += pre > 1;
+          t[3] += a; t[4] += (long long)(sq >> 32); t[5] += (long long)(sq & 0xffffffffull);
+          t[6] += o; t[7] += e; t[8] += (long long)(lost >> 32); t[9] += (long long)(lost & 0xffffffffull);
+          t[10] = min(t[10], (long long)a); t[11] = max(t[11], (long long)a); t[12] = max(t[12], (long long)e);
+          t[13] = max(t[13], (long long)pre);
+        }
+        gs_sum_block_vec<14, 10, 1>(t);
+        amin = min(amin, t[10]); amax = max(amax, t[11]);
+        long long span = 0;
+#pragma unroll
+        for (int m = 0; m < 3; ++m) span = max(span, s[12 + m] - s[9 + m]);
+        gs_sum_select(hist, prefix, seg, pitch, kg, s + 9, span);
+        if (threadIdx.x == 0) {
+          gs_jclass &J = deg ? rec.degraded : rec.clean;
+          J.jobs = kg; J.wait_sum = s[0]; J.turnaround_sum = s[1]; J.jct_sum = s[2]; J.preempt_sum = t[0]; J.gpu_ticks_sum = t[1];
+          gs_sum_add128(J.wait_sq_lo, J.wait_sq_hi, ((gs_i128)s[3] << 32) + s[6]);
+          gs_sum_add128(J.turnaround_sq_lo, J.turnaround_sq_hi, ((gs_i128)s[4] << 32) + s[7]);
+          gs_sum_add128(J.jct_sq_lo, J.jct_sq_hi, ((gs_i128)s[5] << 32) + s[8]);
+          for (int q = 0; q < 5; ++q) {
+            J.wait_q[q] = kg > 0 ? (int)(s[9] + (long long)prefix[q]) : 0;
+            J.turnaround_q[q] = kg > 0 ? (int)(s[10] + (long long)prefix[5 + q]) : 0;
+            J.jct_q[q] = kg > 0 ? (int)(s[11] + (long long)prefix[10 + q]) : 0;
+          }
+          rec.preempted_jobs += t[2];
+          rec.actual_sum += t[3];
+          gs_sum_add128(rec.actual_sq_lo, rec.actual_sq_hi, ((gs_i128)t[4] << 32) + t[5]);
+          rec.original_sum += t[6];
+          if (deg) {
+            rec.excess_sum = t[7];
+            rec.excess_max = kg > 0 ? (int)t[12] : 0;
+            gs_sum_add128(rec.lost_gpu_time_lo, rec.lost_gpu_time_hi, ((gs_i128)t[8] << 32) + t[9]);
+            rec.degraded_jct_mid[0] = J.jct_q[0];                // rank floor((k - 1) / 2): gs_summary's 50 % rank
+          }
+          rec.preempt_max = kg > 0 && t[13] > rec.preempt_max ? (int)t[13] : rec.preempt_max;
+        }
+        __syncthreads();                                    // thread 0 has read prefix before the next select
+        if (deg && kg > 0) {                                // (block-uniform)
+          const long long hi = gs_if_select1(hist, seg + 2 * pitch, kg, s[11], s[14] - s[11], kg / 2);
+          if (threadIdx.x == 0) rec.degraded_jct_mid[1] = (int)hi;
+        }
+        off += kg;
+      }
+      const long long kc = off - off_c;
+      const int *arow = vals + 3 * pitch + off_c;
+      gs_sum_select<1>(hist, prefix, arow, pitch, kc, &amin, amax - amin);
+      if (threadIdx.x == 0)
+        for (int q = 0; q < 5; ++q) rec.actual_q[q] = kc > 0 ? (int)(amin + (long long)prefix[q]) : 0;
+      __syncthreads();
+      if (kc > 0) {
+        const long long hi = gs_if_select1(hist, arow, kc, amin, amax - amin, kc / 2);
+        if (threadIdx.x == 0) { rec.actual_mid[0] = rec.actual_q[0]; rec.actual_mid[1] = (int)hi; }
+      }
+      if (threadIdx.x == 0) recs[(size_t)r * C + c] = rec;
+      __syncthreads();
     }
   }
 }

@@ -26,6 +26,13 @@ Engine.slowdown / HorusEngine.slowdown): `slowdown_derived` gives per class jobd
 mean, sample std, minimum and five quantiles of the bounded slowdown (in units of slowdown: the record's fixed point
 over 1024), and the four CDFs; `slowdown_spread` their spread per class over the replicas that have jobs in it.
 
+Interference of the utilisation-aware engine (capi.IFCLASS_DTYPE records from HorusEngine.interference):
+`interference_derived` gives per class scheduler_analysis.ipynb's "Degrade_Only" line (mean, median and sample std of
+the jct of the jobs co-location slowed, actual > original) and its "normal" line (the same of actual_duration over
+every finished job, in ticks), the share of jobs degraded, their mean excess, the GPU time they lost, the share
+preempted more than once, and jobdist's numbers of the degraded and the clean jobs; `interference_spread` their spread
+per class over runs (seeded repeats) that have jobs in it.
+
 Time-weighted occupancy (capi.OCC_DTYPE records and histograms from Engine.occupancy / HorusEngine.occupancy):
 `occupancy_derived` gives the time-weighted GPU share, the shares of time saturated and with jobs waiting, the GPU
 time left idle while jobs waited, mean running and queued jobs, busy-GPU points over all time and over waiting time,
@@ -428,6 +435,93 @@ def slowdown_spread_columns():
 
 def slowdown_spread_flat(sp, c):
     return [float(sp[name][s][c]) for name in SLOWDOWN_METRICS for s in SPREAD_STATS]
+
+
+# ---------------------------------------------------------------- interference (utilisation-aware engine)
+IF_ONE = 1024                                             # fixed-point units per tick
+IF_COUNTS = ("jobs", "degraded", "preempted_jobs", "clamped")
+IF_NOTEBOOK = ("degraded_jct_mean", "degraded_jct_median", "degraded_jct_std", "actual_mean", "actual_median", "actual_std")
+IF_METRICS = (IF_NOTEBOOK + ("degraded_share", "excess_mean", "lost_gpu_time", "preempted_share")
+              + tuple(f"{g}_{m}" for g in ("degraded", "clean") for m in JOBDIST_METRICS if f"{g}_{m}" not in IF_NOTEBOOK))
+
+
+def _ifclass_numbers(rec):
+    """the IF_COUNTS and IF_METRICS of one IFCLASS_DTYPE record (durations in ticks: the fixed point over 1024, an
+    exact division; NaN where a group is empty; std NaN below two jobs).  Means and sample variances are exact in
+    Python ints and rounded once."""
+    kd, kc = int(rec["degraded"]["jobs"]), int(rec["clean"]["jobs"])
+    n = kd + kc
+    out = dict(jobs=n, degraded=kd, preempted_jobs=int(rec["preempted_jobs"]), clamped=int(rec["clamped"]))
+    deg, cln = _jclass_numbers(rec["degraded"]), _jclass_numbers(rec["clean"])
+    out["degraded_jct_mean"], out["degraded_jct_std"] = deg["jct_mean"], deg["jct_std"]
+    out["degraded_jct_median"] = sum(int(v) for v in rec["degraded_jct_mid"]) / 2 if kd else math.nan
+    s, sq = int(rec["actual_sum"]), u128(rec["actual_sq_lo"], rec["actual_sq_hi"])
+    out["actual_mean"] = s / (n * IF_ONE) if n else math.nan
+    out["actual_median"] = sum(int(v) for v in rec["actual_mid"]) / (2 * IF_ONE) if n else math.nan
+    out["actual_std"] = math.sqrt(float(Fraction(n * sq - s * s, n * (n - 1)))) / IF_ONE if n > 1 else math.nan
+    lost = u128(rec["lost_gpu_time_lo"], rec["lost_gpu_time_hi"])
+    out["degraded_share"] = kd / n if n else math.nan
+    out["excess_mean"] = int(rec["excess_sum"]) / (kd * IF_ONE) if kd else math.nan
+    out["lost_gpu_time"] = lost / IF_ONE if n else math.nan
+    out["preempted_share"] = int(rec["preempted_jobs"]) / n if n else math.nan
+    for g, d in (("degraded", deg), ("clean", cln)):
+        for m in JOBDIST_METRICS:
+            out.setdefault(f"{g}_{m}", d[m])
+    return out
+
+
+def interference_derived(recs):
+    """Per class of one replica: `recs` IFCLASS_DTYPE (C,).  Returns {count: int array (C,) for every IF_COUNTS entry,
+    metric: float array (C,) for every IF_METRICS entry}.  degraded_jct_mean / _median / _std are the notebook's
+    "Degrade_Only" jct.mean() / .median() / .std() and actual_mean / _median / _std its "normal" actual_duration ones
+    (to within 2^-11 tick: the durations are kept in units of 2^-10)."""
+    recs = np.asarray(recs)
+    if recs.ndim != 1:
+        raise ValueError("interference_derived: expected IFCLASS_DTYPE records (C,)")
+    nums = [_ifclass_numbers(rec) for rec in recs]
+    out = {k: np.array([d[k] for d in nums], dtype=np.int64) for k in IF_COUNTS}
+    for name in IF_METRICS:
+        out[name] = np.array([d[name] for d in nums], dtype=np.float64)
+    return out
+
+
+def interference_spread(recs, level=0.95):
+    """Spread per class across runs (e.g. seeded repeats of one configuration): `recs` (runs, C).  For every class,
+    over the runs that have at least one finished job in it: {"replicas": int array (C,), metric: {mean, std, lo, hi:
+    float arrays (C,)} for every IF_METRICS entry}, with spread's rules (sample std, nearest-rank interval holding the
+    central `level`, NaN where a value is NaN for any of those runs or no run has jobs in the class)."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    recs = np.asarray(recs)
+    if recs.ndim != 2:
+        raise ValueError("interference_spread: expected recs (runs, C)")
+    per = [interference_derived(recs[r]) for r in range(recs.shape[0])]
+    reach = (recs["degraded"]["jobs"] + recs["clean"]["jobs"]) > 0
+    out = {"replicas": reach.sum(axis=0).astype(np.int64)}
+    for name in IF_METRICS:
+        cols = [_spread_of(np.array([d[name][c] for r, d in enumerate(per) if reach[r, c]], dtype=np.float64), level)
+                for c in range(recs.shape[1])]
+        out[name] = {s: np.array([col[s] for col in cols], dtype=np.float64) for s in SPREAD_STATS}
+    return out
+
+
+def interference_columns():
+    """names of the flat per-class columns `interference_flat` returns, in order"""
+    return list(IF_COUNTS) + list(IF_METRICS)
+
+
+def interference_flat(d, c):
+    """class c of an interference_derived dict as a list of Python values"""
+    return [int(d[k][c]) for k in IF_COUNTS] + [float(d[name][c]) for name in IF_METRICS]
+
+
+def interference_spread_columns():
+    return [f"{name}_{s}" for name in IF_METRICS for s in SPREAD_STATS]
+
+
+def interference_spread_flat(sp, c):
+    return [float(sp[name][s][c]) for name in IF_METRICS for s in SPREAD_STATS]
 
 
 # ---------------------------------------------------------------- time-weighted occupancy

@@ -257,6 +257,14 @@ def _occ_pitch(flag_sets):
     return pitch
 
 
+def check_interference(bounds):
+    """the class bounds of an interference argument as a tuple of ints, or ValueError (jobdist's rules)"""
+    try:
+        return check_jobdist((bounds, ()))[0]
+    except ValueError as e:
+        raise ValueError(f"interference: {str(e).split(': ', 1)[1]}") from None
+
+
 DEFAULT_DIFF_EDGES = tuple(-2 ** i for i in range(30, -1, -1)) + (0,) + tuple(2 ** i for i in range(31))
 
 
@@ -292,7 +300,7 @@ def _compare_in(eng, pairs, members, bounds, edges):
 
 
 def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None, compare=None, slowdown=None,
-                      occupancy=None):
+                      occupancy=None, interference=None):
     """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
     same configurations and random streams as run_batched, but no row or job record is read back and nothing is
     written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus.
@@ -308,7 +316,13 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
     (len(flag_sets), C, 3 * (E + 1) + Esd + 1)) after the jobdist element (before the compare element).
     occupancy=queue edges: also compute every replica's time-weighted occupancy on the device (gs_set_occupancy) and
     append (OCC_DTYPE records (len(flag_sets),), busy histograms (len(flag_sets), 2, P), queue histograms
-    (len(flag_sets), E + 1)) as the last element, P the largest M * G of the configurations plus 1."""
+    (len(flag_sets), E + 1)) as the last element, P the largest M * G of the configurations plus 1.
+    interference=class bounds: also compute the interference statistics of every utilisation-aware replica on the
+    device (gs_horus_set_interference) and append IFCLASS_DTYPE records (len(flag_sets), C) as the last element (after
+    the occupancy element); the rows of the other configurations are zero."""
+    if interference is not None:
+        if_bounds = check_interference(interference)
+        if_recs = np.zeros((len(flag_sets), len(if_bounds) + 1), dtype=capi.IFCLASS_DTYPE)
     if occupancy is not None:
         occ_edges = check_occupancy(occupancy)
         occ_recs = np.zeros(len(flag_sets), dtype=capi.OCC_DTYPE)
@@ -346,7 +360,11 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 eng.set_slowdown(*sd)
             if occupancy is not None:
                 eng.set_occupancy(occ_edges)
+            if interference is not None:
+                eng.set_interference(if_bounds)
             out[aware] = eng.summarize()
+            if interference is not None:
+                if_recs[aware] = eng.interference()
             if occupancy is not None:
                 occ_recs[aware], ob, occ_q[aware] = eng.occupancy()
                 occ_busy[aware, :, :ob.shape[2]] = ob
@@ -386,7 +404,7 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 cmp_recs[sel], cmp_hist[sel] = _compare_in(eng, [pairs[k] for k in sel], plain, cmp_bounds, cmp_edges)
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
            + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ())
-           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()))
+           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()) + ((if_recs,) if interference is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -724,6 +742,40 @@ def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, l
                 for c in range(cl.shape[1]):
                     w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [c]
                                + _class_range(c, bounds) + [int(sp["replicas"][c]), level] + summary.jobdist_spread_flat(sp, c))
+
+
+def write_interference_csv(path, flag_sets, recs, bounds):
+    """one line per (utilisation-aware configuration, class): the flags, the class, its num_gpu range and
+    summary.interference_derived's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["class", "gpus_min", "gpus_max"] + summary.interference_columns())
+        for fl, rc in zip(flag_sets, recs):
+            if not _is_utilisation_aware(fl):
+                continue
+            d = summary.interference_derived(rc)
+            for c in range(len(rc)):
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, c] + _class_range(c, bounds)
+                           + summary.interference_flat(d, c))
+
+
+def write_interference_ci_csv(path, flag_sets, repeats, recs, bounds, level=0.95):
+    """one line per (utilisation-aware configuration, class) over its `repeats` seeded repeats (flag_sets[i * repeats
+    + rep]): the flags with the first repeat's seed, the repeat count, the class, its num_gpu range, the number of
+    repeats with jobs in it and summary.interference_spread's columns"""
+    import csv
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["repeats", "class", "gpus_min", "gpus_max", "replicas", "level"] + summary.interference_spread_columns())
+        for i in range(0, len(flag_sets), repeats):
+            fl = flag_sets[i]
+            if not _is_utilisation_aware(fl):
+                continue
+            sp = summary.interference_spread(recs[i:i + repeats], level=level)
+            for c in range(recs.shape[1]):
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, repeats, c]
+                           + _class_range(c, bounds) + [int(sp["replicas"][c]), level] + summary.interference_spread_flat(sp, c))
 
 
 def write_jobdist_cdf_csv(path, flag_sets, classes, hist, bounds, edges):
@@ -1080,7 +1132,25 @@ def main(argv=None):
                     help="with --occupancy: one CSV line per (configuration[, load], quantity, point): the time share with at most "
                          "b busy GPUs for every b, over all time and over the time with jobs queued, and with a queue length at "
                          "most each queue edge")
+    ap.add_argument("--interference", default=None, metavar="FILE",
+                    help="with --summary: also compute the interference statistics of the utilisation-aware configurations "
+                         "(horus, horus+, gandiva) on the GPU -- the jobs co-location slowed (actual > original duration), their "
+                         "jct, the actual durations, the GPU time lost -- and write one CSV line per (configuration, seed, class) "
+                         "to FILE.  Classes: --gpu-classes")
+    ap.add_argument("--interference-ci", default=None, metavar="FILE",
+                    help="with --interference and --repeats R >= 2: one CSV line per (configuration, class) with the spread of "
+                         "the interference numbers over the R seeded repeats")
     a = ap.parse_args(argv)
+    interference = None
+    if a.interference is not None:
+        if not a.summary:
+            ap.error("--interference needs --summary FILE")
+        try:
+            interference = check_interference(a.gpu_classes or ())
+        except ValueError as e:
+            ap.error(str(e))
+    if a.interference_ci is not None and (a.interference is None or a.repeats < 2):
+        ap.error("--interference-ci needs --interference FILE and --repeats R >= 2")
     occupancy = None
     if a.occupancy is not None:
         if not a.summary:
@@ -1114,9 +1184,9 @@ def main(argv=None):
         except ValueError as e:
             ap.error(str(e))
     elif ((a.cdf_edges is not None and a.slowdown is None) or a.jobdist_cdf is not None
-          or (a.gpu_classes is not None and a.paired is None)):
-        ap.error("--gpu-classes, --cdf-edges and --jobdist-cdf need --jobdist FILE (--gpu-classes: or --paired FILE; "
-                 "--cdf-edges: or --slowdown FILE)")
+          or (a.gpu_classes is not None and a.paired is None and a.interference is None)):
+        ap.error("--gpu-classes, --cdf-edges and --jobdist-cdf need --jobdist FILE (--gpu-classes: or --paired FILE or "
+                 "--interference FILE; --cdf-edges: or --slowdown FILE)")
     if a.compare is None:
         if a.paired is not None or a.paired_cdf is not None or a.diff_edges is not None or a.paired_summary is not None:
             ap.error("--paired, --paired-cdf, --diff-edges and --paired-summary need --compare BASE")
@@ -1167,6 +1237,8 @@ def main(argv=None):
                                        num_node_p_switch=a.num_node_p_switch, num_queue=a.num_queue, num_buffer=a.num_buffer,
                                        log_path=os.path.join(f"batched_{tag}", f"{scheme}_{sc}"),
                                        seed=a.seed if a.seed < 0 else a.seed + rep))
+    if interference is not None and not any(_is_utilisation_aware(fl) for fl in sets):
+        ap.error("--interference: no configuration runs on the utilisation-aware engine (--schedule horus, horus+ or gandiva)")
     compare = None
     if a.compare is not None:
         pairs, S, R = [], len(a.schedule), a.repeats
@@ -1229,9 +1301,16 @@ def main(argv=None):
               + (f" x {len(mix_text)} mixes" if mix_text else "") + f" x {a.bootstrap} replicas")
         return
     if a.summary:
-        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare, slowdown=slowdown, occupancy=occupancy)
+        res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare, slowdown=slowdown, occupancy=occupancy,
+                                interference=interference)
         recs, rest = (res, ()) if (timeline is None and jobdist is None and compare is None and slowdown is None
-                                   and occupancy is None) else (res[0], res[1:])
+                                   and occupancy is None and interference is None) else (res[0], res[1:])
+        if interference is not None:
+            irec = rest[-1]
+            rest = rest[:-1]
+            write_interference_csv(a.interference, sets, irec, interference)
+            if a.interference_ci:
+                write_interference_ci_csv(a.interference_ci, sets, a.repeats, irec, interference)
         if occupancy is not None:
             orec, obusy, oq = rest[-1]
             rest = rest[:-1]

@@ -119,6 +119,51 @@ int gs_horus_fetch_slowdown(gs_horus_handle h, int32_t first, int32_t count, gs_
 int gs_horus_set_occupancy(gs_horus_handle h, int32_t on, int32_t nedges, const int32_t *edges);
 int gs_horus_fetch_occupancy(gs_horus_handle h, int32_t first, int32_t count, gs_occ *out, uint64_t *busy_hist, int32_t busy_pitch,
                              uint64_t *queue_hist);
+/* ---- interference statistics (interference) -------------------------------------------------------------------
+ * The jobs are jobdist's: the finished jobs of gs_summary's job part, classed by jobdist's C - 1 bounds on num_gpu
+ * (1 <= C <= GS_JOBDIST_MAX_CLASSES, the same rules).  A job is DEGRADED when actual > original (its gs_horus_job_rec,
+ * compared as doubles): co-location stretched its longest task.  Every other finished job is clean.
+ * Durations are kept in fixed point, units of 2^-10 tick: fp(x) = min(2^31 - 1, max(0, round(1024 * x))), rounded to
+ * nearest with ties to even.  a = fp(actual) and o = fp(original) for every job; e = fp(actual - original), the
+ * difference taken in IEEE double, for a degraded job.  The rounding makes the reference's interference penalty of 5
+ * ticks, which reaches the records as 4.999999999999998 or 5.0, one value (e = 5120).  `clamped` counts the jobs with a
+ * value that saturated (or was NaN).  Per class one gs_ifclass, every field an integer (a repeated call gives the
+ * same bytes):
+ *   degraded, clean      jobdist's gs_jclass restricted to each group (degraded + clean = gs_horus_fetch_jobdist's
+ *                        record under the same bounds, for counts and sums)
+ *   degraded_jct_mid     the degraded jobs' jct at ranks floor((k - 1) / 2) and ceil((k - 1) / 2) (the median is
+ *                        their mean; [0] equals degraded.jct_q[0])
+ *   actual_*             a over the class's finished jobs: sum, 128-bit sum of squares, gs_summary's 50 / 90 / 95 /
+ *                        99 / 100 % and the two middle order statistics
+ *   original_sum         sum of o
+ *   excess_*, lost_gpu_time_*   over the degraded jobs: sum and maximum of e, 128-bit sum of gpus * e
+ *   preempted_jobs, preempt_max jobs with preempt > 1 (gandiva's time slicing) and the largest preempt
+ * Order statistics and maxima are 0 for an empty group. */
+typedef struct gs_ifclass {
+  gs_jclass degraded, clean;
+  int64_t actual_sum;
+  uint64_t actual_sq_lo, actual_sq_hi;
+  int64_t original_sum;
+  int64_t excess_sum;
+  uint64_t lost_gpu_time_lo, lost_gpu_time_hi;
+  int64_t preempted_jobs;
+  int64_t clamped;
+  int32_t degraded_jct_mid[2];
+  int32_t actual_q[5];
+  int32_t actual_mid[2];
+  int32_t excess_max;
+  int32_t preempt_max;
+  int32_t reserved;
+} gs_ifclass;                        /* 440 bytes */
+/* gs_horus_set_interference: while nclasses > 0, every gs_horus_summarize also computes the class records of the
+ * replicas it summarises; nclasses = 0 (the default) turns it off.  Every replica is marked as not summarised with
+ * this setting.  GS_ERR_ARG for nclasses outside 0..8, bounds that are not strictly increasing or below 1, or NULL
+ * bounds with nclasses > 1; nothing changes on an error.
+ * gs_horus_fetch_interference copies count * C records (replica-major) as of the last gs_horus_summarize.  GS_ERR_ARG
+ * for a bad range or a NULL output, GS_ERR_STATE when the feature is off or a replica has not been summarised with
+ * this setting since it was prepared.                                                                          */
+int gs_horus_set_interference(gs_horus_handle h, int32_t nclasses, const int32_t *bounds);
+int gs_horus_fetch_interference(gs_horus_handle h, int32_t first, int32_t count, gs_ifclass *out);
 /* Paired per-job comparison (gs_jpair, gsched.h: gs_compare) of replicas of this handle that hold the same trace: equal
  * arrival, gpus, gpu_per_container, duration, memory, utilisation and mean-memory fields for every job.  The same
  * outputs, launches and errors as gs_compare; a replica has run once gs_horus_run has prepared it.           */
