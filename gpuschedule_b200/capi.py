@@ -145,6 +145,10 @@ JOBIN_DTYPE = np.dtype([("arrive_tick", "<i4"), ("gpus", "<i4"), ("gpu_per_task"
 # gs_boot_params (include/gsched.h): one bootstrap replica -- Philox key (seed, stream), jobs, gap scale gap_num / gap_den
 BOOT_PARAMS_DTYPE = np.dtype([("seed", "<u8"), ("stream", "<u8"), ("n", "<i8"), ("gap_num", "<i4"), ("gap_den", "<i4")])
 assert BOOT_PARAMS_DTYPE.itemsize == 32
+# gs_boot_seg (include/gsched.h): one segment of a load profile -- start tick, gap scale gap_num / gap_den, reserved 0
+BOOT_SEG_DTYPE = np.dtype([("start", "<i4"), ("gap_num", "<i4"), ("gap_den", "<i4"), ("reserved", "<i4")])
+assert BOOT_SEG_DTYPE.itemsize == 16
+BOOT_MAX_SEGMENTS = 64
 NODE_DTYPE = np.dtype([("busy_mask", "<u8"), ("cpu_used", "<i4"), ("mem_used", "<i4")])
 JOBREQ_DTYPE = np.dtype([("gpus", "<i4"), ("gpu_per_task", "<i4"), ("mem_bytes", "<i8")])
 
@@ -321,6 +325,9 @@ def load_library():
     lib.gs_boot_traces_blocked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, f64p]
     lib.gs_boot_mixes.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     lib.gs_boot_traces_mixed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, f64p]
+    lib.gs_boot_profiles.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.gs_boot_traces_profiled.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, f64p]
+    lib.gs_boot_profiles.restype = lib.gs_boot_traces_profiled.restype = C.c_int
     lib.gs_fetch_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.gs_set_timeline.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
     lib.gs_fetch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
@@ -888,13 +895,33 @@ class Engine:
         w = np.ascontiguousarray(w, dtype=np.uint32)
         self._check(self.lib.gs_boot_mixes(self.h, len(w), w.ctypes.data_as(C.c_void_p)), "gs_boot_mixes")
 
-    def boot_traces(self, params, with_time=False, block_len=None, mix=None):
+    def boot_profiles(self, profiles):
+        """the load profiles of the handle (gs_boot_profiles): a list of (segments, period), segments being
+        BOOT_SEG_DTYPE records or (start, gap_num, gap_den) triples; an empty list clears them"""
+        from .tracegen import check_profile
+        segs, nseg, period = [], [], []
+        for prof in profiles:
+            t, num, den, P = check_profile(*prof)
+            segs += [(a, b, c, 0) for a, b, c in zip(t, num, den)]
+            nseg.append(len(t))
+            period.append(P)
+        if not nseg:
+            self._check(self.lib.gs_boot_profiles(self.h, 0, None, None, None), "gs_boot_profiles")
+            return
+        S = np.array(segs, dtype=np.int64).astype(np.int32).view(BOOT_SEG_DTYPE).reshape(-1)
+        N, P = np.array(nseg, dtype=np.int32), np.array(period, dtype=np.int32)
+        self._check(self.lib.gs_boot_profiles(self.h, len(N), N.ctypes.data_as(C.c_void_p), P.ctypes.data_as(C.c_void_p),
+                                              S.ctypes.data_as(C.c_void_p)), "gs_boot_profiles")
+
+    def boot_traces(self, params, with_time=False, block_len=None, mix=None, profile=None):
         """draw every replica's trace from the population: `params` holds one BOOT_PARAMS_DTYPE record per replica.
         block_len: the mean block length L of a block bootstrap (gs_boot_traces_blocked), one integer for every
         replica or one per replica; None draws iid replicas (gs_boot_traces).  mix: the job mix of boot_mixes each
         replica draws its rows from (gs_boot_traces_mixed), one index for every replica or one per replica, -1 for
-        the unweighted bootstrap; None draws every replica unweighted.  with_time: returns the generator's kernel
-        milliseconds"""
+        the unweighted bootstrap; None draws every replica unweighted.  profile: the load profile of boot_profiles
+        each replica takes its arrivals from (gs_boot_traces_profiled; a profiled replica's gap scale must be 1 / 1),
+        one index for every replica or one per replica, -1 for none; None profiles no replica.  with_time: returns the
+        generator's kernel milliseconds"""
         params = np.ascontiguousarray(params, dtype=BOOT_PARAMS_DTYPE)
         if params.shape != (self.nsims,):
             raise ValueError(f"boot_traces: one parameter record per replica ({self.nsims}), got shape {params.shape}")
@@ -909,6 +936,16 @@ class Engine:
             if M.dtype.kind not in "iu" or M.shape not in ((), (self.nsims,)) or (M < -2 ** 31).any() or (M > 2 ** 31 - 1).any():
                 raise ValueError(f"boot_traces: mix must be one int32 or one per replica ({self.nsims})")
             M = np.ascontiguousarray(np.broadcast_to(M, (self.nsims,)), dtype=np.int32)
+        if profile is not None:
+            Q = np.asarray(profile)
+            if Q.dtype.kind not in "iu" or Q.shape not in ((), (self.nsims,)) or (Q < -2 ** 31).any() or (Q > 2 ** 31 - 1).any():
+                raise ValueError(f"boot_traces: profile must be one int32 or one per replica ({self.nsims})")
+            Q = np.ascontiguousarray(np.broadcast_to(Q, (self.nsims,)), dtype=np.int32)
+            self._check(self.lib.gs_boot_traces_profiled(self.h, params.ctypes.data_as(C.c_void_p),
+                                                         None if block_len is None else L.ctypes.data_as(C.c_void_p),
+                                                         None if mix is None else M.ctypes.data_as(C.c_void_p),
+                                                         Q.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces_profiled")
+        elif mix is not None:
             self._check(self.lib.gs_boot_traces_mixed(self.h, params.ctypes.data_as(C.c_void_p),
                                                       None if block_len is None else L.ctypes.data_as(C.c_void_p),
                                                       M.ctypes.data_as(C.c_void_p), C.byref(ms)), "gs_boot_traces_mixed")

@@ -36,6 +36,16 @@
 // (0 for other jobs), carried between chunks like the gap sum, so each job reads b_j and s_{b_j} from its scanned key
 // however many chunks and wraps of the population its block spans.  The mixed instantiations (MIXED = true) read a
 // replica's table offset and T from one extra per-replica record and load one 16-byte table entry per job.
+//
+// Profiled replicas (gs_boot_profiles / gs_boot_traces_profiled) keep every draw above and move only the arrivals: a
+// profile of m segments {t_k, num_k, den_k} and period P becomes, on the host and exactly, base-time starts
+//   s_0 = 0, s_(k+1) = s_k + ceil((t_(k+1) - t_k) * den_k / num_k), B = s_m with t_m := P (P > 0 only)
+// and job j with gap sum S arrives at
+//   a(S) = t_k + floor((S - s_k) * num_k / den_k), k the last segment with s_k <= S    (P = 0)
+//   (S div B) * P + a(S mod B)                                                        (P > 0)
+// The profiled instantiations load their replica's segments into shared memory once and find each job's segment by
+// binary search after the gap scan (gs_boot_profile_seg / gs_boot_profile_arrive, which the host also uses for the
+// arrival bound).
 #pragma once
 
 #include <stdint.h>
@@ -180,6 +190,71 @@ GS_BOOT_HD long long gs_boot_arrive_bound(long long n, long long max_gap, int ga
   return x > (__int128)0x7fffffffffffffffll ? 0x7fffffffffffffffll : (long long)x;
 }
 
+// One segment of a profile in device form: base-time start s, real start t and gap scale num / den.
+struct GsBootProfSeg {
+  long long s;
+  int t, num, den, reserved;
+};
+
+// Why the profile of m segments seg[] with period P breaks the rules of gs_boot_profiles (include/gsched.h), or
+// nullptr when it keeps them.
+static inline const char *gs_boot_profile_invalid(const gs_boot_seg *seg, int m, int P) {
+  if (m < 1 || m > GS_BOOT_MAX_SEGMENTS) return "nseg must be in 1..GS_BOOT_MAX_SEGMENTS";
+  if (seg[0].start != 0) return "the first segment must start at tick 0";
+  for (int k = 0; k < m; ++k) {
+    if (k > 0 && seg[k].start <= seg[k - 1].start) return "segment starts must be strictly increasing";
+    if (seg[k].start >= 0x7fffffff) return "segment starts must be below 2^31 - 1";
+    if (seg[k].gap_num < 1 || seg[k].gap_den < 1) return "every gap scale needs gap_num >= 1 and gap_den >= 1";
+  }
+  if (P < 0) return "the period must be >= 0";
+  if (P > 0 && P <= seg[m - 1].start) return "a period must exceed the last segment's start";
+  return nullptr;
+}
+
+// The device form out[m] of a valid profile (seg[m], period P): s_0 = 0, s_(k+1) = s_k + ceil((t_(k+1) - t_k) *
+// den_k / num_k).  Returns B = s_m with t_m := P, the base length of one period, or 0 when P = 0.  Every s_k and B
+// stay below 2^62 + 64: the t_k differences add up to less than 2^31 and each den_k is below 2^31.
+static inline long long gs_boot_profile_base(const gs_boot_seg *seg, int m, int P, GsBootProfSeg *out) {
+  long long s = 0;
+  for (int k = 0; k < m; ++k) {
+    out[k].s = s; out[k].t = seg[k].start; out[k].num = seg[k].gap_num; out[k].den = seg[k].gap_den; out[k].reserved = 0;
+    if (k + 1 < m || P > 0) {
+      const long long d = (long long)((k + 1 < m ? seg[k + 1].start : P) - seg[k].start);
+      s += (d * seg[k].gap_den + seg[k].gap_num - 1) / seg[k].gap_num;
+    }
+  }
+  return P > 0 ? s : 0;
+}
+
+// The last of the m segments with s <= x (x >= 0; s_0 = 0), by binary search.
+template <class I>
+GS_BOOT_HD int gs_boot_profile_seg(const GsBootProfSeg *seg, int m, I x) {
+  int lo = 0, hi = m;                                  // seg[lo].s <= x < seg[hi].s, seg[m].s = infinity
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if ((I)seg[mid].s <= x) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// Arrival tick of base time S >= 0 under a profile (seg[m], period P, base period B; P = 0: aperiodic).  I = long long
+// on the device, where the caller's bound keeps (S - s_k) * num_k below 2^62; __int128 on the host for that bound.
+template <class I>
+GS_BOOT_HD I gs_boot_profile_arrive(const GsBootProfSeg *seg, int m, int P, long long B, I S) {
+  I q = 0;
+  if (P > 0) { q = S / (I)B; S -= q * (I)B; }
+  const GsBootProfSeg &g = seg[gs_boot_profile_seg(seg, m, S)];
+  return q * (I)P + (I)g.t + (S - (I)g.s) * (I)g.num / (I)g.den;
+}
+
+// Largest arrival tick any profiled replica of n jobs can reach: arrive((n - 1) * max_gap), exactly; saturated at
+// 2^63 - 1.
+static inline long long gs_boot_profile_bound(const GsBootProfSeg *seg, int m, int P, long long B, long long n, long long max_gap) {
+  if (n <= 1) return 0;
+  const __int128 x = gs_boot_profile_arrive<__int128>(seg, m, P, B, (__int128)(n - 1) * max_gap);
+  return x > (__int128)0x7fffffffffffffffll ? 0x7fffffffffffffffll : (long long)x;
+}
+
 #ifdef __CUDACC__
 namespace {
 
@@ -195,6 +270,18 @@ struct alignas(16) GsBootMix {   // one replica's alias table as the mixed insta
   long long off;                 // first entry of the replica's table in tabs
 };
 
+struct GsBootProf {              // one replica's profile as the profiled instantiations read it
+  long long B;                   // base length of one period (0: aperiodic)
+  int period, off, nseg;         // period P, first segment in segs, segments (0: unprofiled, profile -1)
+  int reserved;
+};
+
+// The I-th argument of a pack.
+template <int I, class T, class... Ts>
+static __device__ __forceinline__ auto gs_boot_nth(T a, Ts... rest) {
+  if constexpr (I == 0) return a; else return gs_boot_nth<I - 1>(rest...);
+}
+
 // gs_boot_pick_mixed of job j of this block's replica, whose table is {T, off} = mixes[blockIdx.x] (T = 0: mix -1).
 static __device__ __forceinline__ bool gs_boot_pick_in_mix(const GsBootMix *mixes, const GsBootAlias *tabs, uint64_t seed, uint64_t stream,
                                                            long long j, long long K, uint64_t L, long long &row, long long &gap) {
@@ -205,20 +292,32 @@ static __device__ __forceinline__ bool gs_boot_pick_in_mix(const GsBootMix *mixe
 // out[2 b] = sum over the jobs of min(tasks, M), out[2 b + 1] = last arrival tick (0 without jobs).
 // BLOCKED = false is the iid bootstrap; BLOCKED = true draws blocks of mean length R.block_len (1 gives the iid trace).
 // MIXED = true picks rows (block starts when blocked) through the alias table {T, off} = mixes[b] at tabs + off, two
-// parameters appended as the pack `mix` = (const GsBootMix *mixes, const GsBootAlias *tabs).  The other
-// instantiations have an empty pack: their parameter list, and so their code, is the one they had before mixes.
+// parameters appended as the pack `mix` = (const GsBootMix *mixes, const GsBootAlias *tabs).  The profiled
+// instantiations append (const GsBootProf *profs, const GsBootProfSeg *segs) to the pack, after the mixed pair when MIXED:
+// replica b's arrivals follow the profs[b].nseg segments at segs + profs[b].off (none: the gap scale as before).  The
+// other instantiations have an empty pack: their parameter list, and so their code, is the one they had before mixes.
 template <bool BLOCKED, bool MIXED, class... Mix>
 __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRep *reps, const JobIn *pop, const int *gaps, long long K,
                                                                  JobIn *arena, long long stride_recs, long long *out, Mix... mix) {
-  static_assert(sizeof...(Mix) == (MIXED ? 2 : 0), "the mixed instantiations take (mixes, tabs)");
+  constexpr bool PROFILED = sizeof...(Mix) == (MIXED ? 4 : 2);
+  static_assert(sizeof...(Mix) == (MIXED ? 2 : 0) + (PROFILED ? 2 : 0),
+                "the mixed instantiations take (mixes, tabs), the profiled ones (profs, segs) after them");
   __shared__ int4 stage[2 * GS_BOOT_THREADS];
   __shared__ long long warp_tot[GS_BOOT_THREADS / 32];
   __shared__ long long warp_key[BLOCKED ? GS_BOOT_THREADS / 32 : 1];
   __shared__ long long red[2][GS_BOOT_THREADS / 32];
+  __shared__ GsBootProfSeg pseg[PROFILED ? GS_BOOT_MAX_SEGMENTS : 1];
   const GsBootRep R = reps[blockIdx.x];
   int4 *dst = reinterpret_cast<int4 *>(arena + stride_recs * (long long)blockIdx.x);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   long long carry = 0, spans = 0, last = 0, key_carry = 0;
+  [[maybe_unused]] GsBootProf prof{};
+  if constexpr (PROFILED) {                            // the replica's segments, once
+    prof = gs_boot_nth<MIXED ? 2 : 0>(mix...)[blockIdx.x];
+    const GsBootProfSeg *segs = gs_boot_nth<MIXED ? 3 : 1>(mix...) + prof.off;
+    for (int k = threadIdx.x; k < prof.nseg; k += blockDim.x) pseg[k] = segs[k];
+    __syncthreads();
+  }
   for (long long j0 = 0; j0 < R.n; j0 += blockDim.x) {
     const long long j = j0 + threadIdx.x;
     const bool in = j < R.n;
@@ -229,7 +328,7 @@ __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRe
       bool start = false;
       if (in) {
         if constexpr (MIXED) {
-          start = gs_boot_pick_in_mix(mix..., R.seed, R.stream, j, K, R.block_len, s, gi);
+          start = gs_boot_pick_in_mix(gs_boot_nth<0>(mix...), gs_boot_nth<1>(mix...), R.seed, R.stream, j, K, R.block_len, s, gi);
         } else {
           start = gs_boot_pick_blocked(R.seed, R.stream, j, K, R.block_len, s, gi);
         }
@@ -255,7 +354,7 @@ __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRe
     } else if (in) {
       long long row, gi;
       if constexpr (MIXED) {
-        gs_boot_pick_in_mix(mix..., R.seed, R.stream, j, K, 1u, row, gi);
+        gs_boot_pick_in_mix(gs_boot_nth<0>(mix...), gs_boot_nth<1>(mix...), R.seed, R.stream, j, K, 1u, row, gi);
       } else {
         gs_boot_pick(R.seed, R.stream, j, K, row, gi);
       }
@@ -275,7 +374,13 @@ __global__ void __launch_bounds__(GS_BOOT_THREADS) gs_boot_kernel(const GsBootRe
     for (int w = 0; w < nwarps; ++w) { const long long t = warp_tot[w]; before += w < warp ? t : 0; chunk += t; }
     carry += chunk;
     if (in) {
-      const int arrive = gs_boot_arrive(before + x, R.gap_num, R.gap_den);
+      int arrive;
+      if constexpr (PROFILED) {
+        arrive = prof.nseg > 0 ? (int)gs_boot_profile_arrive<long long>(pseg, prof.nseg, prof.period, prof.B, before + x)
+                               : gs_boot_arrive(before + x, R.gap_num, R.gap_den);
+      } else {
+        arrive = gs_boot_arrive(before + x, R.gap_num, R.gap_den);
+      }
       const long long tasks = lo.y / lo.z;
       spans += tasks < R.M ? tasks : R.M;
       last = arrive;                                   // arrivals do not decrease: the thread's latest job is its largest

@@ -139,6 +139,9 @@ struct gs_engine {
   void *d_pop = nullptr; int64_t pop_k = 0; int64_t pop_max_gap = 0; double pop_max_need = 1.0;
   // gs_boot_mixes: nmix alias tables of pop_k entries each, mix-major, and their weight sums
   GsBootAlias *d_mix = nullptr; int32_t nmix = 0; std::vector<uint64_t> mix_T;
+  // gs_boot_profiles: the device form of nprof profiles, profile-major, with a host copy for the arrival bound
+  GsBootProfSeg *d_prof = nullptr; int32_t nprof = 0;
+  std::vector<GsBootProfSeg> prof_seg; std::vector<int32_t> prof_off, prof_nseg, prof_period; std::vector<long long> prof_B;
 };
 
 static std::string g_create_err;
@@ -226,6 +229,7 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->d_occ_q) cudaFree(h->d_occ_q);
   if (h->d_pop) cudaFree(h->d_pop);
   if (h->d_mix) cudaFree(h->d_mix);
+  if (h->d_prof) cudaFree(h->d_prof);
   for (int q = 0; q < GS_MAX_RANKS; ++q) if (h->comm_opened[q] && h->comm_peer[q]) cudaIpcCloseMemHandle(h->comm_peer[q]);
   if (h->comm_buf) cudaFree(h->comm_buf);
   if (h->e0) cudaEventDestroy(h->e0);
@@ -1615,6 +1619,46 @@ extern "C" int gs_boot_traces_blocked(gs_handle h, const gs_boot_params *params,
 
 extern "C" int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params, const uint32_t *block_len, const int32_t *mix,
                                     double *kernel_ms) {
+  return gs_boot_traces_profiled(h, params, block_len, mix, nullptr, kernel_ms);
+}
+
+extern "C" int gs_boot_profiles(gs_handle h, int32_t nprof, const int32_t *nseg, const int32_t *period, const gs_boot_seg *segs) {
+  if (!h) return GS_ERR_ARG;
+  if (nprof < 0) return fail(h, GS_ERR_ARG, "gs_boot_profiles: nprof must be >= 0");
+  if (nprof > 0 && (!nseg || !period || !segs)) return fail(h, GS_ERR_ARG, "gs_boot_profiles: NULL array");
+  // every check before anything changes: a refused call leaves the profiles as they were
+  std::vector<int32_t> off((size_t)nprof);
+  size_t total = 0;
+  for (int32_t p = 0; p < nprof; ++p) {
+    const char *why = gs_boot_profile_invalid(segs + total, nseg[p], period[p]);
+    if (why) return fail(h, GS_ERR_ARG, "gs_boot_profiles: profile " + std::to_string(p) + ": " + why);
+    off[(size_t)p] = (int32_t)total;
+    total += (size_t)nseg[p];
+  }
+  std::vector<GsBootProfSeg> dev(total);
+  std::vector<long long> B((size_t)nprof);
+  for (int32_t p = 0; p < nprof; ++p)
+    B[(size_t)p] = gs_boot_profile_base(segs + off[(size_t)p], nseg[p], period[p], dev.data() + off[(size_t)p]);
+  CU(cudaSetDevice(h->device));
+  GsBootProfSeg *d = nullptr;
+  if (total > 0) {
+    if (cudaMalloc(&d, sizeof(GsBootProfSeg) * total) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(h, GS_ERR_CUDA, "gs_boot_profiles: allocation of the profiles failed");
+    }
+    if (cudaMemcpy(d, dev.data(), sizeof(GsBootProfSeg) * total, cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaFree(d);
+      return fail(h, GS_ERR_CUDA, "gs_boot_profiles: upload failed");
+    }
+  }
+  if (h->d_prof) { CU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_prof); }
+  h->d_prof = d; h->nprof = nprof; h->prof_seg.swap(dev); h->prof_off.swap(off); h->prof_B.swap(B);
+  h->prof_nseg.assign(nseg, nseg + nprof); h->prof_period.assign(period, period + nprof);
+  return GS_OK;
+}
+
+extern "C" int gs_boot_traces_profiled(gs_handle h, const gs_boot_params *params, const uint32_t *block_len, const int32_t *mix,
+                                       const int32_t *profile, double *kernel_ms) {
   if (!h) return GS_ERR_ARG;
   if (!params) return fail(h, GS_ERR_ARG, "gs_boot_traces: params is NULL");
   if (!h->d_pop) return fail(h, GS_ERR_STATE, "gs_boot_traces: call gs_boot_population first");
@@ -1623,6 +1667,7 @@ extern "C" int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params, c
   int64_t nmax = 1;
   bool blocked = false;                                 // some replica has L > 1: the blocked instantiation
   bool mixed = false;                                   // some replica has a mix >= 0: the mixed instantiation
+  bool profiled = false;                                // some replica has a profile >= 0: the profiled instantiation
   for (int i = 0; i < h->nsims; ++i) {
     const SimHost &s = h->sims[(size_t)i];
     const gs_boot_params &p = params[i];
@@ -1630,16 +1675,29 @@ extern "C" int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params, c
     if (s.cl.enable_network_costs) return fail(h, GS_ERR_ARG, "gs_boot_traces: traces with network columns go through gs_load_trace");
     if (p.n < 0 || p.n >= (1ll << 31) - 64) return fail(h, GS_ERR_ARG, "gs_boot_traces: n out of range");
     if (p.gap_num < 0 || p.gap_den < 1) return fail(h, GS_ERR_ARG, "gs_boot_traces: the gap scale needs gap_num >= 0 and gap_den >= 1");
-    if (gs_boot_arrive_bound(p.n, h->pop_max_gap, p.gap_num, p.gap_den) >= 0x7fffffffll)
+    const bool prof = profile && profile[i] >= 0;      // a profiled replica's bound is checked through its profile
+    if (!prof && gs_boot_arrive_bound(p.n, h->pop_max_gap, p.gap_num, p.gap_den) >= 0x7fffffffll)
       return fail(h, GS_ERR_ARG, "gs_boot_traces: the last arrival tick can reach 2^31 - 1 (fewer jobs or a smaller gap scale)");
     if (block_len && block_len[i] == 0) return fail(h, GS_ERR_ARG, "gs_boot_traces_blocked: block_len must be >= 1");
     if (mix && (mix[i] < -1 || mix[i] >= h->nmix))
       return fail(h, GS_ERR_ARG, "gs_boot_traces_mixed: mix index out of range [-1, nmix) for replica " + std::to_string(i));
+    if (profile && (profile[i] < -1 || profile[i] >= h->nprof))
+      return fail(h, GS_ERR_ARG, "gs_boot_traces_profiled: profile index out of range [-1, nprof) for replica " + std::to_string(i));
+    if (prof && (p.gap_num != 1 || p.gap_den != 1))
+      return fail(h, GS_ERR_ARG, "gs_boot_traces_profiled: a profiled replica needs the gap scale 1 / 1 (replica " + std::to_string(i) + ")");
+    if (prof) {
+      const size_t q = (size_t)profile[i];
+      if (gs_boot_profile_bound(h->prof_seg.data() + h->prof_off[q], h->prof_nseg[q], h->prof_period[q], h->prof_B[q], p.n,
+                                h->pop_max_gap) >= 0x7fffffffll)
+        return fail(h, GS_ERR_ARG, "gs_boot_traces_profiled: the last arrival tick of replica " + std::to_string(i) +
+                                       " can reach 2^31 - 1 under its profile (fewer jobs or a lighter profile)");
+    }
     GsBootRep &r = reps[(size_t)i];
     r.seed = p.seed; r.stream = p.stream; r.n = p.n; r.gap_num = p.gap_num; r.gap_den = p.gap_den;
     r.M = s.cl.num_switch * s.cl.num_node_p_switch; r.block_len = block_len ? block_len[i] : 1u;
     blocked = blocked || r.block_len > 1;
     mixed = mixed || (mix && mix[i] >= 0);
+    profiled = profiled || prof;
     nmax = std::max(nmax, p.n);
   }
   std::vector<GsBootMix> mixes(mixed ? (size_t)h->nsims : 0);
@@ -1647,11 +1705,23 @@ extern "C" int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params, c
     mixes[i].T = mix[i] >= 0 ? h->mix_T[(size_t)mix[i]] : 0;
     mixes[i].off = mix[i] >= 0 ? (long long)mix[i] * (long long)h->pop_k : 0;
   }
+  std::vector<GsBootProf> profs(profiled ? (size_t)h->nsims : 0);
+  for (size_t i = 0; i < profs.size(); ++i) {
+    GsBootProf &r = profs[i];
+    const int32_t q = profile[i];
+    r.B = q >= 0 ? h->prof_B[(size_t)q] : 0;
+    r.period = q >= 0 ? h->prof_period[(size_t)q] : 0;
+    r.off = q >= 0 ? h->prof_off[(size_t)q] : 0;
+    r.nseg = q >= 0 ? h->prof_nseg[(size_t)q] : 0;
+    r.reserved = 0;
+  }
   CU(cudaSetDevice(h->device));
   int rc = reserve_trace_arena(h, nmax);
   if (rc) return rc;
   const size_t off_out = align_up(sizeof(GsBootRep) * reps.size()), off_mix = align_up(off_out + 16 * reps.size());
-  rc = ensure_scratch(h, mixed ? off_mix + sizeof(GsBootMix) * mixes.size() : off_out + 16 * reps.size());
+  const size_t off_prof = align_up(off_mix + sizeof(GsBootMix) * mixes.size());
+  rc = ensure_scratch(h, profiled ? off_prof + sizeof(GsBootProf) * profs.size()
+                                  : mixed ? off_mix + sizeof(GsBootMix) * mixes.size() : off_out + 16 * reps.size());
   if (rc) return rc;
   unsigned char *d = (unsigned char *)h->d_scratch;
   std::vector<long long> res(2 * reps.size());
@@ -1659,9 +1729,23 @@ extern "C" int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params, c
   const int *gaps = (const int *)((unsigned char *)h->d_pop + align_up(sizeof(JobIn) * (size_t)h->pop_k));
   CU(cudaMemcpyAsync(d, reps.data(), sizeof(GsBootRep) * reps.size(), cudaMemcpyHostToDevice, h->stream));
   if (mixed) CU(cudaMemcpyAsync(d + off_mix, mixes.data(), sizeof(GsBootMix) * mixes.size(), cudaMemcpyHostToDevice, h->stream));
+  if (profiled) CU(cudaMemcpyAsync(d + off_prof, profs.data(), sizeof(GsBootProf) * profs.size(), cudaMemcpyHostToDevice, h->stream));
   CU(cudaEventRecord(h->e0, h->stream));
   const long long stride = (long long)(h->tarena_stride / sizeof(JobIn));
-  if (mixed)
+  using MixT = const GsBootMix *;
+  using TabT = const GsBootAlias *;
+  using ProfT = const GsBootProf *;
+  using SegT = const GsBootProfSeg *;
+  if (profiled && mixed)
+    (blocked ? gs_boot_kernel<true, true, MixT, TabT, ProfT, SegT> : gs_boot_kernel<false, true, MixT, TabT, ProfT, SegT>)
+        <<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>((const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena, stride,
+                                                               (long long *)(d + off_out), (MixT)(d + off_mix), h->d_mix,
+                                                               (ProfT)(d + off_prof), h->d_prof);
+  else if (profiled)
+    (blocked ? gs_boot_kernel<true, false, ProfT, SegT> : gs_boot_kernel<false, false, ProfT, SegT>)
+        <<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>((const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena, stride,
+                                                               (long long *)(d + off_out), (ProfT)(d + off_prof), h->d_prof);
+  else if (mixed)
     (blocked ? gs_boot_kernel<true, true, const GsBootMix *, const GsBootAlias *> : gs_boot_kernel<false, true, const GsBootMix *, const GsBootAlias *>)
         <<<(unsigned)h->nsims, GS_BOOT_THREADS, 0, h->stream>>>((const GsBootRep *)d, pop, gaps, (long long)h->pop_k, (JobIn *)h->tarena, stride,
                                                                (long long *)(d + off_out), (const GsBootMix *)(d + off_mix), h->d_mix);

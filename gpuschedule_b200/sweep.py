@@ -7,6 +7,7 @@ from __future__ import annotations
 import argparse
 import datetime
 import math
+import operator
 import os
 import types
 from fractions import Fraction
@@ -448,7 +449,73 @@ def parse_mix_spec(spec, nclasses):
     return m
 
 
-def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1, mix=None):
+def check_profiles(profile):
+    """[(points, period), ...] of a profile argument as a list of (((tick, factor), ...), period), or ValueError: at
+    least one profile; each with 1..64 points whose ticks are ints starting at 0, strictly increasing and below
+    2^31 - 1, whose load factors are positive and finite, and a period 0 (aperiodic) or above the last tick and below
+    2^31 - 1"""
+    try:
+        out = []
+        for points, period in profile:
+            pts = tuple((operator.index(t), float(f)) for t, f in points)
+            out.append((pts, operator.index(period)))
+    except (TypeError, ValueError):
+        raise ValueError("profile: expected [(points, period), ...] with points (tick, load factor) pairs") from None
+    if not out:
+        raise ValueError("profile: at least one profile")
+    for pts, period in out:
+        if not 1 <= len(pts) <= tracegen.MAX_SEGMENTS:
+            raise ValueError(f"profile: every profile needs 1..{tracegen.MAX_SEGMENTS} points")
+        ticks = [t for t, _ in pts]
+        if ticks[0] != 0 or any(b <= a for a, b in zip(ticks, ticks[1:])) or ticks[-1] >= 2 ** 31 - 1:
+            raise ValueError("profile: the ticks must start at 0, increase strictly and stay below 2^31 - 1")
+        if not all(math.isfinite(f) and f > 0 for _, f in pts):
+            raise ValueError("profile: every load factor must be positive and finite")
+        if period < 0 or period >= 2 ** 31 - 1 or 0 < period <= ticks[-1]:
+            raise ValueError("profile: the period must be 0, or above the last tick and below 2^31 - 1")
+    return out
+
+
+def profile_segments(points, period, load):
+    """the gs_boot_profiles segments of a profile at offered load L: segment k starts at tick T_k with the gap scale
+    load_gap_scale(L * F_k).  Returns (segments as (start, gap_num, gap_den) triples, period), or ValueError for a
+    scale whose numerator is 0 or above 2^31 - 1"""
+    segs = []
+    for t, f in points:
+        try:
+            num, den = load_gap_scale(float(load) * f)
+        except (OverflowError, ZeroDivisionError):
+            num = 0
+        if not 1 <= num <= 2 ** 31 - 1:
+            raise ValueError(f"profile: the load {float(load) * f!r} (load {load} x factor {f}) cannot be expressed as a gap scale")
+        segs.append((t, num, den))
+    return segs, period
+
+
+def parse_profile_spec(spec):
+    """the (points, period) of a --load-profile SPEC T0:F0,T1:F1,...[@P]: integer ticks from 0, positive finite load
+    factors, an optional period; or ValueError"""
+    text = str(spec)
+    body, at, per = text.partition("@")
+    if at and not (per.isascii() and per.isdigit()):
+        raise ValueError(f"--load-profile: {spec!r}: the period after '@' must be a non-negative integer")
+    points = []
+    for part in body.split(","):
+        t, colon, f = part.partition(":")
+        if not colon or not (t.isascii() and t.isdigit()):
+            raise ValueError(f"--load-profile: {spec!r} is not TICK:FACTOR pairs joined by ','")
+        try:
+            fv = float(f)
+        except ValueError:
+            raise ValueError(f"--load-profile: {spec!r}: {f!r} is not a load factor") from None
+        points.append((int(t), fv))
+    try:
+        return check_profiles([(points, int(per) if at else 0)])[0]
+    except ValueError as e:
+        raise ValueError(f"--load-profile: {spec!r}: {e}") from None
+
+
+def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1, mix=None, profile=None):
     if int(replicas) < 1:
         raise ValueError("bootstrap: replicas must be >= 1")
     if not len(loads) or not all(math.isfinite(float(L)) and float(L) > 0 for L in loads):
@@ -463,13 +530,17 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1, mix=None):
         raise ValueError(f"bootstrap: {e}") from None
     if mix is not None:
         check_mix(mix)
+    if profile is not None:
+        for points, period in check_profiles(profile):
+            for L in loads:
+                tracegen.check_profile(*profile_segments(points, period, L))
     aware = [fl.schedule for fl in flag_sets if _is_utilisation_aware(fl)]
     if aware:
         raise ValueError(f"bootstrap: the utilisation-aware engine ({', '.join(sorted(set(aware)))}) has no generated traces")
 
 
 def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1,
-                        compare=None, mix=None, slowdown=None, occupancy=None):
+                        compare=None, mix=None, slowdown=None, occupancy=None, profile=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -499,10 +570,19 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     slowdown=(key, bounds, tau, edges, sd_edges): also append (SDCLASS_DTYPE records (..., C), CDF counts (..., C,
     3 * (E + 1) + Esd + 1)) with the replicas' leading axes, after the jobdist element (before the compare element).
     occupancy=queue edges: also append (OCC_DTYPE records (...), busy histograms (..., 2, P), queue histograms
-    (..., E + 1)) with the replicas' leading axes as the last element, P as in summarize_batched."""
+    (..., E + 1)) with the replicas' leading axes as the last element, P as in summarize_batched.
+    profile=[(points, period), ...]: give the replicas a time-varying offered load (gs_boot_traces_profiled).  points
+    are (tick, load factor) pairs starting at tick 0; at load L, the segment from tick T_k on has the gap scale
+    load_gap_scale(L * F_k), and a period P > 0 repeats the profile every P ticks.  Rows, gaps, block starts and mix
+    picks are those of the unprofiled replica; only the arrivals move.  Every returned array gains a profile axis
+    right after the mix axis (after the loads axis without mixes), and compare pairs (a, L[, mix], profile, r) with
+    (b, L[, mix], profile, r).  A replica whose last arrival could reach 2^31 - 1 is a ValueError, raised after the
+    traces are read and before any engine is created."""
     if occupancy is not None:
         occ_edges = check_occupancy(occupancy)
-    _check_bootstrap_args(flag_sets, replicas, loads, n, block_len, mix)
+    _check_bootstrap_args(flag_sets, replicas, loads, n, block_len, mix, profile)
+    if profile is not None:
+        profile = check_profiles(profile)
     if slowdown is not None:
         sd = check_slowdown(slowdown)
         sd_nc, sd_row = len(sd[1]) + 1, _sd_row(sd)
@@ -518,8 +598,10 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
         nc, nb = len(jd_bounds) + 1, len(jd_edges) + 1
     R, loads = int(replicas), [float(L) for L in loads]
     M = 1 if mix is None else len(mix_mults)
-    lead = (len(loads), R) if mix is None else (len(loads), M, R)   # the axes of one configuration's replicas
-    per = len(loads) * M * R
+    NP = 1 if profile is None else len(profile)
+    lead = (len(loads),) + (() if mix is None else (M,)) + (() if profile is None else (NP,)) + (R,)   # one configuration's replicas
+    per = len(loads) * M * NP * R
+    profs = None if profile is None else [profile_segments(pts, period, L) for L in loads for pts, period in profile]
     out = np.zeros((len(flag_sets),) + lead, dtype=capi.SUMMARY_DTYPE)
     if timeline is not None:
         bins = np.zeros((len(flag_sets),) + lead + (B,), dtype=capi.TBIN_DTYPE)
@@ -552,28 +634,41 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
                 if not w.any():
                     raise ValueError(f"bootstrap: mix {':'.join(map(str, mix_mults[m]))} gives every job of "
                                      f"{flag_sets[configs[0]].trace_file} weight 0")
+        if profs is not None:
+            jobs = base.n if n is None else int(n)
+            gaps = np.diff(base.arrive_tick.astype(np.int64))
+            max_gap = int(gaps.max()) if len(gaps) else 0
+            for q, prof in enumerate(profs):
+                if tracegen.profile_bound(jobs, max_gap, *prof) >= 2 ** 31 - 1:
+                    pts, period = profile[q % NP]
+                    raise ValueError(f"bootstrap: under the profile {pts}{f' @ {period}' if period else ''} at load {loads[q // NP]}, "
+                                     f"a replica of {jobs} jobs of {flag_sets[configs[0]].trace_file} can arrive at 2^31 - 1 or later")
         groups.append((configs, sims, base, weights))
     for configs, sims, base, weights in groups:
         jobs = base.n if n is None else int(n)
         params = np.zeros(len(configs) * per, dtype=capi.BOOT_PARAMS_DTYPE)
-        mix_of = np.zeros(len(params), dtype=np.int32)    # replica (config k, load l, mix m, r) is k * per + (l * M + m) * R + r
+        mix_of = np.zeros(len(params), dtype=np.int32)    # replica (config k, load l, mix m, profile q, r) is
+        prof_of = np.zeros(len(params), dtype=np.int32)   # k * per + ((l * M + m) * NP + q) * R + r
         with capi.Engine(device=device, nsims=len(params)) as eng:
             i = 0
             for fl, infra, jm, pol in sims:
-                for L in loads:
-                    num, den = load_gap_scale(L)
+                for li, L in enumerate(loads):
+                    num, den = load_gap_scale(L) if profile is None else (1, 1)
                     for m in range(M):
-                        for r in range(R):
-                            eng.config(i, infra.gs_cluster(), pol)
-                            params[i] = (seed, r, jobs, num, den)
-                            mix_of[i] = m
-                            i += 1
+                        for q in range(NP):
+                            for r in range(R):
+                                eng.config(i, infra.gs_cluster(), pol)
+                                params[i] = (seed, r, jobs, num, den)
+                                mix_of[i] = m
+                                prof_of[i] = li * NP + q
+                                i += 1
             eng.boot_population(base)
-            if weights is None:
-                eng.boot_traces(params, block_len=None if block_len == 1 else block_len)
-            else:
+            if weights is not None:
                 eng.boot_mixes(weights)
-                eng.boot_traces(params, block_len=None if block_len == 1 else block_len, mix=mix_of)
+            if profs is not None:
+                eng.boot_profiles(profs)
+            eng.boot_traces(params, block_len=None if block_len == 1 else block_len, mix=None if weights is None else mix_of,
+                            profile=None if profs is None else prof_of)
             if timeline is not None:
                 eng.set_timeline(W, B)
             if jobdist is not None:
@@ -627,45 +722,50 @@ def _block_val(block_len):
     return [] if block_len is None else [block_len]
 
 
-def _mix_col(mix):
-    """the mix column of the bootstrap files: none without job mixes (mix None)"""
-    return [] if mix is None else ["mix"]
+def _mix_col(mix, profile=None):
+    """the mix and profile columns of the bootstrap files: none without job mixes (mix None) and load profiles
+    (profile None)"""
+    return ([] if mix is None else ["mix"]) + ([] if profile is None else ["profile"])
 
 
-def _load_lines(loads, block_len, mix, per_load):
-    """[(values of the load, block_len and mix columns, arrays)] of one configuration's (load[, mix]) lines in line
-    order: per_load holds one entry per load, and with mixes (their SPEC texts) one per (load, mix)"""
-    if mix is None:
-        return [([L] + _block_val(block_len), x) for L, x in zip(loads, per_load)]
-    return [([L] + _block_val(block_len) + [m], x) for L, per_mix in zip(loads, per_load) for m, x in zip(mix, per_mix)]
+def _load_lines(loads, block_len, mix, per_load, profile=None):
+    """[(values of the load, block_len, mix and profile columns, arrays)] of one configuration's (load[, mix][, profile])
+    lines in line order: per_load holds one entry per load, with mixes (their SPEC texts) one per (load, mix), and with
+    load profiles (their SPEC texts) one per (load[, mix], profile)"""
+    lines = [([L] + _block_val(block_len), x) for L, x in zip(loads, per_load)]
+    if mix is not None:
+        lines = [(keys + [m], x) for keys, per_mix in lines for m, x in zip(mix, per_mix)]
+    if profile is not None:
+        lines = [(keys + [p], x) for keys, per_prof in lines for p, x in zip(profile, per_prof)]
+    return lines
 
 
-def write_bootstrap_csv(path, flag_sets, loads, records, block_len=None, mix=None):
+def write_bootstrap_csv(path, flag_sets, loads, records, block_len=None, mix=None, profile=None):
     """one line per (configuration, load[, mix], replica): replica, load, block_len (with a block length), mix (with
     job mixes: their SPEC texts), the configuration's flags, the summary columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(["replica", "load"] + _block_col(block_len) + _mix_col(mix) + SUMMARY_KEYS + summary.columns())
+        w.writerow(["replica", "load"] + _block_col(block_len) + _mix_col(mix, profile) + SUMMARY_KEYS + summary.columns())
         for fl, per_load in zip(flag_sets, records):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
-            for keys, recs in _load_lines(loads, block_len, mix, per_load):
+            for keys, recs in _load_lines(loads, block_len, mix, per_load, profile):
                 for r, rec in enumerate(recs):
                     w.writerow([r] + keys + [fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + summary.flat(rec, *shape))
 
 
-def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95, block_len=None, mix=None):
+def write_bootstrap_ci_csv(path, flag_sets, loads, records, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration, load[, mix]): the flags, the load, block_len (with a block length), mix (with job
     mixes), the replica count and summary.spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["replicas", "level"] + summary.spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix, profile) + ["replicas", "level"] + summary.spread_columns())
         for fl, per_load in zip(flag_sets, records):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
-            for keys, recs in _load_lines(loads, block_len, mix, per_load):
+            for keys, recs in _load_lines(loads, block_len, mix, per_load, profile):
                 w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [len(recs), level]
                            + summary.spread_flat(summary.spread(recs, *shape, level=level)))
 
@@ -692,17 +792,17 @@ def write_timeline_csv(path, flag_sets, bins, width):
                            + _bin_bounds(b, width, len(tb)) + summary.timeline_flat(d, b))
 
 
-def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95, block_len=None, mix=None):
+def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration, load[, mix], bin): the flags, the load, block_len (with a block length), mix (with
     job mixes), the bin, its tick range, the number of replicas with rows in it and summary.timeline_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["bin", "bin_start", "bin_end", "replicas", "level"] + summary.timeline_spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix, profile) + ["bin", "bin_start", "bin_end", "replicas", "level"] + summary.timeline_spread_columns())
         for fl, per_load in zip(flag_sets, bins):
             cl = Infrastructure(fl).gs_cluster()
             shape = (cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib)
-            for keys, tb in _load_lines(loads, block_len, mix, per_load):
+            for keys, tb in _load_lines(loads, block_len, mix, per_load, profile):
                 sp = summary.timeline_spread(tb, *shape, level=level)
                 for b in range(tb.shape[1]):
                     w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [b]
@@ -727,17 +827,17 @@ def write_jobdist_csv(path, flag_sets, classes, hist, bounds, edges):
                            + summary.jobdist_flat(d, c))
 
 
-def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None, mix=None):
+def write_jobdist_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration, load[, mix], class): the flags, the load, block_len (with a block length), mix
     (with job mixes), the class, its num_gpu range, the number of replicas with jobs in it and
     summary.jobdist_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["class", "gpus_min", "gpus_max", "replicas", "level"]
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix, profile) + ["class", "gpus_min", "gpus_max", "replicas", "level"]
                    + summary.jobdist_spread_columns())
         for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
-            for (keys, cl), (_, hs) in zip(_load_lines(loads, block_len, mix, per_cl), _load_lines(loads, block_len, mix, per_hs)):
+            for (keys, cl), (_, hs) in zip(_load_lines(loads, block_len, mix, per_cl, profile), _load_lines(loads, block_len, mix, per_hs, profile)):
                 sp = summary.jobdist_spread(cl, hs, edges, level=level)
                 for c in range(cl.shape[1]):
                     w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [c]
@@ -794,17 +894,17 @@ def write_jobdist_cdf_csv(path, flag_sets, classes, hist, bounds, edges):
                                    + [m, edge, int(d["jobs"][c]), float(d[m + "_cdf"][c, e])])
 
 
-def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None, mix=None):
+def write_jobdist_cdf_ci_csv(path, flag_sets, loads, classes, hist, bounds, edges, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration, load[, mix], class, quantity, edge): the flags, the load, block_len (with a block
     length), mix (with job mixes), the class, its num_gpu range, the quantity, the edge, the number of replicas with jobs in the class and
     the spread of the CDF value"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["class", "gpus_min", "gpus_max", "quantity", "edge", "replicas", "level"]
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix, profile) + ["class", "gpus_min", "gpus_max", "quantity", "edge", "replicas", "level"]
                    + [f"cdf_{s}" for s in summary.SPREAD_STATS])
         for fl, per_cl, per_hs in zip(flag_sets, classes, hist):
-            for (keys, cl), (_, hs) in zip(_load_lines(loads, block_len, mix, per_cl), _load_lines(loads, block_len, mix, per_hs)):
+            for (keys, cl), (_, hs) in zip(_load_lines(loads, block_len, mix, per_cl, profile), _load_lines(loads, block_len, mix, per_hs, profile)):
                 sp = summary.jobdist_spread(cl, hs, edges, level=level)
                 for c in range(cl.shape[1]):
                     for m in summary.JOBDIST_QUANTITIES:
@@ -838,23 +938,23 @@ def write_slowdown_csv(path, flag_sets, recs, hist, sd):
                 w.writerow(_sd_keys(fl, sd, c) + summary.slowdown_flat(d, c))
 
 
-def write_slowdown_ci_csv(path, flag_sets, loads, recs, hist, sd, level=0.95, block_len=None, mix=None):
+def write_slowdown_ci_csv(path, flag_sets, loads, recs, hist, sd, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration, load[, block_len][, mix], class): the flags, the load, block_len (with a block
     length), mix (with job mixes), the key, the class, its key range, tau, the replicas with jobs in the class and
     summary.slowdown_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["key", "class", "key_min", "key_max", "tau"]
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix, profile) + ["key", "class", "key_min", "key_max", "tau"]
                    + ["replicas", "level"] + summary.slowdown_spread_columns())
         for fl, per_rc, per_hs in zip(flag_sets, recs, hist):
-            for (keys, rc), (_, hs) in zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)):
+            for (keys, rc), (_, hs) in zip(_load_lines(loads, block_len, mix, per_rc, profile), _load_lines(loads, block_len, mix, per_hs, profile)):
                 sp = summary.slowdown_spread(rc, hs, sd[3], sd[4], level=level)
                 for c in range(rc.shape[1]):
                     w.writerow(_sd_keys(fl, sd, c, keys) + [int(sp["replicas"][c]), level] + summary.slowdown_spread_flat(sp, c))
 
 
-def write_slowdown_cdf_csv(path, flag_sets, recs, hist, sd, loads=None, level=0.95, block_len=None, mix=None):
+def write_slowdown_cdf_csv(path, flag_sets, recs, hist, sd, loads=None, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration[, load[, block_len][, mix]], class, quantity, edge): the flags[, the load, block_len,
     mix], the key, the class, its key range, tau, the quantity (wait, turnaround, jct in ticks; sd in units of slowdown),
     the edge in that unit and the fraction of the class's jobs with a value <= the edge (with loads: the replicas with
@@ -863,10 +963,10 @@ def write_slowdown_cdf_csv(path, flag_sets, recs, hist, sd, loads=None, level=0.
     boot = loads is not None
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["key", "class", "key_min", "key_max", "tau"]
+        w.writerow(SUMMARY_KEYS + (["load"] + _block_col(block_len) + _mix_col(mix, profile) if boot else []) + ["key", "class", "key_min", "key_max", "tau"]
                    + ["quantity", "edge"] + (["replicas", "level"] + [f"cdf_{s}" for s in summary.SPREAD_STATS] if boot else ["jobs", "cdf"]))
         for fl, per_rc, per_hs in zip(flag_sets, recs, hist):
-            lines = (zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)) if boot
+            lines = (zip(_load_lines(loads, block_len, mix, per_rc, profile), _load_lines(loads, block_len, mix, per_hs, profile)) if boot
                      else [(([], per_rc), ([], per_hs))])
             for (lk, rc), (_, hs) in lines:
                 d = summary.slowdown_spread(rc, hs, sd[3], sd[4], level=level) if boot else summary.slowdown_derived(rc, hs, sd[3], sd[4])
@@ -888,15 +988,15 @@ def write_occupancy_csv(path, flag_sets, recs, busy, queue, edges):
             w.writerow(_occ_keys(fl) + summary.occupancy_flat(rc, summary.occupancy_derived(rc, bh, qh, edges)))
 
 
-def write_occupancy_ci_csv(path, flag_sets, loads, recs, busy, queue, edges, level=0.95, block_len=None, mix=None):
+def write_occupancy_ci_csv(path, flag_sets, loads, recs, busy, queue, edges, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration, load[, block_len][, mix]): the flags, the load columns, the replica count and
     summary.occupancy_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix) + ["replicas", "level"] + summary.occupancy_spread_columns())
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix, profile) + ["replicas", "level"] + summary.occupancy_spread_columns())
         for fl, per_rc, per_bh, per_qh in zip(flag_sets, recs, busy, queue):
-            lines = zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_bh), _load_lines(loads, block_len, mix, per_qh))
+            lines = zip(_load_lines(loads, block_len, mix, per_rc, profile), _load_lines(loads, block_len, mix, per_bh, profile), _load_lines(loads, block_len, mix, per_qh, profile))
             for (keys, rc), (_, bh), (_, qh) in lines:
                 sp = summary.occupancy_spread(rc, bh, qh, edges, level=level)
                 w.writerow(_occ_keys(fl) + keys + [len(rc), level] + summary.occupancy_spread_flat(sp))
@@ -913,7 +1013,7 @@ def _cdf_points(hist):
     return t, (cum / t if t else np.full(len(cum), np.nan))
 
 
-def write_occupancy_cdf_csv(path, flag_sets, recs, busy, queue, edges, loads=None, level=0.95, block_len=None, mix=None):
+def write_occupancy_cdf_csv(path, flag_sets, recs, busy, queue, edges, loads=None, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration[, load[, block_len][, mix]], quantity, point): quantity busy (every b = 0 .. M * G,
     all time), busy_wait (the same over the ticks with a queue) or queue (at every queue edge), the point and the
     share of time at or below it (with loads: the replicas and the spread of that share)"""
@@ -921,13 +1021,13 @@ def write_occupancy_cdf_csv(path, flag_sets, recs, busy, queue, edges, loads=Non
     boot = loads is not None
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["quantity", "point"]
+        w.writerow(SUMMARY_KEYS + (["load"] + _block_col(block_len) + _mix_col(mix, profile) if boot else []) + ["quantity", "point"]
                    + (["replicas", "level"] + [f"cdf_{s}" for s in summary.SPREAD_STATS] if boot else ["ticks", "cdf"]))
         for fl, per_rc, per_bh, per_qh in zip(flag_sets, recs, busy, queue):
             G = Infrastructure(fl).gs_cluster()
             G = G.num_switch * G.num_node_p_switch * G.num_gpu_p_node
-            lines = (zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_bh),
-                         _load_lines(loads, block_len, mix, per_qh)) if boot else [(([], per_rc), ([], per_bh), ([], per_qh))])
+            lines = (zip(_load_lines(loads, block_len, mix, per_rc, profile), _load_lines(loads, block_len, mix, per_bh, profile),
+                         _load_lines(loads, block_len, mix, per_qh, profile)) if boot else [(([], per_rc), ([], per_bh), ([], per_qh))])
             for (lk, rc), (_, bh), (_, qh) in lines:
                 if not boot:
                     rc, bh, qh = rc[None], bh[None], qh[None]
@@ -963,17 +1063,17 @@ def write_paired_csv(path, flag_sets, pairs, recs, hist, bounds, edges):
                     w.writerow(_pair_keys(flag_sets[b], flag_sets[a]) + [c] + _class_range(c, bounds) + [m] + summary.pair_flat(d, c, m))
 
 
-def write_paired_ci_csv(path, flag_sets, pairs, loads, recs, hist, bounds, edges, level=0.95, block_len=None, mix=None):
+def write_paired_ci_csv(path, flag_sets, pairs, loads, recs, hist, bounds, edges, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration b of a pair, load[, mix], class, quantity): b's flags, the base schedule, the load,
     block_len (with a block length), mix (with job mixes), the class, its num_gpu range, the quantity, the replicas with jobs finished in
     both runs in the class and summary.pair_spread's columns"""
     import csv
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["base_schedule", "load"] + _block_col(block_len) + _mix_col(mix) + ["class", "gpus_min", "gpus_max", "quantity", "replicas", "level"]
+        w.writerow(SUMMARY_KEYS + ["base_schedule", "load"] + _block_col(block_len) + _mix_col(mix, profile) + ["class", "gpus_min", "gpus_max", "quantity", "replicas", "level"]
                    + summary.pair_spread_columns())
         for (a, b), per_rc, per_hs in zip(pairs, recs, hist):
-            for (keys, rc), (_, hs) in zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)):
+            for (keys, rc), (_, hs) in zip(_load_lines(loads, block_len, mix, per_rc, profile), _load_lines(loads, block_len, mix, per_hs, profile)):
                 sp = summary.pair_spread(rc, hs, edges, level=level)
                 for c in range(rc.shape[1]):
                     for m in summary.JOBDIST_QUANTITIES:
@@ -981,7 +1081,7 @@ def write_paired_ci_csv(path, flag_sets, pairs, loads, recs, hist, bounds, edges
                                    + [m, int(sp["replicas"][c]), level] + summary.pair_spread_flat(sp, c, m))
 
 
-def write_paired_cdf_csv(path, flag_sets, pairs, recs, hist, bounds, edges, loads=None, level=0.95, block_len=None, mix=None):
+def write_paired_cdf_csv(path, flag_sets, pairs, recs, hist, bounds, edges, loads=None, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration b of a pair[, load[, mix]], class, quantity, edge): b's flags, the base schedule[, the
     load, block_len, mix], the class, its num_gpu range, the quantity, the edge and the fraction of the jobs finished in both
     runs with d <= edge (with loads: the replicas with such jobs and the spread of that fraction)"""
@@ -989,11 +1089,11 @@ def write_paired_cdf_csv(path, flag_sets, pairs, recs, hist, bounds, edges, load
     boot = loads is not None
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["class", "gpus_min", "gpus_max", "quantity", "edge"]
+        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) + _mix_col(mix, profile) if boot else []) + ["class", "gpus_min", "gpus_max", "quantity", "edge"]
                    + (["replicas", "level"] + [f"cdf_{s}" for s in summary.SPREAD_STATS] if boot else ["jobs", "cdf"]))
         for (a, b), per_rc, per_hs in zip(pairs, recs, hist):
             keys = _pair_keys(flag_sets[b], flag_sets[a])
-            lines = (zip(_load_lines(loads, block_len, mix, per_rc), _load_lines(loads, block_len, mix, per_hs)) if boot
+            lines = (zip(_load_lines(loads, block_len, mix, per_rc, profile), _load_lines(loads, block_len, mix, per_hs, profile)) if boot
                      else [(([], per_rc), ([], per_hs))])
             for (lk, rc), (_, hs) in lines:
                 d = summary.pair_spread(rc, hs, edges, level=level) if boot else summary.pair_derived(rc, hs, edges)
@@ -1005,7 +1105,7 @@ def write_paired_cdf_csv(path, flag_sets, pairs, recs, hist, bounds, edges, load
                             w.writerow(keys + lk + [c] + _class_range(c, bounds) + [m, edge] + tail)
 
 
-def write_paired_summary_csv(path, flag_sets, pairs, records, loads=None, level=0.95, block_len=None, mix=None):
+def write_paired_summary_csv(path, flag_sets, pairs, records, loads=None, level=0.95, block_len=None, mix=None, profile=None):
     """one line per (configuration b of a pair[, load[, mix]]): b's flags, the base schedule[, the load, block_len, mix],
     the replicas and summary.paired_spread's columns: the replica-level differences b - base of the makespan and of
     every derived number (records: (configurations, loads[, mixes], replicas) with loads, else one record per
@@ -1018,11 +1118,11 @@ def write_paired_summary_csv(path, flag_sets, pairs, records, loads=None, level=
         return cl.num_switch * cl.num_node_p_switch, cl.num_gpu_p_node, cl.gpu_mem_cap_mib
     with open(path, "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) + _mix_col(mix) if boot else []) + ["replicas", "level"]
+        w.writerow(SUMMARY_KEYS + ["base_schedule"] + (["load"] + _block_col(block_len) + _mix_col(mix, profile) if boot else []) + ["replicas", "level"]
                    + summary.paired_columns())
         for a, b in pairs:
             sa, sb = shape(flag_sets[a]), shape(flag_sets[b])
-            per = (zip(_load_lines(loads, block_len, mix, records[a]), _load_lines(loads, block_len, mix, records[b])) if boot
+            per = (zip(_load_lines(loads, block_len, mix, records[a], profile), _load_lines(loads, block_len, mix, records[b], profile)) if boot
                    else [(([], records[a:a + 1]), ([], records[b:b + 1]))])
             for (lk, ra), (_, rb) in per:
                 sp = summary.paired_spread(ra, rb, sa, sb, level=level)
@@ -1071,6 +1171,11 @@ def main(argv=None):
                          "block_len with --block-len)")
     ap.add_argument("--mix-classes", type=int, nargs="+", default=None, metavar="B",
                     help="with --mix: class bounds B1 < ... < Bk of the mixes (a job's class is the number of bounds <= its num_gpu)")
+    ap.add_argument("--load-profile", nargs="+", default=None, metavar="SPEC",
+                    help="with --bootstrap: give the replicas each time-varying offered load SPEC, T0:F0,T1:F1,...[@P]: from tick "
+                         "Tk on the load is Fk times --load (integer ticks from 0, strictly increasing; positive load factors), "
+                         "repeating every P ticks when @P is given.  Example: 0:1,20000:3,22000:1 is a 3x surge for 2000 ticks.  "
+                         "Every output file gets a profile column after mix (after load / block_len without --mix)")
     ap.add_argument("--summary-ci", default=None, metavar="FILE",
                     help="with --bootstrap: one CSV line per (configuration, load) with the mean, std and 95%% interval across replicas")
     ap.add_argument("--timeline", default=None, metavar="FILE",
@@ -1222,6 +1327,15 @@ def main(argv=None):
         except ValueError as e:
             ap.error(str(e))
         mix_text = list(a.mix)
+    profile = profile_text = None
+    if a.load_profile is not None:
+        if a.bootstrap is None:
+            ap.error("--load-profile needs --bootstrap")
+        try:
+            profile = [parse_profile_spec(p) for p in a.load_profile]
+        except ValueError as e:
+            ap.error(str(e))
+        profile_text = list(a.load_profile)
     if a.bootstrap is not None:
         if not a.summary:
             ap.error("--bootstrap needs --summary FILE")
@@ -1257,48 +1371,50 @@ def main(argv=None):
     if a.bootstrap is not None:
         loads = a.load or [1.0]
         try:
-            _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs, 1 if a.block_len is None else a.block_len, mix)
+            _check_bootstrap_args(sets, a.bootstrap, loads, a.jobs, 1 if a.block_len is None else a.block_len, mix, profile)
         except ValueError as e:
             ap.error(str(e))
         bl = a.block_len
         res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist,
-                                  block_len=1 if bl is None else bl, compare=compare, mix=mix, slowdown=slowdown, occupancy=occupancy)
+                                  block_len=1 if bl is None else bl, compare=compare, mix=mix, slowdown=slowdown, occupancy=occupancy,
+                                  profile=profile)
         recs, rest = (res, ()) if (timeline is None and jobdist is None and compare is None and slowdown is None
                                    and occupancy is None) else (res[0], res[1:])
         if occupancy is not None:
             orec, obusy, oq = rest[-1]
             rest = rest[:-1]
-            write_occupancy_ci_csv(a.occupancy, sets, loads, orec, obusy, oq, occupancy, block_len=bl, mix=mix_text)
+            write_occupancy_ci_csv(a.occupancy, sets, loads, orec, obusy, oq, occupancy, block_len=bl, mix=mix_text, profile=profile_text)
             if a.occupancy_cdf:
-                write_occupancy_cdf_csv(a.occupancy_cdf, sets, orec, obusy, oq, occupancy, loads=loads, block_len=bl, mix=mix_text)
+                write_occupancy_cdf_csv(a.occupancy_cdf, sets, orec, obusy, oq, occupancy, loads=loads, block_len=bl, mix=mix_text, profile=profile_text)
         if compare is not None:
             pairs, cmp_bounds, cmp_edges = compare
             prec, phist = rest[-1]
             rest = rest[:-1]
             if a.paired:
-                write_paired_ci_csv(a.paired, sets, pairs, loads, prec, phist, cmp_bounds, cmp_edges, block_len=bl, mix=mix_text)
+                write_paired_ci_csv(a.paired, sets, pairs, loads, prec, phist, cmp_bounds, cmp_edges, block_len=bl, mix=mix_text, profile=profile_text)
             if a.paired_cdf:
-                write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges, loads=loads, block_len=bl, mix=mix_text)
+                write_paired_cdf_csv(a.paired_cdf, sets, pairs, prec, phist, cmp_bounds, cmp_edges, loads=loads, block_len=bl, mix=mix_text, profile=profile_text)
             if a.paired_summary:
-                write_paired_summary_csv(a.paired_summary, sets, pairs, recs, loads=loads, block_len=bl, mix=mix_text)
+                write_paired_summary_csv(a.paired_summary, sets, pairs, recs, loads=loads, block_len=bl, mix=mix_text, profile=profile_text)
         if slowdown is not None:
             srec, shist = rest[-1]
             rest = rest[:-1]
-            write_slowdown_ci_csv(a.slowdown, sets, loads, srec, shist, slowdown, block_len=bl, mix=mix_text)
+            write_slowdown_ci_csv(a.slowdown, sets, loads, srec, shist, slowdown, block_len=bl, mix=mix_text, profile=profile_text)
             if a.slowdown_cdf:
-                write_slowdown_cdf_csv(a.slowdown_cdf, sets, srec, shist, slowdown, loads=loads, block_len=bl, mix=mix_text)
+                write_slowdown_cdf_csv(a.slowdown_cdf, sets, srec, shist, slowdown, loads=loads, block_len=bl, mix=mix_text, profile=profile_text)
         if timeline is not None:
-            write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0], block_len=bl, mix=mix_text)
+            write_timeline_ci_csv(a.timeline, sets, loads, rest[0], timeline[0], block_len=bl, mix=mix_text, profile=profile_text)
         if jobdist is not None:
             cls, hist = rest[-1]
-            write_jobdist_ci_csv(a.jobdist, sets, loads, cls, hist, *jobdist, block_len=bl, mix=mix_text)
+            write_jobdist_ci_csv(a.jobdist, sets, loads, cls, hist, *jobdist, block_len=bl, mix=mix_text, profile=profile_text)
             if a.jobdist_cdf:
-                write_jobdist_cdf_ci_csv(a.jobdist_cdf, sets, loads, cls, hist, *jobdist, block_len=bl, mix=mix_text)
-        write_bootstrap_csv(a.summary, sets, loads, recs, block_len=bl, mix=mix_text)
+                write_jobdist_cdf_ci_csv(a.jobdist_cdf, sets, loads, cls, hist, *jobdist, block_len=bl, mix=mix_text, profile=profile_text)
+        write_bootstrap_csv(a.summary, sets, loads, recs, block_len=bl, mix=mix_text, profile=profile_text)
         if a.summary_ci:
-            write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs, block_len=bl, mix=mix_text)
+            write_bootstrap_ci_csv(a.summary_ci, sets, loads, recs, block_len=bl, mix=mix_text, profile=profile_text)
         print(f"{a.summary}: {len(sets)} configurations x {len(loads)} loads"
-              + (f" x {len(mix_text)} mixes" if mix_text else "") + f" x {a.bootstrap} replicas")
+              + (f" x {len(mix_text)} mixes" if mix_text else "") + (f" x {len(profile_text)} load profiles" if profile_text else "")
+              + f" x {a.bootstrap} replicas")
         return
     if a.summary:
         res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare, slowdown=slowdown, occupancy=occupancy,

@@ -180,14 +180,85 @@ def class_weights(gpus, bounds, multipliers):
     return np.asarray(m, dtype=np.uint32)[cls]
 
 
-def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_len=1, weights=None):
+MAX_SEGMENTS = 64
+
+
+def check_profile(segments, period=0):
+    """a load profile (segments, period) as (starts, gap_nums, gap_dens, period), lists of Python ints, or ValueError.
+    segments: BOOT_SEG_DTYPE records or (start, gap_num, gap_den) triples, 1..MAX_SEGMENTS of them; the rules of
+    gs_boot_profiles (include/gsched.h): the first start 0, starts strictly increasing and below 2^31 - 1, every
+    gap_num and gap_den in 1..2^31 - 1, and a period 0 (aperiodic) or above the last start and below 2^31 - 1"""
+    a = np.asarray(segments)
+    try:
+        if a.dtype.names:
+            t, num, den = (a[f].tolist() for f in ("start", "gap_num", "gap_den"))
+        else:
+            if a.ndim != 2 or a.shape[1] != 3 or a.dtype.kind not in "iu" and not (a.dtype == object and all(
+                    isinstance(x, (int, np.integer)) and not isinstance(x, bool) for x in a.ravel().tolist())):
+                raise ValueError
+            t, num, den = ([int(x) for x in a[:, i].tolist()] for i in range(3))
+        P = operator.index(period)
+    except (TypeError, ValueError, IndexError):
+        raise ValueError("profile: expected (segments, period): (start, gap_num, gap_den) integer triples and an integer") from None
+    if not 1 <= len(t) <= MAX_SEGMENTS:
+        raise ValueError(f"profile: needs 1..{MAX_SEGMENTS} segments, got {len(t)}")
+    if t[0] != 0:
+        raise ValueError("profile: the first segment must start at tick 0")
+    if any(b <= a for a, b in zip(t, t[1:])) or t[-1] >= 2 ** 31 - 1:
+        raise ValueError("profile: segment starts must be strictly increasing and below 2^31 - 1")
+    if any(not 1 <= x <= 2 ** 31 - 1 for x in num + den):
+        raise ValueError("profile: every gap scale needs gap_num and gap_den in 1..2^31 - 1")
+    if P < 0 or P >= 2 ** 31 - 1 or 0 < P <= t[-1]:
+        raise ValueError("profile: the period must be 0, or above the last start and below 2^31 - 1")
+    return t, num, den, P
+
+
+def profile_base(segments, period=0):
+    """the exact host conversion of gs_boot_profiles: base-time starts s_0 = 0,
+    s_(k+1) = s_k + ceil((t_(k+1) - t_k) * den_k / num_k), and B = s_m with t_m := P (0 when P = 0).  Returns (s, B)
+    as Python ints"""
+    t, num, den, P = check_profile(segments, period)
+    s, ends = [0], t[1:] + ([P] if P else [])
+    for k, end in enumerate(ends):
+        s.append(s[-1] + -(-(end - t[k]) * den[k] // num[k]))
+    return s[:len(t)], (s[-1] if P else 0)
+
+
+def profile_arrive(S, segments, period=0):
+    """arrival ticks of base times S >= 0 under a profile: a(S) = t_k + floor((S - s_k) * num_k / den_k) with k the
+    last segment with s_k <= S, and (S div B) * P + a(S mod B) when P > 0.  S: an int (Python-int result, exact) or
+    an int64 array (int64 result; the caller keeps the products below 2^63, as gs_boot_traces_profiled's bound does)"""
+    t, num, den, P = check_profile(segments, period)
+    s, B = profile_base(segments, period)
+    if isinstance(S, (int, np.integer)):
+        S = int(S)
+        q, S = divmod(S, B) if P else (0, S)
+        k = max(i for i in range(len(s)) if s[i] <= S)
+        return q * P + t[k] + (S - s[k]) * num[k] // den[k]
+    S = np.asarray(S, dtype=np.int64)
+    q = np.zeros_like(S)
+    if P:
+        q, S = np.divmod(S, np.int64(B))
+    k = np.searchsorted(np.asarray(s, dtype=np.int64), S, side="right") - 1
+    T, sk, nk, dk = (np.asarray(x, dtype=np.int64)[k] for x in (t, s, num, den))
+    return q * np.int64(P) + T + (S - sk) * nk // dk
+
+
+def profile_bound(n, max_gap, segments, period=0):
+    """the largest arrival tick any profiled replica of n jobs can reach, arrive((n - 1) * max_gap), exactly"""
+    return profile_arrive((int(n) - 1) * int(max_gap), segments, period) if int(n) > 1 else 0
+
+
+def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_len=1, weights=None, profile=None):
     """Replica (seed, stream) of `n` jobs drawn from `population` (JOBIN_DTYPE records of one trace in admission order):
     job j resamples a row and an inter-arrival gap of the population with the Philox4x64-10 block at counter
     (j + 1, 0, 0, 0), and its arrival is floor(gap sum * gap_num / gap_den) (include/gsched.h, gs_boot_traces).
     block_len=L > 1 resamples blocks of consecutive rows of mean length L instead, each row with the gap that preceded
     it in the population (gs_boot_traces_blocked); L = 1 is the iid bootstrap.  weights (one uint32 per population
     row) draws row i with probability w_i / sum(w) through alias_table, at block starts only when blocked
-    (gs_boot_traces_mixed); None is the unweighted bootstrap.  Returns (JOBIN_DTYPE records, source rows)."""
+    (gs_boot_traces_mixed); None is the unweighted bootstrap.  profile=(segments, period) takes the arrivals from a load
+    profile, profile_arrive of the gap sums (gs_boot_traces_profiled; gap_num / gap_den must be 1 / 1), and leaves
+    every other draw as it is.  Returns (JOBIN_DTYPE records, source rows)."""
     from .capi import JOBIN_DTYPE
     pop = np.ascontiguousarray(population, dtype=JOBIN_DTYPE)
     k, n, gap_num, gap_den = len(pop), int(n), int(gap_num), int(gap_den)
@@ -199,7 +270,12 @@ def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_le
         U, A = alias_table(weights)
     gaps = np.diff(pop["arrive_tick"].astype(np.int64))
     max_gap = int(gaps.max()) if len(gaps) else 0
-    if n > 1 and (n - 1) * max_gap * gap_num // gap_den >= 2 ** 31 - 1:
+    if profile is not None:
+        if (gap_num, gap_den) != (1, 1):
+            raise ValueError("bootstrap_packed: a profiled replica needs gap_num / gap_den = 1 / 1")
+        if profile_bound(n, max_gap, *profile) >= 2 ** 31 - 1:
+            raise ValueError("bootstrap_packed: the last arrival tick can reach 2^31 - 1 under the profile")
+    elif n > 1 and (n - 1) * max_gap * gap_num // gap_den >= 2 ** 31 - 1:
         raise ValueError("bootstrap_packed: the last arrival tick can reach 2^31 - 1")
     ctr = np.zeros((n, 4), dtype=np.uint64)
     ctr[:, 0] = np.arange(1, n + 1, dtype=np.uint64)
@@ -218,19 +294,22 @@ def bootstrap_packed(population, seed, stream, n, gap_num=1, gap_den=1, block_le
         gi = mulhi64(w[1:, 1], np.uint64(k - 1)).astype(np.int64)
         g[1:] = gaps[np.where(start[1:] | (rows[1:] == 0), gi, rows[1:] - 1)]
     out = np.zeros(n, dtype=JOBIN_DTYPE)
-    out["arrive_tick"] = np.cumsum(g) * gap_num // gap_den       # below 2^62 by the bound checked above
+    if profile is not None:
+        out["arrive_tick"] = profile_arrive(np.cumsum(g), *profile)
+    else:
+        out["arrive_tick"] = np.cumsum(g) * gap_num // gap_den   # below 2^62 by the bound checked above
     src = pop[rows]
     for f in ("gpus", "gpu_per_task", "mem_bytes", "duration"):
         out[f] = src[f]
     return out, rows
 
 
-def bootstrap_table(base_table, seed, stream, n, gap_num=1, gap_den=1, block_len=1, weights=None):
+def bootstrap_table(base_table, seed, stream, n, gap_num=1, gap_den=1, block_len=1, weights=None, profile=None):
     """bootstrap_packed of a JobTable as a JobTable of its own (labels 0..n-1, the source rows' num_gpu_text and
     utilisation columns, submit = arrive), so that a generated replica can go through the ordinary upload path and
     the ordinary log writers."""
     from .ingest import JobTable
-    recs, rows = bootstrap_packed(base_table.packed(), seed, stream, n, gap_num, gap_den, block_len, weights)
+    recs, rows = bootstrap_packed(base_table.packed(), seed, stream, n, gap_num, gap_den, block_len, weights, profile)
     pick = lambda a: None if a is None else np.ascontiguousarray(np.asarray(a)[rows])
     t = JobTable(
         n=len(recs), label=[str(i) for i in range(len(recs))],

@@ -644,6 +644,40 @@ int gs_boot_mixes(gs_handle h, int32_t nmix, const uint32_t *weights /* nmix * k
 int gs_boot_traces_mixed(gs_handle h, const gs_boot_params *params /* nsims */, const uint32_t *block_len /* NULL = all 1 */,
                          const int32_t *mix /* nsims, -1 = unweighted; NULL = all -1 */, double *kernel_ms);
 
+/* ---- profiled bootstrap replicas: a time-varying offered load ----------------------------------------------
+ * gs_boot_profiles gives the handle nprof load profiles (segs: the nseg[p] segments of every profile p in turn).
+ * Profile p has m = nseg[p] segments, 1 <= m <= GS_BOOT_MAX_SEGMENTS, and a period P = period[p] >= 0.  Segment k
+ * starts at tick t_k = segs[k].start (t_0 = 0, strictly increasing, below 2^31 - 1) and scales the gaps it spans by
+ * gap_num / gap_den (both >= 1; reserved is ignored, set it to 0).  P = 0: the last segment never ends; P > 0: the
+ * profile repeats with period P, t_(m-1) < P < 2^31 - 1.  The host converts each profile once, exactly, to base-time
+ * starts s_0 = 0, s_(k+1) = s_k + ceil((t_(k+1) - t_k) * den_k / num_k), and B = s_m with t_m := P (P > 0), and
+ * uploads them as one device array; nprof = 0 clears them.  Profiles do not depend on the population: a new
+ * gs_boot_population keeps them.
+ * gs_boot_traces_profiled is gs_boot_traces_mixed where replica sim with profile[sim] = p >= 0 takes its arrivals
+ * from profile p: with S the job's gap sum (the base time gs_boot_traces scales by gap_num / gap_den),
+ *   a(S) = t_k + floor((S - s_k) * num_k / den_k), k the last segment with s_k <= S
+ *   arrive = a(S) (P = 0), or (S div B) * P + a(S mod B) (P > 0).
+ * Arrivals never decrease, and the first base time that reaches t_k is s_k, which arrives exactly at t_k (in every
+ * period).  Rows, gaps, block starts and mix picks are those of the same replica without a profile, so the same
+ * (seed, stream) stays coupled across profiles; a profiled replica's params[sim] must have gap_num / gap_den = 1 / 1.
+ * One segment {0, num, den} with P = 0 is the unprofiled replica at gap scale num / den, byte for byte, and a
+ * periodic {0, 1, 1} is the identity.  profile[sim] = -1 (profile NULL: all -1) keeps the replica unprofiled, and a
+ * call without any profile >= 0 is gs_boot_traces_mixed exactly (the same launches).
+ * Errors (nothing changes): gs_boot_profiles: GS_ERR_ARG for nprof < 0, NULL arrays with nprof > 0 or a profile
+ * that breaks a rule above; GS_ERR_CUDA if the profiles cannot be allocated.  gs_boot_traces_profiled: the errors of
+ * gs_boot_traces_mixed, checked in the same order (a profiled replica's arrival bound is its profile's, below), then
+ * GS_ERR_ARG for profile[sim] outside [-1, nprof), a profiled replica whose gap scale is not 1 / 1, and a profiled
+ * replica whose worst-case last arrival arrive((n - 1) * max(D)), computed exactly, reaches 2^31 - 1.          */
+#define GS_BOOT_MAX_SEGMENTS 64
+typedef struct gs_boot_seg {
+  int32_t start, gap_num, gap_den, reserved;
+} gs_boot_seg;              /* 16 bytes */
+int gs_boot_profiles(gs_handle h, int32_t nprof, const int32_t *nseg /* nprof */, const int32_t *period /* nprof */,
+                     const gs_boot_seg *segs /* sum of nseg, profile-major */);
+int gs_boot_traces_profiled(gs_handle h, const gs_boot_params *params /* nsims */, const uint32_t *block_len /* NULL = all 1 */,
+                            const int32_t *mix /* NULL = all -1 */, const int32_t *profile /* nsims, -1 = none; NULL = all -1 */,
+                            double *kernel_ms);
+
 /* Stateless candidate scoring: evaluate b jobs against ONE cluster state.
  * first_node[i] = node of a single-node first fit, or the first node of a
  * cross-node fill, or -1 if the job cannot be placed; task_node (optional)
