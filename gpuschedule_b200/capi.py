@@ -106,6 +106,11 @@ JKEYS = {"gpus": 0, "length": 1, "gpu-time": 2}           # GS_JKEY_GPUS, GS_JKE
 SLOWDOWN_MAX_EDGES = 255
 SLOWDOWN_ONE = 1024                                       # sd units per unit of slowdown
 SLOWDOWN_MAX = 2 ** 31 - 1                                # the saturated sd
+# gs_abin (include/gsched.h): one arrival bin of a replica -- slowdown's record of the bin's finished jobs with the
+# arrival tick as the key, then the jobs of the trace that arrived in the bin, finished or not.
+ABIN_DTYPE = np.dtype([("s", SDCLASS_DTYPE), ("arrived", "<i8")])
+assert ABIN_DTYPE.itemsize == 240
+ARRIVALS_MAX_BINS = 1024
 # gs_occ (include/gsched.h): a replica's rows weighed by the ticks they stand for -- rows weighed, T, the sums of
 # w * busy_gpus / running / queued, the ticks with a queue, the idle GPU-ticks while jobs wait, the maxima and M * G.
 # Histograms come separately as uint64 ticks: busy (replica, [all, waiting], total_gpus + 1), queue (replica, E + 1).
@@ -256,6 +261,9 @@ def declare_horus_prototypes(lib):
     lib.gs_horus_set_slowdown.argtypes = [C.c_void_p, C.c_void_p]
     lib.gs_horus_fetch_slowdown.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.gs_horus_set_slowdown.restype = lib.gs_horus_fetch_slowdown.restype = C.c_int
+    lib.gs_horus_set_arrivals.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int64]
+    lib.gs_horus_fetch_arrivals.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+    lib.gs_horus_set_arrivals.restype = lib.gs_horus_fetch_arrivals.restype = C.c_int
     lib.gs_horus_set_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.gs_horus_fetch_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     lib.gs_horus_set_occupancy.restype = lib.gs_horus_fetch_occupancy.restype = C.c_int
@@ -339,6 +347,9 @@ def load_library():
     lib.gs_set_slowdown.argtypes = [C.c_void_p, C.c_void_p]
     lib.gs_fetch_slowdown.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.gs_set_slowdown.restype = lib.gs_fetch_slowdown.restype = C.c_int
+    lib.gs_set_arrivals.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int64]
+    lib.gs_fetch_arrivals.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    lib.gs_set_arrivals.restype = lib.gs_fetch_arrivals.restype = C.c_int
     lib.gs_set_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.gs_fetch_occupancy.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     lib.gs_set_occupancy.restype = lib.gs_fetch_occupancy.restype = C.c_int
@@ -595,6 +606,16 @@ class HorusEngine:
         summarize()"""
         return _fetch_slowdown(self, self.lib.gs_horus_fetch_slowdown, "gs_horus_fetch_slowdown", first, count)
 
+    def set_arrivals(self, width, bins, tau=1):
+        """job statistics by arrival time, filled by every summarize(): `bins` bins of `width` ticks by
+        min(arrival // width, bins - 1), bounded slowdown with lower bound tau; bins = 0 turns it off
+        (include/gsched_horus.h: gs_horus_set_arrivals)"""
+        _set_arrivals(self, self.lib.gs_horus_set_arrivals, "gs_horus_set_arrivals", width, bins, tau)
+
+    def arrivals(self, first=0, count=None):
+        """ABIN_DTYPE records (count, bins) as of the last summarize()"""
+        return _fetch_arrivals(self, self.lib.gs_horus_fetch_arrivals, "gs_horus_fetch_arrivals", first, count)
+
     def set_occupancy(self, queue_edges=None):
         """time-weighted occupancy filled by every summarize(), with queue-length CDF counts at `queue_edges`;
         None turns it off (include/gsched_horus.h: gs_horus_set_occupancy)"""
@@ -658,6 +679,22 @@ def _set_jobdist(eng, fn, what, bounds, edges):
     eng._check(fn(eng.h, len(b) + 1, b.ctypes.data_as(C.c_void_p) if len(b) else None, len(e),
                   e.ctypes.data_as(C.c_void_p) if len(e) else None), what)
     eng._jd_shape = (len(b) + 1, len(e))
+
+
+def _set_arrivals(eng, fn, what, width, bins, tau):
+    bins, width, tau = int(bins), int(width), int(tau)
+    if not (-2 ** 31 <= bins < 2 ** 31 and -2 ** 63 <= width < 2 ** 63 and -2 ** 63 <= tau < 2 ** 63):
+        raise GsError(what + ": bins must be int32, width and tau int64", GS_ERR_ARG)
+    eng._check(fn(eng.h, int(width), bins, int(tau)), what)
+    eng._arr_bins = bins
+
+
+def _fetch_arrivals(eng, fn, what, first, count):
+    count = eng.nsims - first if count is None else int(count)
+    nb = getattr(eng, "_arr_bins", 0)
+    out = np.zeros((max(count, 1), max(nb, 1)), dtype=ABIN_DTYPE)
+    eng._check(fn(eng.h, int(first), count, out.ctypes.data_as(C.c_void_p)), what)
+    return out[:count, :nb]
 
 
 def slowdown_cfg(key, bounds=(), tau=1, edges=(), sd_edges=()):
@@ -1137,6 +1174,17 @@ class Engine:
         and jct rows of E + 1 counts, then the sd row of Esd + 1) of replicas [first, first+count) as of the last
         summarize()"""
         return _fetch_slowdown(self, self.lib.gs_fetch_slowdown, "gs_fetch_slowdown", first, count)
+
+    def set_arrivals(self, width, bins, tau=1):
+        """while bins > 0, every summarize() also computes per-replica job statistics by arrival time on the device:
+        a job that arrived at tick a falls in bin min(a // width, bins - 1), and each bin holds slowdown's record of
+        its finished jobs (bounded slowdown with lower bound tau, the arrival tick as the key) and the count of its
+        trace jobs; bins = 0 turns it off.  May be called at any time (include/gsched.h: gs_set_arrivals)"""
+        _set_arrivals(self, self.lib.gs_set_arrivals, "gs_set_arrivals", width, bins, tau)
+
+    def arrivals(self, first=0, count=None):
+        """ABIN_DTYPE records (count, bins) of replicas [first, first+count) as of the last summarize()"""
+        return _fetch_arrivals(self, self.lib.gs_fetch_arrivals, "gs_fetch_arrivals", first, count)
 
     def set_occupancy(self, queue_edges=None):
         """time-weighted occupancy filled by every summarize(): each row weighed by the ticks it stands for, busy-GPU

@@ -102,6 +102,7 @@ struct GsSumHorusJobs {
   __device__ long long n(int r) const { return sims[r].n; }
   __device__ int order(int r, long long i) const { return sims[r].fin[i]; }
   __device__ GsSumJob job(int r, long long i) const { return job_at(r, sims[r].fin[i]); }
+  __device__ int arrive_at(int r, int j) const { return sims[r].jobs[j].arrive; }
   __device__ bool same_job(int ra, int rb, int j) const { return gs_hjob_same(sims[ra].jobs[j], sims[rb].jobs[j]); }
   __device__ GsSumJob job_at(int r, int j) const {
     const HSim &S = sims[r];
@@ -128,6 +129,7 @@ struct HorusSimHost {
   bool tl_done = false;             // summarised with the timeline on since it was prepared
   bool jd_done = false;             // summarised with the current jobdist setting since it was prepared
   bool sd_done = false;             // summarised with the current slowdown setting since it was prepared
+  bool arr_done = false;            // summarised with the current arrivals setting since it was prepared
   bool occ_done = false;            // summarised with the occupancy on since it was prepared
   bool if_done = false;             // summarised with the current interference setting since it was prepared
   gs_cluster cl{};
@@ -162,6 +164,8 @@ struct gs_horus_handle_s {
   gs_sdclass *d_sd = nullptr; size_t sd_bytes = 0;      // gs_horus_set_slowdown: nsims x C class records
   unsigned *d_sd_hist = nullptr; size_t sd_hist_bytes = 0;   // and nsims x C x (3 (E + 1) + Esd + 1) CDF counts
   GsSdCfg sd{};                                          // sd.nclasses = 0: off
+  gs_abin *d_arr = nullptr; size_t arr_bytes = 0;       // gs_horus_set_arrivals: nsims x B bin records, only while on
+  GsArrCfg arr{};                                        // arr.nbins = 0: off
   bool occ_on = false; GsOccCfg occ{};                   // gs_horus_set_occupancy
   gs_occ *d_occ = nullptr;                               // nsims records
   unsigned long long *d_occ_busy = nullptr; int64_t occ_pitch = 0;   // nsims x [H_all, H_wait] x occ_pitch counters
@@ -221,6 +225,7 @@ extern "C" int gs_horus_destroy(gs_horus_handle h) {
   if (h->d_jd_hist) cudaFree(h->d_jd_hist);
   if (h->d_sd) cudaFree(h->d_sd);
   if (h->d_sd_hist) cudaFree(h->d_sd_hist);
+  if (h->d_arr) cudaFree(h->d_arr);
   if (h->d_occ) cudaFree(h->d_occ);
   if (h->d_occ_busy) cudaFree(h->d_occ_busy);
   if (h->d_occ_q) cudaFree(h->d_occ_q);
@@ -414,7 +419,7 @@ static int prepare(gs_horus_handle h, HorusSimHost &s, long long rows_cap) {
   D.rows_cap = rows_cap;
   D.current_remaining = (long long)n; D.running_jobs = 0;
   s.rows_cap = rows_cap;
-  s.prepared = true; s.tl_done = false; s.jd_done = false; s.sd_done = false; s.occ_done = false; s.if_done = false;
+  s.prepared = true; s.tl_done = false; s.jd_done = false; s.sd_done = false; s.arr_done = false; s.occ_done = false; s.if_done = false;
   return GS_OK;
 }
 
@@ -538,13 +543,21 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
   HCU(cudaMemsetAsync(h->d_sum + first, 0, sizeof(gs_summary) * (size_t)count, h->stream));
   const int B = h->tl_nbins;
   if (B > 0) HCU(cudaMemsetAsync(h->d_tl + (size_t)first * B, 0, sizeof(gs_tbin) * (size_t)B * (size_t)count, h->stream));
-  const int C = h->jd.nclasses, Csd = h->sd.nclasses, Cif = h->ifc.nclasses;
+  const int C = h->jd.nclasses, Csd = h->sd.nclasses, Cif = h->ifc.nclasses, Barr = h->arr.nbins;
 #ifdef __CUDACC__
   int per_sm = 1, sms = 132;
   HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gs_sum_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   const int grid = std::min(count, std::max(1, per_sm) * sms);
-  const size_t pitch = (size_t)(kmax + 63) / 64 * 64, need = (Cif > 0 ? GS_IF_ROWS : Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid;
+  int grid_arr = 0;
+  if (Barr > 0) {
+    int per_arr = 1;
+    HCU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_arr, gs_arr_jobs_kernel<GsSumHorusJobs>, GS_SUM_THREADS, 0));
+    grid_arr = std::min(grid, std::max(1, per_arr) * sms);
+  }
+  const size_t pitch = (size_t)(kmax + 63) / 64 * 64;
+  const size_t need = std::max((Cif > 0 ? GS_IF_ROWS : Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid,
+                               GS_ARR_ROWS * sizeof(int) * pitch * (size_t)grid_arr);   // gs_arr_jobs_kernel: its own rows
   if (h->sum_scratch_bytes < need) {
     if (h->d_sum_scratch) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_sum_scratch); }
     h->d_sum_scratch = nullptr; h->sum_scratch_bytes = 0;
@@ -582,6 +595,12 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     const int grid_if = std::min(grid, std::max(1, per_if) * sms);
     gs_if_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid_if, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->ifc,
                                                                                           h->d_if, h->d_sum_scratch, (long long)pitch);
+    HCU(cudaGetLastError());
+    h->launches += 1;
+  }
+  if (Barr > 0) {         // after the other job kernels, on the same scratch with GS_ARR_ROWS rows
+    gs_arr_jobs_kernel<GsSumHorusJobs><<<(unsigned)grid_arr, GS_SUM_THREADS, 0, h->stream>>>(GsSumHorusJobs{h->d_sims}, first, count, h->arr,
+                                                                                            h->d_arr, h->d_sum_scratch, (long long)pitch);
     HCU(cudaGetLastError());
     h->launches += 1;
   }
@@ -623,6 +642,13 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
       }
       gs_if_serial(jobs.data(), durs.data(), S.nfin, h->ifc, h->d_if + (size_t)r * Cif);
     }
+    if (Barr > 0) {
+      const int n = std::max(S.n, 0);
+      std::vector<int> fin_arrive((size_t)S.nfin), trace_arrive((size_t)n);
+      for (int i = 0; i < S.nfin; ++i) fin_arrive[(size_t)i] = S.jobs[S.fin[i]].arrive;
+      for (int j = 0; j < n; ++j) trace_arrive[(size_t)j] = S.jobs[j].arrive;
+      gs_arr_serial(jobs.data(), fin_arrive.data(), S.nfin, trace_arrive.data(), n, h->arr, h->d_arr + (size_t)r * Barr);
+    }
     if (B > 0) gs_tl_fold_rows_serial(h->d_tl + (size_t)r * B, B, (long long)h->tl_width, S.rows, S.util, 0, 0, S.ticks);
     if (h->occ_on) {
       gs_occ &o = h->d_occ[r];
@@ -646,6 +672,7 @@ extern "C" int gs_horus_summarize(gs_horus_handle h, int32_t first, int32_t coun
     if (B > 0) h->sims[(size_t)i].tl_done = true;
     if (C > 0) h->sims[(size_t)i].jd_done = true;
     if (Csd > 0) h->sims[(size_t)i].sd_done = true;
+    if (Barr > 0) h->sims[(size_t)i].arr_done = true;
     if (h->occ_on) h->sims[(size_t)i].occ_done = true;
     if (Cif > 0) h->sims[(size_t)i].if_done = true;
   }
@@ -774,6 +801,53 @@ extern "C" int gs_horus_fetch_slowdown(gs_horus_handle h, int32_t first, int32_t
     HCU(cudaMemcpyAsync(out, h->d_sd + (size_t)first * C, sizeof(gs_sdclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   if (hist_out)
     HCU(cudaMemcpyAsync(hist_out, h->d_sd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  HCU(cudaStreamSynchronize(h->stream));
+  return GS_OK;
+}
+
+extern "C" int gs_horus_set_arrivals(gs_horus_handle h, int64_t bin_width, int32_t nbins, int64_t tau) {
+  if (!h) return GS_ERR_ARG;
+  GsArrCfg cfg;
+  const char *why = nullptr;
+  if (!gs_arr_make_cfg(bin_width, nbins, tau, cfg, &why)) return hfail(h, GS_ERR_ARG, std::string("gs_horus_set_arrivals: ") + why);
+  HCU(cudaSetDevice(h->device));
+  const size_t need = sizeof(gs_abin) * h->sims.size() * (size_t)cfg.nbins;
+  if (need > h->arr_bytes) {
+    bool fits = true;
+#ifdef __CUDACC__
+    size_t free_b = 0, total_b = 0;
+    HCU(cudaMemGetInfo(&free_b, &total_b));
+    fits = need <= free_b;
+#endif
+    gs_abin *d = nullptr;
+    if (!fits || cudaMalloc(&d, need) != cudaSuccess) {
+      (void)cudaGetLastError();
+      return hfail(h, GS_ERR_CAPACITY, "gs_horus_set_arrivals: the bin records (" + std::to_string(need) + " bytes) do not fit the device's free memory");
+    }
+    if (h->d_arr) { HCU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_arr); }
+    h->d_arr = d; h->arr_bytes = need;
+  } else if (cfg.nbins == 0 && h->d_arr) {           // off: the records are not kept
+    HCU(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_arr);
+    h->d_arr = nullptr; h->arr_bytes = 0;
+  }
+  h->arr = cfg;
+  for (auto &s : h->sims) s.arr_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_horus_fetch_arrivals(gs_horus_handle h, int32_t first, int32_t count, gs_abin *out) {
+  if (!h) return GS_ERR_ARG;
+  const int nsims = (int)h->sims.size();
+  if (first < 0 || count < 0 || first > nsims - count || (count > 0 && !out)) return hfail(h, GS_ERR_ARG, "gs_horus_fetch_arrivals: bad arguments");
+  if (h->arr.nbins == 0) return hfail(h, GS_ERR_STATE, "gs_horus_fetch_arrivals: the arrival statistics are off (gs_horus_set_arrivals)");
+  for (int i = first; i < first + count; ++i)
+    if (!h->sims[(size_t)i].prepared || !h->sims[(size_t)i].arr_done)
+      return hfail(h, GS_ERR_STATE, "gs_horus_fetch_arrivals: a replica has not been summarised with this setting since it was prepared");
+  if (count == 0) return GS_OK;
+  HCU(cudaSetDevice(h->device));
+  const size_t B = (size_t)h->arr.nbins;
+  HCU(cudaMemcpyAsync(out, h->d_arr + (size_t)first * B, sizeof(gs_abin) * B * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   HCU(cudaStreamSynchronize(h->stream));
   return GS_OK;
 }

@@ -355,6 +355,31 @@ static inline bool gs_sd_make_cfg(const gs_slowdown_cfg *in, GsSdCfg &cfg, const
 // uint32 counts per (replica, class): wait, turnaround and jct E + 1 each, then sd Esd + 1.
 GS_SUM_HD long long gs_sd_row_len(const GsSdCfg &cfg) { return 3ll * (cfg.nedges + 1) + cfg.nsd + 1; }
 
+// ---- job statistics by arrival time (gs_abin, include/gsched.h)
+static_assert(sizeof(gs_abin) == 240 && sizeof(gs_abin) % 8 == 0, "gs_abin is 240 bytes, a multiple of 8");
+#define GS_ARR_ROWS 7                // scratch rows per job: wait, turnaround, jct, sd, preempt, gpus, arrival tick
+#define GS_ARR_CUT 256               // a bin of at most this many finished jobs is finished by one warp, larger ones by the block
+
+// An arrivals setting; nbins = 0: off.  A job's bin is gs_tl_bin(arrival tick, width, nbins), the timeline's rule.
+struct GsArrCfg {
+  long long width, tau;
+  int nbins;
+};
+
+// An arrivals setting from the C ABI's arguments, or false (the message in *why) when it is not valid.
+static inline bool gs_arr_make_cfg(long long width, int nbins, long long tau, GsArrCfg &cfg, const char **why) {
+  cfg = GsArrCfg{};
+  *why = "nbins must be in 0..1024";
+  if (nbins < 0 || nbins > GS_ARRIVALS_MAX_BINS) return false;
+  if (nbins == 0) return true;
+  *why = "bin_width must be >= 1";
+  if (width < 1) return false;
+  *why = "tau must be >= 1";
+  if (tau < 1) return false;
+  cfg.width = width; cfg.tau = tau; cfg.nbins = nbins;
+  return true;
+}
+
 // ---- time-weighted occupancy (gs_occ, include/gsched.h)
 static_assert(sizeof(gs_occ) == 72, "gs_occ is 72 bytes");
 #define GS_OCC_MAX_GPUS 65535
@@ -697,6 +722,31 @@ static inline void gs_sd_serial(const GsSumJob *jobs, long long k, const GsSdCfg
     gs_sum_select_serial(seg + pitch, kc, J.turnaround_q);
     gs_sum_select_serial(seg + 2 * pitch, kc, J.jct_q);
     gs_sum_select_serial(seg + 3 * pitch, kc, S.sd_q);
+  }
+}
+
+// Arrival-bin statistics of k finished jobs (jobs[i] arrived at tick arrive[i], in finish order) of a trace whose n
+// jobs arrived at trace_arrive[0 .. n): out[0 .. B) (overwritten).  Each bin's finished jobs are one class of
+// gs_sd_serial (no edges), whose key sum is then replaced by the sum of their arrival ticks.
+static inline void gs_arr_serial(const GsSumJob *jobs, const int *arrive, long long k, const int *trace_arrive, long long n,
+                                 const GsArrCfg &cfg, gs_abin *out) {
+  const int B = cfg.nbins;
+  GsSdCfg one{};
+  one.key = GS_JKEY_GPUS; one.nclasses = 1; one.tau = cfg.tau;
+  std::vector<std::vector<GsSumJob>> bins((size_t)B);
+  std::vector<long long> key((size_t)B, 0);
+  for (int b = 0; b < B; ++b) out[b] = gs_abin{};
+  for (long long j = 0; j < n; ++j) out[gs_tl_bin(trace_arrive[j], cfg.width, B)].arrived += 1;
+  for (long long i = 0; i < k; ++i) {
+    const int b = gs_tl_bin(arrive[i], cfg.width, B);
+    bins[(size_t)b].push_back(jobs[i]);
+    key[(size_t)b] += arrive[i];
+  }
+  uint32_t hist[4];
+  for (int b = 0; b < B; ++b) {
+    gs_sd_serial(bins[(size_t)b].data(), (long long)bins[(size_t)b].size(), one, &out[b].s, hist);
+    out[b].s.key_sum_lo = out[b].s.key_sum_hi = 0;
+    gs_sum_add128(out[b].s.key_sum_lo, out[b].s.key_sum_hi, (gs_i128)key[(size_t)b]);
   }
 }
 // Interference statistics of k finished jobs (jobs[i] and durs[i] of the same job): out[0 .. C) (overwritten).  Each
@@ -1436,6 +1486,247 @@ __global__ void __launch_bounds__(GS_SUM_THREADS) gs_sd_jobs_kernel(Src src, int
       __syncthreads();
       off += kc;
     }
+  }
+}
+
+// ---- job statistics by arrival time.  Every lane of a warp calls gs_arr_count with its bin (b < 0: nothing to
+// count); the lanes of one bin add once.
+__device__ __forceinline__ void gs_arr_count(unsigned *ctr, int b) {
+  const unsigned peers = __match_any_sync(0xffffffffu, b);
+  if (b >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&ctr[b], (unsigned)__popc(peers));
+}
+
+// Bitonic sort of buf[0 .. P) ascending by one warp (P a power of two, 2 <= P); every lane calls it, after a __syncwarp
+// that publishes buf, and returns after one.
+__device__ __forceinline__ void gs_arr_warp_sort(int *buf, int P) {
+  const int lane = threadIdx.x & 31;
+  for (int size = 2; size <= P; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = lane; t < P / 2; t += 32) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;   // the pair (lo, lo + stride), lo's stride bit clear
+        const int x = buf[lo], y = buf[hi];
+        if ((x > y) == ((lo & size) == 0)) { buf[lo] = y; buf[hi] = x; }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// One bin of m <= GS_ARR_CUT finished jobs, seg[row * pitch + i] (i < m, rows as in gs_arr_jobs_kernel), finished by
+// one warp: the sums by lane partials and shuffles; then each value row copied to buf (GS_ARR_CUT ints), padded with
+// 2^31 - 1 to a power of two, sorted, and the five ranks read off (the padding sorts last, past every rank < m).  The
+// record is staged in *wr (shared) and copied to *out as 30 words.  Every lane calls it.
+__device__ void gs_arr_warp_bin(const int *seg, long long pitch, int m, unsigned arrived, int *buf, gs_abin *wr, gs_abin *out) {
+  const int lane = threadIdx.x & 31;
+  // wait, turnaround, jct, sd: sums, square high halves, square low halves; then saturated sd, preempt, gpu ticks, arrivals
+  long long a[16];
+#pragma unroll
+  for (int e = 0; e < 16; ++e) a[e] = 0;
+  for (int i = lane; i < m; i += 32) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int v = seg[c * pitch + i];
+      const unsigned long long sq = (unsigned long long)((long long)v * v);
+      a[c] += v; a[4 + c] += (long long)(sq >> 32); a[8 + c] += (long long)(sq & 0xffffffffull);
+    }
+    a[12] += seg[3 * pitch + i] == (int)GS_SD_MAX;
+    a[13] += seg[4 * pitch + i];
+    a[14] += (long long)seg[5 * pitch + i] * seg[2 * pitch + i];
+    a[15] += seg[6 * pitch + i];
+  }
+#pragma unroll
+  for (int e = 0; e < 16; ++e)
+    for (int o = 16; o > 0; o >>= 1) a[e] += __shfl_xor_sync(0xffffffffu, a[e], o);
+  unsigned long long *w = reinterpret_cast<unsigned long long *>(wr);
+  if (lane < (int)(sizeof(gs_abin) / 8)) w[lane] = 0;
+  __syncwarp();
+  if (lane == 0) {
+    gs_jclass &J = wr->s.jc;
+    J.jobs = m; J.wait_sum = a[0]; J.turnaround_sum = a[1]; J.jct_sum = a[2]; J.preempt_sum = a[13]; J.gpu_ticks_sum = a[14];
+    gs_sum_add128(J.wait_sq_lo, J.wait_sq_hi, ((gs_i128)a[4] << 32) + a[8]);
+    gs_sum_add128(J.turnaround_sq_lo, J.turnaround_sq_hi, ((gs_i128)a[5] << 32) + a[9]);
+    gs_sum_add128(J.jct_sq_lo, J.jct_sq_hi, ((gs_i128)a[6] << 32) + a[10]);
+    wr->s.sd_sum = a[3];
+    gs_sum_add128(wr->s.sd_sq_lo, wr->s.sd_sq_hi, ((gs_i128)a[7] << 32) + a[11]);
+    wr->s.sd_clamped = a[12];
+    gs_sum_add128(wr->s.key_sum_lo, wr->s.key_sum_hi, (gs_i128)a[15]);
+    wr->arrived = arrived;
+  }
+  if (m > 0) {
+    int P = 32;
+    while (P < m) P <<= 1;
+    for (int c = 0; c < 4; ++c) {
+      for (int i = lane; i < P; i += 32) buf[i] = i < m ? seg[c * pitch + i] : 0x7fffffff;
+      __syncwarp();
+      gs_arr_warp_sort(buf, P);
+      if (lane < 5) {
+        int *q = c == 0 ? wr->s.jc.wait_q : c == 1 ? wr->s.jc.turnaround_q : c == 2 ? wr->s.jc.jct_q : wr->s.sd_q;
+        q[lane] = buf[gs_sum_rank(gs_sum_permille(lane), m)];
+      }
+      if (c == 3 && lane == 0) wr->s.sd_min = buf[0];
+      __syncwarp();                                         // buf is read before the next row overwrites it
+    }
+  }
+  __syncwarp();
+  if (lane < (int)(sizeof(gs_abin) / 8)) reinterpret_cast<unsigned long long *>(out)[lane] = w[lane];
+  __syncwarp();                                             // *wr is read before the warp's next bin
+}
+
+// Arrival-bin statistics (gs_abin) of replicas first .. first + count - 1 (the jobs of gs_sum_jobs_kernel), one block
+// per replica in turn (grid-stride).  Src supplies n(r), finished(r), order(r, i), job_at(r, j) and arrive_at(r, j).
+// Its own scratch: GS_ARR_ROWS * pitch ints per block, rows wait, turnaround, jct, sd, preempt, gpus, arrival tick.
+// (1) finished jobs per bin, and every trace job per bin (`arrived`), in shared counters (warp-aggregated adds);
+// (2) an exclusive scan of the finished counts gives each bin's segment; (3) every finished job's seven values are
+// written to its bin's segment through warp-aggregated shared cursors (the order inside a segment is free, nothing
+// depends on it); (4) each bin of at most GS_ARR_CUT jobs is finished by one warp (gs_arr_warp_bin: sums by shuffles,
+// order statistics by a bitonic sort in shared memory), eight bins in flight; (5) each larger bin is finished by the
+// block, as gs_sd_jobs_kernel finishes a class: sums, minima and maxima block-reduced, gs_sum_select over the three
+// rows and a one-row gs_sum_select over sd.  Both paths are exact, so a bin's record does not depend on its path.
+// The warps' sort buffers and staging records live in the selects' histogram space, which (4) and (5) use in turn.
+template <class Src>
+__global__ void __launch_bounds__(GS_SUM_THREADS) gs_arr_jobs_kernel(Src src, int first, int count, GsArrCfg cfg, gs_abin *recs,
+                                                                    int *scratch, long long pitch) {
+  constexpr int NW = GS_SUM_THREADS / 32;
+  static_assert(GS_ARRIVALS_MAX_BINS <= 4 * GS_SUM_THREADS, "the scan takes four bins per thread");
+  static_assert(NW * (GS_ARR_CUT * sizeof(int) + sizeof(gs_abin)) <= GS_SUM_TARGETS * GS_SUM_BINS * sizeof(unsigned),
+                "the warps' buffers fit the histogram space");
+  __shared__ __align__(16) unsigned hist[GS_SUM_TARGETS * GS_SUM_BINS];
+  __shared__ unsigned long long prefix[GS_SUM_TARGETS];
+  __shared__ unsigned cnt[GS_ARRIVALS_MAX_BINS + 1];      // finished jobs per bin, then the segments' first positions
+  __shared__ unsigned cursor[GS_ARRIVALS_MAX_BINS];
+  __shared__ unsigned arrived[GS_ARRIVALS_MAX_BINS];
+  __shared__ unsigned wtot[NW];
+  __shared__ gs_abin rec;
+  const int B = cfg.nbins, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int *buf = reinterpret_cast<int *>(hist) + warp * GS_ARR_CUT;
+  gs_abin *wr = reinterpret_cast<gs_abin *>(hist + NW * GS_ARR_CUT) + warp;
+  int *vals = scratch + (size_t)blockIdx.x * GS_ARR_ROWS * (size_t)pitch;
+  for (int rb = blockIdx.x; rb < count; rb += gridDim.x) {
+    const int r = first + rb;
+    const long long n = src.n(r), k = src.finished(r);
+    for (int i = threadIdx.x; i < B; i += blockDim.x) { cnt[i] = 0; arrived[i] = 0; }
+    __syncthreads();
+    for (long long i0 = 0; i0 < n; i0 += blockDim.x) {     // (warp-uniform trip count: the matches see full warps)
+      const long long i = i0 + threadIdx.x;
+      gs_arr_count(arrived, i < n ? gs_tl_bin(src.arrive_at(r, (int)i), cfg.width, B) : -1);
+      gs_arr_count(cnt, i < k ? gs_tl_bin(src.arrive_at(r, src.order(r, i)), cfg.width, B) : -1);
+    }
+    __syncthreads();
+    {                                                       // cnt[b] := jobs of bins < b; cnt[B] = k
+      unsigned v[4], sum = 0;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int b = 4 * threadIdx.x + q;
+        v[q] = b < B ? cnt[b] : 0u;
+        sum += v[q];
+      }
+      unsigned inc = sum;
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += t;
+      }
+      if (lane == 31) wtot[warp] = inc;
+      __syncthreads();
+      unsigned base = inc - sum;
+      for (int u = 0; u < warp; ++u) base += wtot[u];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int b = 4 * threadIdx.x + q;
+        if (b < B) { cnt[b] = base; cursor[b] = base; }
+        base += v[q];
+      }
+      if (threadIdx.x == 0) cnt[B] = (unsigned)k;
+    }
+    __syncthreads();
+    for (long long i0 = 0; i0 < k; i0 += blockDim.x) {     // (warp-uniform trip count: the shuffles see full warps)
+      const long long i = i0 + threadIdx.x;
+      const bool in = i < k;
+      GsSumJob v;
+      int a = 0, b = -1;
+      if (in) {
+        const int j = src.order(r, i);
+        v = src.job_at(r, j);
+        a = src.arrive_at(r, j);
+        b = gs_tl_bin(a, cfg.width, B);
+      }
+      const unsigned peers = __match_any_sync(0xffffffffu, b);
+      const int head = __ffs(peers) - 1;
+      unsigned base = 0;
+      if (in && lane == head) base = atomicAdd(&cursor[b], (unsigned)__popc(peers));
+      base = __shfl_sync(0xffffffffu, base, head);
+      if (in) {
+        const long long pos = (long long)base + __popc(peers & ((1u << lane) - 1u));
+        vals[pos] = v.wait; vals[pitch + pos] = v.turn; vals[2 * pitch + pos] = v.jct;
+        vals[3 * pitch + pos] = gs_sd_value(v.turn, v.jct, cfg.tau);
+        vals[4 * pitch + pos] = v.preempt; vals[5 * pitch + pos] = v.gpus; vals[6 * pitch + pos] = a;
+      }
+    }
+    __syncthreads();
+    for (int b = warp; b < B; b += NW) {
+      const int o = (int)cnt[b], m = (int)(cnt[b + 1] - cnt[b]);
+      if (m <= GS_ARR_CUT) gs_arr_warp_bin(vals + o, pitch, m, arrived[b], buf, wr, recs + (size_t)r * B + b);
+    }
+    __syncthreads();                                        // the warps are done with the histogram space
+    for (int b = 0; b < B; ++b) {                           // (uniform: every thread reads the same counts)
+      const long long o = cnt[b], m = (long long)cnt[b + 1] - o;
+      if (m <= GS_ARR_CUT) continue;
+      const int *seg = vals + o;
+      // wait, turnaround, jct: sums, square high halves, square low halves; preempt, gpu ticks, arrivals; minima; maxima
+      long long s[18] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0x7fffffff, 0x7fffffff, 0x7fffffff, -0x80000000ll, -0x80000000ll, -0x80000000ll};
+      for (long long i = threadIdx.x; i < m; i += blockDim.x) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const int v = seg[c * pitch + i];
+          const unsigned long long sq = (unsigned long long)((long long)v * v);
+          s[c] += v; s[3 + c] += (long long)(sq >> 32); s[6 + c] += (long long)(sq & 0xffffffffull);
+          s[12 + c] = min(s[12 + c], (long long)v); s[15 + c] = max(s[15 + c], (long long)v);
+        }
+        s[9] += seg[4 * pitch + i];
+        s[10] += (long long)seg[5 * pitch + i] * seg[2 * pitch + i];
+        s[11] += seg[6 * pitch + i];
+      }
+      gs_sum_block_vec<18, 12, 3>(s);
+      // sd: sum, square halves, saturated count, minimum, maximum
+      long long t[6] = {0, 0, 0, 0, GS_SD_MAX, 0};
+      for (long long i = threadIdx.x; i < m; i += blockDim.x) {
+        const int v = seg[3 * pitch + i];
+        const unsigned long long sq = (unsigned long long)((long long)v * v);
+        t[0] += v; t[1] += (long long)(sq >> 32); t[2] += (long long)(sq & 0xffffffffull); t[3] += v == (int)GS_SD_MAX;
+        t[4] = min(t[4], (long long)v); t[5] = max(t[5], (long long)v);
+      }
+      gs_sum_block_vec<6, 4, 1>(t);
+      long long span = 0;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) span = max(span, s[15 + c] - s[12 + c]);
+      gs_sum_select(hist, prefix, seg, pitch, m, s + 12, span);
+      if (threadIdx.x == 0) {
+        rec = gs_abin{};
+        gs_jclass &J = rec.s.jc;
+        J.jobs = m; J.wait_sum = s[0]; J.turnaround_sum = s[1]; J.jct_sum = s[2]; J.preempt_sum = s[9]; J.gpu_ticks_sum = s[10];
+        gs_sum_add128(J.wait_sq_lo, J.wait_sq_hi, ((gs_i128)s[3] << 32) + s[6]);
+        gs_sum_add128(J.turnaround_sq_lo, J.turnaround_sq_hi, ((gs_i128)s[4] << 32) + s[7]);
+        gs_sum_add128(J.jct_sq_lo, J.jct_sq_hi, ((gs_i128)s[5] << 32) + s[8]);
+        for (int q = 0; q < 5; ++q) {
+          J.wait_q[q] = (int)(s[12] + (long long)prefix[q]);
+          J.turnaround_q[q] = (int)(s[13] + (long long)prefix[5 + q]);
+          J.jct_q[q] = (int)(s[14] + (long long)prefix[10 + q]);
+        }
+        rec.s.sd_sum = t[0];
+        gs_sum_add128(rec.s.sd_sq_lo, rec.s.sd_sq_hi, ((gs_i128)t[1] << 32) + t[2]);
+        rec.s.sd_clamped = t[3];
+        rec.s.sd_min = (int)t[4];
+        gs_sum_add128(rec.s.key_sum_lo, rec.s.key_sum_hi, (gs_i128)s[11]);
+        rec.arrived = arrived[b];
+      }
+      __syncthreads();                                      // thread 0 has read prefix before the second select
+      gs_sum_select<1>(hist, prefix, seg + 3 * pitch, pitch, m, t + 4, t[5] - t[4]);
+      if (threadIdx.x == 0) {
+        for (int q = 0; q < 5; ++q) rec.s.sd_q[q] = (int)(t[4] + (long long)prefix[q]);
+        recs[(size_t)r * B + b] = rec;
+      }
+      __syncthreads();
+    }
+    __syncthreads();                                        // every thread has read cnt before the next replica clears it
   }
 }
 

@@ -87,6 +87,7 @@ struct SimHost {
   bool tl_done = false;                   // summarised with the timeline on since it was prepared
   bool jd_done = false;                   // summarised with the current jobdist setting since it was prepared
   bool sd_done = false;                   // summarised with the current slowdown setting since it was prepared
+  bool arr_done = false;                  // summarised with the current arrivals setting since it was prepared
   bool occ_fresh = true;                  // the occupancy record, carry and histograms are to be zeroed before the next fold
   bool occ_done = false;                  // summarised with the occupancy on since it was prepared
   SimDev dev;
@@ -131,6 +132,8 @@ struct gs_engine {
   gs_sdclass *d_sd = nullptr; size_t sd_bytes = 0;      // gs_set_slowdown: nsims x C class records
   unsigned *d_sd_hist = nullptr; size_t sd_hist_bytes = 0;   // and nsims x C x (3 (E + 1) + Esd + 1) CDF counts
   GsSdCfg sd{};                                          // sd.nclasses = 0: off
+  gs_abin *d_arr = nullptr; size_t arr_bytes = 0;       // gs_set_arrivals: nsims x B bin records, only while on
+  GsArrCfg arr{};                                        // arr.nbins = 0: off
   bool occ_on = false; GsOccCfg occ{};                   // gs_set_occupancy
   gs_occ *d_occ = nullptr; GsOccCarry *d_occ_carry = nullptr;   // nsims records and carries
   unsigned long long *d_occ_busy = nullptr; int64_t occ_pitch = 0;   // nsims x [H_all, H_wait] x occ_pitch counters
@@ -223,6 +226,7 @@ extern "C" void gs_destroy(gs_handle h) {
   if (h->d_jd_hist) cudaFree(h->d_jd_hist);
   if (h->d_sd) cudaFree(h->d_sd);
   if (h->d_sd_hist) cudaFree(h->d_sd_hist);
+  if (h->d_arr) cudaFree(h->d_arr);
   if (h->d_occ) cudaFree(h->d_occ);
   if (h->d_occ_carry) cudaFree(h->d_occ_carry);
   if (h->d_occ_busy) cudaFree(h->d_occ_busy);
@@ -558,7 +562,7 @@ static int bind_sim(gs_handle h, SimHost &s, const SimLayout &L, unsigned char *
   D.mem_busy = D.sum_arr = D.span_used = D.events = D.evals = D.started = D.ticks = D.row_first = 0;
   D.need_init = 1;
   s.sum_rows = 0; s.sum_fresh = true;
-  s.tl_fresh = true; s.tl_done = false; s.jd_done = false; s.sd_done = false;
+  s.tl_fresh = true; s.tl_done = false; s.jd_done = false; s.sd_done = false; s.arr_done = false;
   s.occ_fresh = true; s.occ_done = false;
   s.prepared = true;
   return GS_OK;
@@ -1153,6 +1157,7 @@ struct GsSumEngineJobs {
   __device__ long long n(int r) const { return sims[r].n; }
   __device__ int order(int r, long long i) const { return sims[r].fin[i]; }
   __device__ GsSumJob job(int r, long long i) const { return job_at(r, sims[r].fin[i]); }
+  __device__ int arrive_at(int r, int j) const { return sims[r].jobs[j].arrive; }
   // the gs_jobin records of job j in the traces of replicas ra and rb are byte-equal
   __device__ bool same_job(int ra, int rb, int j) const {
     const unsigned long long *x = reinterpret_cast<const unsigned long long *>(sims[ra].jobs + j);
@@ -1220,8 +1225,15 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   const int grid = std::min(count, std::max(1, per_sm) * sms);
   const size_t pitch = (size_t)align_up((size_t)kmax, 64);
-  const int Csd = h->sd.nclasses;
-  int rc = ensure_scratch(h, (Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid);   // gs_sd_jobs_kernel: a fourth row
+  const int Csd = h->sd.nclasses, Barr = h->arr.nbins;
+  int grid_arr = 0;
+  if (Barr > 0) {
+    int per_arr = 1;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_arr, gs_arr_jobs_kernel<GsSumEngineJobs>, GS_SUM_THREADS, 0));
+    grid_arr = std::min(grid, std::max(1, per_arr) * sms);
+  }
+  int rc = ensure_scratch(h, std::max((Csd > 0 ? 4 : 3) * sizeof(int) * pitch * (size_t)grid,    // gs_sd_jobs_kernel: a fourth row
+                                      GS_ARR_ROWS * sizeof(int) * pitch * (size_t)grid_arr));
   if (rc) return rc;
   const int B = h->tl_nbins;
   for (int i = first; i < first + count; ++i) {
@@ -1279,6 +1291,12 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
     CU(cudaGetLastError());
     h->launches += 1;
   }
+  if (Barr > 0) {         // after the other job kernels: its own GS_ARR_ROWS rows on the same scratch
+    gs_arr_jobs_kernel<GsSumEngineJobs><<<(unsigned)grid_arr, GS_SUM_THREADS, 0, h->stream>>>(src, first, count, h->arr, h->d_arr,
+                                                                                             (int *)h->d_scratch, (long long)pitch);
+    CU(cudaGetLastError());
+    h->launches += 1;
+  }
   CU(cudaEventRecord(h->e1, h->stream));
   CU(cudaMemcpyAsync(out, h->d_sum + first, sizeof(gs_summary) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
@@ -1289,6 +1307,7 @@ extern "C" int gs_summarize(gs_handle h, int first, int count, gs_summary *out, 
     if (B > 0) h->sims[(size_t)i].tl_done = true;
     if (C > 0) h->sims[(size_t)i].jd_done = true;
     if (Csd > 0) h->sims[(size_t)i].sd_done = true;
+    if (Barr > 0) h->sims[(size_t)i].arr_done = true;
     if (h->occ_on) h->sims[(size_t)i].occ_done = true;
   }
   return GS_OK;
@@ -1421,6 +1440,50 @@ extern "C" int gs_fetch_slowdown(gs_handle h, int first, int count, gs_sdclass *
     CU(cudaMemcpyAsync(out, h->d_sd + (size_t)first * C, sizeof(gs_sdclass) * C * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   if (hist_out)
     CU(cudaMemcpyAsync(hist_out, h->d_sd_hist + (size_t)first * per, sizeof(unsigned) * per * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+  CU(wait_stream(h));
+  return GS_OK;
+}
+
+extern "C" int gs_set_arrivals(gs_handle h, int64_t bin_width, int32_t nbins, int64_t tau) {
+  if (!h) return GS_ERR_ARG;
+  GsArrCfg cfg;
+  const char *why = nullptr;
+  if (!gs_arr_make_cfg(bin_width, nbins, tau, cfg, &why)) return fail(h, GS_ERR_ARG, std::string("gs_set_arrivals: ") + why);
+  CU(cudaSetDevice(h->device));
+  const size_t need = sizeof(gs_abin) * (size_t)h->nsims * (size_t)cfg.nbins;
+  if (need > h->arr_bytes) {
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    gs_abin *d = nullptr;
+    if (need > free_b || cudaMalloc(&d, need) != cudaSuccess) {
+      (void)cudaGetLastError();
+      return fail(h, GS_ERR_CAPACITY, "gs_set_arrivals: the bin records (" + std::to_string(need) + " bytes) do not fit the device's free memory");
+    }
+    if (h->d_arr) { CU(cudaStreamSynchronize(h->stream)); cudaFree(h->d_arr); }
+    h->d_arr = d; h->arr_bytes = need;
+  } else if (cfg.nbins == 0 && h->d_arr) {           // off: the records are not kept
+    CU(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_arr);
+    h->d_arr = nullptr; h->arr_bytes = 0;
+  }
+  h->arr = cfg;
+  for (SimHost &s : h->sims) s.arr_done = false;
+  return GS_OK;
+}
+
+extern "C" int gs_fetch_arrivals(gs_handle h, int first, int count, gs_abin *out) {
+  if (!h) return GS_ERR_ARG;
+  if (first < 0 || count < 0 || first + count > h->nsims || (count > 0 && !out)) return fail(h, GS_ERR_ARG, "gs_fetch_arrivals: bad arguments");
+  if (h->arr.nbins == 0) return fail(h, GS_ERR_STATE, "gs_fetch_arrivals: the arrival statistics are off (gs_set_arrivals)");
+  for (int i = first; i < first + count; ++i) {
+    const SimHost &s = h->sims[(size_t)i];
+    if (!s.prepared || !s.arr_done)
+      return fail(h, GS_ERR_STATE, "gs_fetch_arrivals: a replica has not been summarised with this setting since it was prepared");
+  }
+  if (count == 0) return GS_OK;
+  CU(cudaSetDevice(h->device));
+  const size_t B = (size_t)h->arr.nbins;
+  CU(cudaMemcpyAsync(out, h->d_arr + (size_t)first * B, sizeof(gs_abin) * B * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
   CU(wait_stream(h));
   return GS_OK;
 }

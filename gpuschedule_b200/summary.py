@@ -437,6 +437,76 @@ def slowdown_spread_flat(sp, c):
     return [float(sp[name][s][c]) for name in SLOWDOWN_METRICS for s in SPREAD_STATS]
 
 
+# ---------------------------------------------------------------- job statistics by arrival time
+ARRIVAL_COUNTS = ("arrived", "jobs", "unfinished", "sd_clamped")
+ARRIVAL_METRICS = SLOWDOWN_METRICS                        # key_mean: the mean arrival tick of the bin's finished jobs
+ARRIVAL_SPREAD_METRICS = ("arrived", "jobs", "unfinished") + ARRIVAL_METRICS
+
+
+def _i128(lo, hi):
+    v = u128(lo, hi)
+    return v - (1 << 128) if v >> 127 else v
+
+
+def arrivals_derived(recs):
+    """Per arrival bin of one replica: `recs` ABIN_DTYPE (B,).  Returns {"arrived", "jobs", "unfinished" (arrived -
+    jobs), "sd_clamped": int arrays (B,), metric: float array (B,) for every ARRIVAL_METRICS entry}, the numbers of
+    slowdown_derived over each bin's finished jobs, with key_mean the mean arrival tick; NaN for a bin without
+    finished jobs."""
+    recs = np.asarray(recs)
+    if recs.ndim != 1:
+        raise ValueError("arrivals_derived: expected recs (B,)")
+    s = recs["s"]
+    jobs = s["jc"]["jobs"].astype(np.int64)
+    arrived = recs["arrived"].astype(np.int64)
+    out = {"arrived": arrived, "jobs": jobs, "unfinished": arrived - jobs, "sd_clamped": s["sd_clamped"].astype(np.int64)}
+    nums = [_sdclass_numbers(rec) for rec in s]
+    for d, rec, n in zip(nums, s, jobs.tolist()):
+        d["key_mean"] = _i128(rec["key_sum_lo"], rec["key_sum_hi"]) / n if n else math.nan
+    for name in ARRIVAL_METRICS:
+        out[name] = np.array([d[name] for d in nums], dtype=np.float64)
+    return out
+
+
+def arrivals_spread(recs, level=0.95):
+    """Spread per bin across replicas: `recs` ABIN_DTYPE (replicas, B).  For every bin, over the replicas with at least
+    one finished job in it: {"replicas": int array (B,), metric: {mean, std, lo, hi: float arrays (B,)} for every
+    ARRIVAL_SPREAD_METRICS entry}, with spread's rules (sample std, nearest-rank interval holding the central `level`,
+    NaN where no replica has finished jobs in the bin)."""
+    level = Fraction(str(level))
+    if not 0 < level <= 1:
+        raise ValueError("level must be in (0, 1]")
+    recs = np.asarray(recs)
+    if recs.ndim != 2:
+        raise ValueError("arrivals_spread: expected recs (replicas, B)")
+    per = [arrivals_derived(recs[r]) for r in range(recs.shape[0])]
+    nb = recs.shape[1]
+    reach = recs["s"]["jc"]["jobs"] > 0
+    out = {"replicas": reach.sum(axis=0).astype(np.int64)}
+    for name in ARRIVAL_SPREAD_METRICS:
+        cols = [_spread_of(np.array([d[name][b] for r, d in enumerate(per) if reach[r, b]], dtype=np.float64), level) for b in range(nb)]
+        out[name] = {s: np.array([col[s] for col in cols], dtype=np.float64) for s in SPREAD_STATS}
+    return out
+
+
+def arrivals_columns():
+    """names of the flat per-bin columns `arrivals_flat` returns, in order"""
+    return list(ARRIVAL_COUNTS) + list(ARRIVAL_METRICS)
+
+
+def arrivals_flat(d, b):
+    """bin b of an arrivals_derived dict as a list of Python values"""
+    return [int(d[k][b]) for k in ARRIVAL_COUNTS] + [float(d[name][b]) for name in ARRIVAL_METRICS]
+
+
+def arrivals_spread_columns():
+    return [f"{name}_{s}" for name in ARRIVAL_SPREAD_METRICS for s in SPREAD_STATS]
+
+
+def arrivals_spread_flat(sp, b):
+    return [float(sp[name][s][b]) for name in ARRIVAL_SPREAD_METRICS for s in SPREAD_STATS]
+
+
 # ---------------------------------------------------------------- interference (utilisation-aware engine)
 IF_ONE = 1024                                             # fixed-point units per tick
 IF_COUNTS = ("jobs", "degraded", "preempted_jobs", "clamped")

@@ -232,6 +232,22 @@ def _sd_row(sd):
     return 3 * (len(sd[3]) + 1) + len(sd[4]) + 1
 
 
+def check_arrivals(arrivals):
+    """(bin width W, bins B, tau) of an arrivals argument, or ValueError: W >= 1 and int64, B in 1..1024, tau >= 1
+    and int64"""
+    try:
+        W, B, tau = (int(x) for x in arrivals)
+    except (TypeError, ValueError):
+        raise ValueError("arrivals: expected (bin width, bins, tau)") from None
+    if not 1 <= W < 2 ** 63:
+        raise ValueError("arrivals: the bin width must be >= 1 and int64")
+    if not 1 <= B <= capi.ARRIVALS_MAX_BINS:
+        raise ValueError(f"arrivals: the bin count must be in 1..{capi.ARRIVALS_MAX_BINS}")
+    if not 1 <= tau < 2 ** 63:
+        raise ValueError("arrivals: tau must be >= 1 and int64")
+    return W, B, tau
+
+
 DEFAULT_QUEUE_EDGES = (0,) + tuple(2 ** i for i in range(31))      # queue length 0, 1, 2, 4, ... 2^30
 
 
@@ -301,7 +317,7 @@ def _compare_in(eng, pairs, members, bounds, edges):
 
 
 def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, timeline=None, jobdist=None, compare=None, slowdown=None,
-                      occupancy=None, interference=None):
+                      occupancy=None, interference=None, arrivals=None):
     """One run summary (capi.SUMMARY_DTYPE) per configuration of `flag_sets`, in order, computed on the device: the
     same configurations and random streams as run_batched, but no row or job record is read back and nothing is
     written.  The utilisation-aware configurations go through the gs_horus retry loop of run_batched_horus.
@@ -320,7 +336,12 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
     (len(flag_sets), E + 1)) as the last element, P the largest M * G of the configurations plus 1.
     interference=class bounds: also compute the interference statistics of every utilisation-aware replica on the
     device (gs_horus_set_interference) and append IFCLASS_DTYPE records (len(flag_sets), C) as the last element (after
-    the occupancy element); the rows of the other configurations are zero."""
+    the occupancy element); the rows of the other configurations are zero.
+    arrivals=(W, B, tau): also compute every replica's job statistics by arrival time on the device (gs_set_arrivals)
+    and append ABIN_DTYPE records (len(flag_sets), B) as the last element."""
+    if arrivals is not None:
+        arr = check_arrivals(arrivals)
+        arr_recs = np.zeros((len(flag_sets), arr[1]), dtype=capi.ABIN_DTYPE)
     if interference is not None:
         if_bounds = check_interference(interference)
         if_recs = np.zeros((len(flag_sets), len(if_bounds) + 1), dtype=capi.IFCLASS_DTYPE)
@@ -363,7 +384,11 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 eng.set_occupancy(occ_edges)
             if interference is not None:
                 eng.set_interference(if_bounds)
+            if arrivals is not None:
+                eng.set_arrivals(*arr)
             out[aware] = eng.summarize()
+            if arrivals is not None:
+                arr_recs[aware] = eng.arrivals()
             if interference is not None:
                 if_recs[aware] = eng.interference()
             if occupancy is not None:
@@ -390,7 +415,11 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 eng.set_slowdown(*sd)
             if occupancy is not None:
                 eng.set_occupancy(occ_edges)
+            if arrivals is not None:
+                eng.set_arrivals(*arr)
             out[plain] = eng.run_summarized()
+            if arrivals is not None:
+                arr_recs[plain] = eng.arrivals()
             if occupancy is not None:
                 occ_recs[plain], ob, occ_q[plain] = eng.occupancy()
                 occ_busy[plain, :, :ob.shape[2]] = ob
@@ -405,7 +434,8 @@ def summarize_batched(flag_sets, device=0, chunk=1 << 21, rows_cap=1 << 16, time
                 cmp_recs[sel], cmp_hist[sel] = _compare_in(eng, [pairs[k] for k in sel], plain, cmp_bounds, cmp_edges)
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
            + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ())
-           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()) + ((if_recs,) if interference is not None else ()))
+           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()) + ((if_recs,) if interference is not None else ())
+           + ((arr_recs,) if arrivals is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -540,7 +570,7 @@ def _check_bootstrap_args(flag_sets, replicas, loads, n, block_len=1, mix=None, 
 
 
 def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, device=0, timeline=None, jobdist=None, block_len=1,
-                        compare=None, mix=None, slowdown=None, occupancy=None, profile=None):
+                        compare=None, mix=None, slowdown=None, occupancy=None, profile=None, arrivals=None):
     """Bootstrap spread of a sweep: every configuration of `flag_sets` runs `replicas` traces drawn on the device from
     its base trace file (gs_boot_traces: jobs and inter-arrival gaps resampled with Philox4x64-10 under key
     (seed, replica index)), at every offered load L of `loads` (the base trace's gaps scaled by 1/L), each replica
@@ -577,7 +607,10 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     picks are those of the unprofiled replica; only the arrivals move.  Every returned array gains a profile axis
     right after the mix axis (after the loads axis without mixes), and compare pairs (a, L[, mix], profile, r) with
     (b, L[, mix], profile, r).  A replica whose last arrival could reach 2^31 - 1 is a ValueError, raised after the
-    traces are read and before any engine is created."""
+    traces are read and before any engine is created.
+    arrivals=(W, B, tau): also append ABIN_DTYPE records (..., B) with the replicas' leading axes as the last element."""
+    if arrivals is not None:
+        arr = check_arrivals(arrivals)
     if occupancy is not None:
         occ_edges = check_occupancy(occupancy)
     _check_bootstrap_args(flag_sets, replicas, loads, n, block_len, mix, profile)
@@ -616,6 +649,8 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
     if slowdown is not None:
         sd_recs = np.zeros((len(flag_sets),) + lead + (sd_nc,), dtype=capi.SDCLASS_DTYPE)
         sd_hist = np.zeros((len(flag_sets),) + lead + (sd_nc, sd_row), dtype=np.uint32)
+    if arrivals is not None:
+        arr_recs = np.zeros((len(flag_sets),) + lead + (arr[1],), dtype=capi.ABIN_DTYPE)
     if compare is not None:
         cmp_nc, cmp_nb = len(cmp_bounds) + 1, len(cmp_edges) + 1
         cmp_recs = np.zeros((len(pairs),) + lead + (cmp_nc,), dtype=capi.JPAIR_DTYPE)
@@ -677,8 +712,11 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
                 eng.set_slowdown(*sd)
             if occupancy is not None:
                 eng.set_occupancy(occ_edges)
+            if arrivals is not None:
+                eng.set_arrivals(*arr)
             recs = eng.run_summarized()
             occ = eng.occupancy() if occupancy is not None else None
+            ar = eng.arrivals() if arrivals is not None else None
             tl = eng.timeline() if timeline is not None else None
             jd = eng.jobdist() if jobdist is not None else None
             sdr = eng.slowdown() if slowdown is not None else None
@@ -707,9 +745,11 @@ def summarize_bootstrap(flag_sets, replicas, loads=(1.0,), seed=0, n=None, devic
                 occ_recs[c] = occ[0][part].reshape(lead)
                 occ_busy[c][..., :ob.shape[2]] = ob.reshape(lead + (2, ob.shape[2]))
                 occ_q[c] = occ[2][part].reshape(lead + (len(occ_edges) + 1,))
+            if ar is not None:
+                arr_recs[c] = ar[part].reshape(lead + (arr[1],))
     res = ((out,) + ((bins,) if timeline is not None else ()) + (((jd_cls, jd_hist),) if jobdist is not None else ())
            + (((sd_recs, sd_hist),) if slowdown is not None else ()) + (((cmp_recs, cmp_hist),) if compare is not None else ())
-           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()))
+           + (((occ_recs, occ_busy, occ_q),) if occupancy is not None else ()) + ((arr_recs,) if arrivals is not None else ()))
     return res[0] if len(res) == 1 else res
 
 
@@ -807,6 +847,39 @@ def write_timeline_ci_csv(path, flag_sets, loads, bins, width, level=0.95, block
                 for b in range(tb.shape[1]):
                     w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [b]
                                + _bin_bounds(b, width, tb.shape[1]) + [int(sp["replicas"][b]), level] + summary.timeline_spread_flat(sp, b))
+
+
+def write_arrivals_csv(path, flag_sets, recs, arr):
+    """one line per (configuration, arrival bin): the flags, the bin, its arrival-tick range, tau and
+    summary.arrivals_derived's columns; arr = (W, B, tau)"""
+    import csv
+    W, _, tau = arr
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["bin", "bin_start", "bin_end", "tau"] + summary.arrivals_columns())
+        for fl, rc in zip(flag_sets, recs):
+            d = summary.arrivals_derived(rc)
+            for b in range(len(rc)):
+                w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed, b]
+                           + _bin_bounds(b, W, len(rc)) + [tau] + summary.arrivals_flat(d, b))
+
+
+def write_arrivals_ci_csv(path, flag_sets, loads, recs, arr, level=0.95, block_len=None, mix=None, profile=None):
+    """one line per (configuration, load[, block_len][, mix][, profile], arrival bin): the flags, the load columns, the
+    bin, its arrival-tick range, tau, the number of replicas with finished jobs in it and summary.arrivals_spread's
+    columns"""
+    import csv
+    W, _, tau = arr
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(SUMMARY_KEYS + ["load"] + _block_col(block_len) + _mix_col(mix, profile) + ["bin", "bin_start", "bin_end", "tau", "replicas", "level"]
+                   + summary.arrivals_spread_columns())
+        for fl, per_load in zip(flag_sets, recs):
+            for keys, rc in _load_lines(loads, block_len, mix, per_load, profile):
+                sp = summary.arrivals_spread(rc, level=level)
+                for b in range(rc.shape[1]):
+                    w.writerow([fl.trace_file, fl.scheme, fl.schedule, fl.num_buffer, fl.num_queue, fl.seed] + keys + [b]
+                               + _bin_bounds(b, W, rc.shape[1]) + [tau, int(sp["replicas"][b]), level] + summary.arrivals_spread_flat(sp, b))
 
 
 def _class_range(c, bounds):
@@ -1245,7 +1318,31 @@ def main(argv=None):
     ap.add_argument("--interference-ci", default=None, metavar="FILE",
                     help="with --interference and --repeats R >= 2: one CSV line per (configuration, class) with the spread of "
                          "the interference numbers over the R seeded repeats")
+    ap.add_argument("--arrivals", default=None, metavar="FILE",
+                    help="with --summary and --arrival-width: also compute job statistics by arrival time on the GPU -- wait, "
+                         "turnaround, jct and bounded slowdown of the jobs that arrived in each bin of --arrival-width ticks -- "
+                         "and write one CSV line per (configuration, bin) to FILE; with --bootstrap one line per (configuration, "
+                         "load, bin) with the spread across the replicas with finished jobs in the bin")
+    ap.add_argument("--arrival-width", type=int, default=None, metavar="W",
+                    help="with --arrivals: arrival ticks per bin (the ticks of --bin-width, so both may share W)")
+    ap.add_argument("--arrival-bins", type=int, default=None, metavar="B",
+                    help=f"with --arrivals: bins (1..{capi.ARRIVALS_MAX_BINS}, default 128); the last one is open-ended")
+    ap.add_argument("--arrival-bound", type=int, default=None, metavar="TAU",
+                    help="with --arrivals: bounded slowdown turnaround / max(jct, TAU), TAU >= 1 in ticks (default 1: plain slowdown)")
     a = ap.parse_args(argv)
+    arrivals = None
+    if a.arrivals is not None:
+        if not a.summary:
+            ap.error("--arrivals needs --summary FILE")
+        if a.arrival_width is None:
+            ap.error("--arrivals needs --arrival-width W")
+        try:
+            arrivals = check_arrivals((a.arrival_width, 128 if a.arrival_bins is None else a.arrival_bins,
+                                       1 if a.arrival_bound is None else a.arrival_bound))
+        except ValueError as e:
+            ap.error(str(e))
+    elif a.arrival_width is not None or a.arrival_bins is not None or a.arrival_bound is not None:
+        ap.error("--arrival-width, --arrival-bins and --arrival-bound need --arrivals FILE")
     interference = None
     if a.interference is not None:
         if not a.summary:
@@ -1377,9 +1474,13 @@ def main(argv=None):
         bl = a.block_len
         res = summarize_bootstrap(sets, a.bootstrap, loads, seed=max(a.seed, 0), n=a.jobs, timeline=timeline, jobdist=jobdist,
                                   block_len=1 if bl is None else bl, compare=compare, mix=mix, slowdown=slowdown, occupancy=occupancy,
-                                  profile=profile)
+                                  profile=profile, arrivals=arrivals)
         recs, rest = (res, ()) if (timeline is None and jobdist is None and compare is None and slowdown is None
-                                   and occupancy is None) else (res[0], res[1:])
+                                   and occupancy is None and arrivals is None) else (res[0], res[1:])
+        if arrivals is not None:
+            arec = rest[-1]
+            rest = rest[:-1]
+            write_arrivals_ci_csv(a.arrivals, sets, loads, arec, arrivals, block_len=bl, mix=mix_text, profile=profile_text)
         if occupancy is not None:
             orec, obusy, oq = rest[-1]
             rest = rest[:-1]
@@ -1418,9 +1519,13 @@ def main(argv=None):
         return
     if a.summary:
         res = summarize_batched(sets, timeline=timeline, jobdist=jobdist, compare=compare, slowdown=slowdown, occupancy=occupancy,
-                                interference=interference)
+                                interference=interference, arrivals=arrivals)
         recs, rest = (res, ()) if (timeline is None and jobdist is None and compare is None and slowdown is None
-                                   and occupancy is None and interference is None) else (res[0], res[1:])
+                                   and occupancy is None and interference is None and arrivals is None) else (res[0], res[1:])
+        if arrivals is not None:
+            arec = rest[-1]
+            rest = rest[:-1]
+            write_arrivals_csv(a.arrivals, sets, arec, arrivals)
         if interference is not None:
             irec = rest[-1]
             rest = rest[:-1]

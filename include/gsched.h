@@ -508,6 +508,33 @@ typedef struct gs_slowdown_cfg {
 int gs_set_slowdown(gs_handle h, const gs_slowdown_cfg *cfg);
 int gs_fetch_slowdown(gs_handle h, int first, int count, gs_sdclass *out, uint32_t *hist_out);
 
+/* ---- job statistics by arrival time (arrivals) -------------------------------------------------------------------
+ * The jobs are slowdown's, binned by arrival tick instead of a class key.  A setting is a bin width W >= 1 (ticks),
+ * B bins (1 <= B <= GS_ARRIVALS_MAX_BINS) and a slowdown bound tau >= 1.  A job that arrives at tick a falls in bin
+ * min(floor(a / W), B - 1), a negative a in bin 0: the last bin is open-ended.  The ticks are the timeline's `delta`
+ * ticks, so a timeline and the arrival bins may share W.  Per (replica, bin) one gs_abin: `s` is slowdown's gs_sdclass
+ * field for field, restricted to the bin's finished jobs, with the arrival tick as the key (key_sum is the exact sum
+ * of their arrival ticks), and `arrived` counts the bin's jobs of the replica's trace, finished or not: arrived -
+ * s.jc.jobs of them had not finished (a run of several windows, a job wider than the cluster).  There are no CDF
+ * histograms.  Every field is an integer; a repeated call gives the same bytes.                                  */
+#define GS_ARRIVALS_MAX_BINS 1024
+typedef struct gs_abin {
+  gs_sdclass s;                      /* slowdown's record of the bin's finished jobs, key = arrival tick              */
+  int64_t arrived;                   /* jobs of the replica's trace in this bin, finished or not                      */
+} gs_abin;                           /* 240 bytes */
+/* gs_set_arrivals: while nbins > 0, every gs_summarize also computes the bin records of the replicas it summarises
+ * (the job part is recomputed in full on every call, so this may be called at any time); nbins = 0 (the default)
+ * turns it off, and bin_width and tau are then ignored.  Every replica is marked as not summarised with this setting.
+ * Jobdist, slowdown and arrivals may all be on; each keeps its own arrays and state.  The records take nsims * B * 240
+ * bytes of device memory, allocated only while the feature is on.  GS_ERR_ARG for nbins outside 0..1024, or, when
+ * nbins > 0, bin_width < 1 or tau < 1; GS_ERR_CAPACITY when the records do not fit the device's free memory; nothing
+ * changes on an error.
+ * gs_fetch_arrivals copies count * B records (replica-major) as of the last gs_summarize (synchronous).  GS_ERR_ARG
+ * for a bad range, GS_ERR_STATE when the feature is off or a replica has not been summarised since it was prepared
+ * (first gs_run, gs_reset, a new trace, gs_boot_traces) or since the last gs_set_arrivals.                     */
+int gs_set_arrivals(gs_handle h, int64_t bin_width, int32_t nbins, int64_t tau);
+int gs_fetch_arrivals(gs_handle h, int first, int count, gs_abin *out);
+
 /* ---- time-weighted occupancy (occupancy) -----------------------------------------------------------------------
  * The rows of gs_summary's row part, each weighed by the ticks it stands for.  busy = busy_gpus as the row holds it
  * (horus: devices with at least one task), G = M * G of the replica's cluster (at most 65535).

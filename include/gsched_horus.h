@@ -112,6 +112,10 @@ int gs_horus_fetch_jobdist(gs_horus_handle h, int32_t first, int32_t count, gs_j
  * gs_horus_summarize from the same finished jobs.  Same meaning and errors as gs_set_slowdown / gs_fetch_slowdown. */
 int gs_horus_set_slowdown(gs_horus_handle h, const gs_slowdown_cfg *cfg);
 int gs_horus_fetch_slowdown(gs_horus_handle h, int32_t first, int32_t count, gs_sdclass *out, uint32_t *hist_out);
+/* Job statistics by arrival time (gs_abin, gsched.h) filled by gs_horus_summarize from the same finished jobs and the
+ * replica's loaded trace.  Same meaning and errors as gs_set_arrivals / gs_fetch_arrivals.                      */
+int gs_horus_set_arrivals(gs_horus_handle h, int64_t bin_width, int32_t nbins, int64_t tau);
+int gs_horus_fetch_arrivals(gs_horus_handle h, int32_t first, int32_t count, gs_abin *out);
 /* Time-weighted occupancy (gs_occ and histograms, gsched.h) filled by gs_horus_summarize from the same rows [0, ticks),
  * every row one tick.  gs_horus_summarize folds every row again on every call, so no carry is kept and the feature may
  * be set at any time; setting it marks every replica as not summarised.  Otherwise the same meaning and errors as
